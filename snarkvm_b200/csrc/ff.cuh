@@ -10,7 +10,8 @@
 // Multiplication is a word-serial interleaved Montgomery product built from
 // two carry chains per row ("even" columns and "odd" columns) so that every
 // 32x32->64 product lands in an aligned register pair and ptxas can fuse the
-// mad.lo.cc / madc.hi.cc pairs into IMAD.WIDE.U32(.X) on the fma pipe.
+// mad.lo.cc / madc.hi.cc pairs into IMAD.WIDE.U32(.X) on the fma pipe
+// (see ptx_neg for what keeps the reduction rows fused).
 // No tensor cores: this is integer modular arithmetic (BASELINE.json north_star).
 #pragma once
 #include <cstdint>
@@ -36,6 +37,12 @@ FF_DEV uint32_t ptx_mad_lo_cc(uint32_t a, uint32_t b, uint32_t c) { uint32_t r; 
 FF_DEV uint32_t ptx_madc_lo_cc(uint32_t a, uint32_t b, uint32_t c) { uint32_t r; asm volatile("madc.lo.cc.u32 %0, %1, %2, %3;" : "=r"(r) : "r"(a), "r"(b), "r"(c)); return r; }
 FF_DEV uint32_t ptx_madc_hi_cc(uint32_t a, uint32_t b, uint32_t c) { uint32_t r; asm volatile("madc.hi.cc.u32 %0, %1, %2, %3;" : "=r"(r) : "r"(a), "r"(b), "r"(c)); return r; }
 FF_DEV uint32_t ptx_madc_hi(uint32_t a, uint32_t b, uint32_t c) { uint32_t r; asm volatile("madc.hi.u32 %0, %1, %2, %3;" : "=r"(r) : "r"(a), "r"(b), "r"(c)); return r; }
+
+// The Montgomery multiplier m = x·INV32 = −x mod 2^32 of a reduction row (INV32 = −1 for both moduli, asserted where it is
+// used).  Written as `sub.u32 m, 0, x` on purpose: from the compiler's own `x * INV32` NVVM emits `neg.s32`, and ptxas
+// folds that negation into the m·p products, issuing each as IMAD.X + IMAD.HI.U32.X (two fmaheavy instructions and a
+// carry chain twice as long) instead of one IMAD.WIDE.U32.X.  tests/test_sass_mix.py checks the instruction mix.
+FF_DEV uint32_t ptx_neg(uint32_t x) { uint32_t r; asm volatile("sub.u32 %0, 0, %1;" : "=r"(r) : "r"(x)); return r; }
 
 // ---------------------------------------------------------------------------
 // Row helpers.  A running value V is held as two N-limb arrays:
@@ -86,7 +93,8 @@ FF_DEV void mont_step(uint32_t (&ev)[N], uint32_t (&od)[N], const uint32_t (&a)[
         od[N - 1] = ptx_addc(od[N - 1], 0u);
     }
     // Montgomery reduction row: m = -ev[0] / p mod 2^32
-    uint32_t m = ev[0] * P::INV32;
+    static_assert(P::INV32 == 0xffffffffu, "m = ev[0]·INV32 is computed as −ev[0]");
+    const uint32_t m = ptx_neg(ev[0]);
     uint32_t pm[N];
 #pragma unroll
     for (int k = 0; k < N; k++) pm[k] = P::mod(k);
@@ -276,7 +284,8 @@ struct Fp {
         for (int k = 0; k < N; k++) pm[k] = P::mod(k);
 #pragma unroll
         for (int i = 0; i < N; i++) {
-            const uint32_t m = ev[0] * P::INV32;
+            static_assert(P::INV32 == 0xffffffffu, "m = ev[0]·INV32 is computed as −ev[0]");
+            const uint32_t m = ptx_neg(ev[0]);
             row_mad<N>(od, &pm[1], m);
             if (P::MOD0_IS_ONE) {
                 ev[0] = ptx_add_cc(ev[0], m);
