@@ -165,14 +165,21 @@ def test_window_sums_and_host_finish(oracle_cpu):
     assert (device.msm_finish(tot.cpu().numpy(), planh["c"]) == want).all()
 
 
-@pytest.mark.parametrize("lg", [20, 22, 24])
+# default plans (c, pair levels) of the sizes below: 2^19, 2^21 and 2^23 are the only sizes that run c = 13, and c = 16 / 17
+# with 4 / 5 levels, on the plain path
+DEFAULT_PLANS = {19: (13, 2), 20: (15, 3), 21: (16, 4), 22: (16, 4), 23: (17, 5), 24: (17, 5)}
+
+
+@pytest.mark.parametrize("lg", [19, 20, 21, 22, 23, 24])
 def test_msm_full_size_properties(oracle_cpu, lg):
     """BASELINE config 2 sizes through size-independent properties: (1) bases are known multiples k_i·G, so
     Σ s_i·P_i = (Σ s_i·k_i mod r)·G — one scalar multiplication by the oracle; (2) linearity in the scalars;
-    (3) at 2^20 also the full oracle MSM."""
+    (3) up to 2^20 also the full oracle MSM."""
     from snarkvm_b200 import device
     n = 1 << lg
     seed = 1000 + lg
+    p = device.msm_plan(n)
+    assert (p["c"], p["levels"]) == DEFAULT_PLANS[lg]
     bases = device.generate_bases(n, seed)
     scal = random_canonical_fr(n, seed=lg)
     got = device.msm(bases, _dev(scal))
@@ -194,6 +201,41 @@ def test_msm_full_size_properties(oracle_cpu, lg):
         st[i0:i0 + (1 << 18)] = _add_mod_r(a, b)
     lhs = oracle_cpu.g1_add(got, device.msm(bases, _dev(t)))
     assert (lhs == device.msm(bases, _dev(st))).all()
+
+
+@pytest.mark.parametrize("lg", [19, 21, 23])
+def test_msm_full_size_adversarial(oracle_cpu, lg):
+    """The default plans of 2^19, 2^21 and 2^23 points on a hostile input, by the closed form: a run of one repeated
+    (point, scalar), points next to their negations with equal scalars, ∞ rows, and half of all scalars equal (a hot bucket in
+    every window over a full background, through every pair level and the hot-bucket folds)."""
+    import torch
+    import msm_corpus as mc
+    from snarkvm_b200 import device
+    n = 1 << lg
+    seed = 3000 + lg
+    bases = device.generate_bases(n, seed)
+    ks = np.zeros((n, 4), dtype=np.uint64)
+    ks[:, 0] = generated_base_multipliers(seed, n)
+    idx = np.arange(n // 3, n // 3 + 6000)                           # edited rows: a small slice, so the host copy stays small
+    b = mc.Bases(bases[idx[0]:idx[-1] + 1].cpu().numpy(), ks[idx].copy())
+    b.repeat(0, np.arange(1, 2000))
+    b.alternate(2000, np.arange(2000, 2200))
+    pairs = np.arange(2200, 4000, 2)                                   # P_i, −P_i with equal scalars
+    b.rows[pairs + 1] = b.rows[pairs]
+    b.ks[pairs + 1] = b.ks[pairs]
+    b.negate(pairs + 1)
+    b.infinity(np.arange(4000, 4100))
+    bases[idx[0]:idx[-1] + 1] = torch.from_numpy(b.rows).cuda()
+    ks[idx] = b.ks
+    scal = random_canonical_fr(n, seed=lg + 11)
+    rng = np.random.default_rng(lg)
+    scal[rng.permutation(n)[: n // 2]] = scal[0]
+    scal[idx[:2000]] = scal[idx[0]]
+    scal[idx[2000:2200]] = scal[idx[2000]]
+    scal[idx[pairs + 1]] = scal[idx[pairs]]
+    b.ks = ks
+    got = device.msm(bases, _dev(scal))
+    assert (got == mc.closed_form(oracle_cpu, b, scal)).all()
 
 
 def _add_mod_r(a, b):
