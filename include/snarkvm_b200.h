@@ -202,6 +202,23 @@ SNARKVM_API int snarkvm_b200_fr_vec_op_device(void* d_out, const void* d_a, cons
 SNARKVM_API int snarkvm_b200_fr_vec_scalar_op_device(void* d_out, const void* d_a, const void* scalar_mont_host, size_t n, int op, void* stream);
 /* EvaluationDomain::elements (fft/domain.rs:307-309): d_out[i] = group_gen^i, i < 2^lg, Montgomery. */
 SNARKVM_API int snarkvm_b200_domain_elements_device(void* d_out, uint32_t lg, void* stream);
+/* Varuna's matrix_evals (snark/varuna/ahp/matrices.rs:138-195, called by index_helper, ahp/indexer/indexer.rs:186-203) for one CSR
+ * matrix in HBM: row_ptr = nrows + 1 u32, cols = nnz u32 variable indices (public first), vals = nnz Montgomery Fr.  Entry e gets
+ * row = w_R^(its row), col = w_C^(reindex_by_subdomain(col), fft/domain.rs:322-344) and row_col_val = val * row * col; entries
+ * nnz .. 2^lg_non_zero - 1 get (1, 1, 0).  d_row, d_col, d_row_col_val receive 2^lg_non_zero Montgomery Fr each.  input_size is the
+ * (power-of-two) input domain; 2^lg_variable <= input_size (where reindex_by_subdomain errors), nrows > 2^lg_constraint,
+ * nnz > 2^lg_non_zero or nvars > 2^lg_variable return cudaErrorInvalidValue before any launch; a column >= nvars returns
+ * cudaErrorInvalidValue after the pass.  Synchronises the stream. */
+SNARKVM_API int snarkvm_b200_varuna_matrix_evals_device(void* d_row, void* d_col, void* d_row_col_val, const void* d_row_ptr, size_t nrows,
+                                                        const void* d_cols, const void* d_vals, size_t nnz, size_t nvars, size_t input_size,
+                                                        uint32_t lg_constraint, uint32_t lg_variable, uint32_t lg_non_zero, void* stream);
+/* Varuna's transpose (snark/varuna/ahp/matrices.rs:249-270) of the same CSR matrix over the variable domain: transposed row
+ * reindex_by_subdomain(col) holds (val, row) for every entry of that column.  d_t_row_ptr receives 2^lg_variable + 1 u32, d_t_cols nnz
+ * u32 row indices, d_t_vals nnz Montgomery Fr; the order of the entries inside a transposed row is unspecified (equal to the
+ * reference's as a matrix).  Same argument checks and errors as snarkvm_b200_varuna_matrix_evals_device.  Synchronises the stream. */
+SNARKVM_API int snarkvm_b200_csr_transpose_device(void* d_t_row_ptr, void* d_t_cols, void* d_t_vals, const void* d_row_ptr, size_t nrows,
+                                                  const void* d_cols, const void* d_vals, size_t nnz, size_t nvars, size_t input_size,
+                                                  uint32_t lg_variable, void* stream);
 /* DensePolynomial::evaluate (fft/polynomial/dense.rs:98-114): out = sum c_i * point^i; out and point are 32-byte HOST buffers. */
 SNARKVM_API int snarkvm_b200_poly_evaluate_device(void* out_mont_host, const void* d_coeffs, size_t m, const void* point_mont_host,
                                                   void* stream);

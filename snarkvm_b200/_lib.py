@@ -32,6 +32,7 @@ SYMBOLS = (
     "snarkvm_b200_kzg_commit_batch_precomputed_device", "snarkvm_b200_msm_scratch_stats", "snarkvm_b200_msm_set_scratch_limit", "snarkvm_b200_msm_window_sums_host", "snarkvm_b200_selftest_coop", "snarkvm_b200_msm_plan_levels", "snarkvm_b200_msm_g2", "snarkvm_b200_msm_g2_device", "snarkvm_b200_generate_bases_g2_device",
     "snarkvm_b200_sonic_commit_batch_device", "snarkvm_b200_generator_mul_device", "snarkvm_b200_selftest_host_copy",
     "snarkvm_b200_test_field_op_device", "snarkvm_b200_test_curve_op_device", "snarkvm_b200_test_field_op_host",
+    "snarkvm_b200_varuna_matrix_evals_device", "snarkvm_b200_csr_transpose_device",
 )
 
 
@@ -110,6 +111,8 @@ def lib():
     L.snarkvm_b200_fr_vec_op_device.argtypes = [vp, vp, vp, sz, i32, vp]
     L.snarkvm_b200_fr_vec_scalar_op_device.argtypes = [vp, vp, vp, sz, i32, vp]
     L.snarkvm_b200_domain_elements_device.argtypes = [vp, u32, vp]
+    L.snarkvm_b200_varuna_matrix_evals_device.argtypes = [vp, vp, vp, vp, sz, vp, vp, sz, sz, sz, u32, u32, u32, vp]
+    L.snarkvm_b200_csr_transpose_device.argtypes = [vp, vp, vp, vp, sz, vp, vp, sz, sz, sz, u32, vp]
     L.snarkvm_b200_msm_batch_device.argtypes = [vp, vp, sz, vp, vp, sz, vp]
     L.snarkvm_b200_msm_window_sums_plan_device.argtypes = [vp, vp, sz, vp, sz, vp, sz, vp]
     L.snarkvm_b200_kzg_commit_batch_hiding_device.argtypes = [vp, vp, sz, vp, vp, vp, vp, vp, sz, vp]

@@ -1152,6 +1152,18 @@ int snarkvm_b200_fr_vec_scalar_op_device(void* d_out, const void* d_a, const voi
 int snarkvm_b200_domain_elements_device(void* d_out, uint32_t lg, void* stream) {
     return domain_elements_device(d_out, lg, (cudaStream_t)stream);
 }
+int snarkvm_b200_varuna_matrix_evals_device(void* d_row, void* d_col, void* d_row_col_val, const void* d_row_ptr, size_t nrows,
+                                            const void* d_cols, const void* d_vals, size_t nnz, size_t nvars, size_t input_size,
+                                            uint32_t lg_constraint, uint32_t lg_variable, uint32_t lg_non_zero, void* stream) {
+    return varuna_matrix_evals_device(d_row, d_col, d_row_col_val, d_row_ptr, nrows, d_cols, d_vals, nnz, nvars, input_size, lg_constraint,
+                                      lg_variable, lg_non_zero, (cudaStream_t)stream);
+}
+int snarkvm_b200_csr_transpose_device(void* d_t_row_ptr, void* d_t_cols, void* d_t_vals, const void* d_row_ptr, size_t nrows,
+                                      const void* d_cols, const void* d_vals, size_t nnz, size_t nvars, size_t input_size,
+                                      uint32_t lg_variable, void* stream) {
+    return csr_transpose_device(d_t_row_ptr, d_t_cols, d_t_vals, d_row_ptr, nrows, d_cols, d_vals, nnz, nvars, input_size, lg_variable,
+                                (cudaStream_t)stream);
+}
 int snarkvm_b200_poly_evaluate_device(void* out_mont_host, const void* d_coeffs, size_t m, const void* point_mont_host, void* stream) {
     return poly_evaluate_device(out_mont_host, d_coeffs, m, point_mont_host, (cudaStream_t)stream);
 }

@@ -413,14 +413,17 @@ __global__ void k_fr_vec_scalar_op(uint32_t* out, const uint32_t* a, FrArg s_arg
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) fr_apply(op, Fr::load(a + i * 8), fr_from_arg(s_arg)).store(out + i * 8);
 }
-// out[i] = ω_n^i from the NTT's table ω_N^j (j < N/2): ω_n^i = ω_N^{i·N/n}, and ω^{i} = −ω^{i − n/2} in the upper half
+// ω_n^i (i < n = 2^lg) from the NTT's table ω_N^j (j < N/2): ω_n^i = ω_N^{i·N/n}, and ω^{i} = −ω^{i − n/2} in the upper half
+FF_DEV Fr domain_element(size_t i, int lg, const uint32_t* __restrict__ tw, int lgN) {
+    if (lg == 0) return Fr::one();
+    const size_t half = (size_t)1 << (lg - 1), j = i < half ? i : i - half;
+    const Fr w = Fr::load_ldg(tw + (j << (lgN - lg)) * 8);
+    return i < half ? w : w.neg();
+}
 __global__ void k_domain_elements(uint32_t* __restrict__ out, int lg, const uint32_t* __restrict__ tw, int lgN) {
-    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x, n = (size_t)1 << lg, half = n >> 1;
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x, n = (size_t)1 << lg;
     if (i >= n) return;
-    if (lg == 0) { Fr::one().store(out); return; }
-    const size_t j = i < half ? i : i - half;
-    Fr w = Fr::load_ldg(tw + (j << (lgN - lg)) * 8);
-    (i < half ? w : w.neg()).store(out + i * 8);
+    domain_element(i, lg, tw, lgN).store(out + i * 8);
 }
 
 int fr_vec_op_device(void* d_out, const void* d_a, const void* d_b, size_t n, int op, cudaStream_t stream) {
@@ -448,6 +451,214 @@ int domain_elements_device(void* d_out, uint32_t lg, cudaStream_t stream) {
     k_domain_elements<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>((uint32_t*)d_out, (int)lg, (const uint32_t*)tw, lgN);
     count_launch();
     return (int)cudaGetLastError();
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// The Varuna indexer over a CSR matrix (row_ptr u32 [nrows + 1], cols u32 [nnz], vals Montgomery Fr [nnz]):
+//   matrix_evals (snark/varuna/ahp/matrices.rs:138-195) — entry e gets row = ω_R^{row(e)}, col = ω_C^{reindex(col(e))} and
+//     row_col_val = val·row·col; entries nnz … |K| − 1 get the padding (1, 1, 0);
+//   transpose (matrices.rs:249-270) over the variable domain — a counting sort: histogram of the reindexed columns, exclusive
+//     scan, scatter.  Entries land in a transposed row in atomic order; the sums sparse_matvec takes over them are exact.
+// row(e) is the last row whose first entry is ≤ e (a binary search of row_ptr, so empty rows are skipped); reindex is
+// EvaluationDomain::reindex_by_subdomain (fft/domain.rs:322-344) of the variable domain C by the input domain I, |C| > |I|.
+// A column ≥ nvars, or a row_ptr that does not run from 0 to nnz, raises the bad flag; such an entry is never indexed by.
+// ---------------------------------------------------------------------------------------------------------------------
+struct CsrArgs {
+    const uint32_t* row_ptr; const uint32_t* cols; const uint32_t* vals;
+    uint32_t nrows, nnz, nvars, input_size, period;    // period = |C| / |I| ≥ 2
+};
+FF_DEV uint32_t csr_row_of(const uint32_t* __restrict__ row_ptr, uint32_t nrows, uint32_t e) {
+    uint32_t lo = 0, hi = nrows;                        // row_ptr[lo] ≤ e < row_ptr[hi]; lo < nrows always
+    while (hi - lo > 1) {
+        const uint32_t mid = lo + (hi - lo) / 2;
+        if (__ldg(row_ptr + mid) <= e) lo = mid; else hi = mid;
+    }
+    return lo;
+}
+FF_DEV uint32_t reindex_by_subdomain(uint32_t index, uint32_t input_size, uint32_t period) {
+    if (index < input_size) return index * period;
+    const uint32_t i = index - input_size;
+    return i + i / (period - 1) + 1;
+}
+FF_DEV void csr_check_bounds(const CsrArgs& m, int* bad) {
+    if (blockIdx.x == 0 && threadIdx.x == 0 && (m.row_ptr[0] != 0 || m.row_ptr[m.nrows] != m.nnz)) *bad = 1;
+}
+
+__global__ void k_matrix_evals(CsrArgs m, uint64_t K, const uint32_t* __restrict__ tw, int lgN, int lgR, int lgC,
+                               uint32_t* __restrict__ row_out, uint32_t* __restrict__ col_out, uint32_t* __restrict__ rcv_out,
+                               int* __restrict__ bad) {
+    const size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    csr_check_bounds(m, bad);
+    if (e >= K) return;
+    if (e >= m.nnz) {                                                       // padding (matrices.rs:174-181)
+        Fr::one().store(row_out + e * 8); Fr::one().store(col_out + e * 8); Fr::zero().store(rcv_out + e * 8);
+        return;
+    }
+    const uint32_t c = __ldg(m.cols + e);
+    if (c >= m.nvars) {
+        *bad = 1;
+        Fr::zero().store(row_out + e * 8); Fr::zero().store(col_out + e * 8); Fr::zero().store(rcv_out + e * 8);
+        return;
+    }
+    const Fr r = domain_element(csr_row_of(m.row_ptr, m.nrows, (uint32_t)e), lgR, tw, lgN);
+    const Fr cc = domain_element(reindex_by_subdomain(c, m.input_size, m.period), lgC, tw, lgN);
+    r.store(row_out + e * 8);
+    cc.store(col_out + e * 8);
+    (Fr::load_ldg(m.vals + e * 8) * (r * cc)).store(rcv_out + e * 8);
+}
+
+__global__ void k_csr_col_histogram(CsrArgs m, uint32_t* __restrict__ counts, int* __restrict__ bad) {
+    const size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    csr_check_bounds(m, bad);
+    if (e >= m.nnz) return;
+    const uint32_t c = __ldg(m.cols + e);
+    if (c >= m.nvars) { *bad = 1; return; }
+    atomicAdd(counts + reindex_by_subdomain(c, m.input_size, m.period), 1u);
+}
+
+// exclusive scan of n u32 counts into out[0 … n] (out[n] = total): SCAN_TILE per CTA, then one CTA scans the tile sums,
+// then every tile adds its offset
+static constexpr int SCAN_THREADS = 256, SCAN_PER = 4, SCAN_TILE = SCAN_THREADS * SCAN_PER;
+FF_DEV uint32_t cta_exclusive_scan(uint32_t v, uint32_t* sh, uint32_t* total) {
+    const uint32_t t = threadIdx.x;
+    sh[t] = v;
+    __syncthreads();
+    for (uint32_t d = 1; d < SCAN_THREADS; d <<= 1) {                      // Hillis–Steele inclusive scan
+        const uint32_t add = t >= d ? sh[t - d] : 0;
+        __syncthreads();
+        sh[t] += add;
+        __syncthreads();
+    }
+    const uint32_t incl = sh[t];
+    *total = sh[SCAN_THREADS - 1];
+    __syncthreads();
+    return incl - v;
+}
+__global__ void __launch_bounds__(SCAN_THREADS) k_scan_tiles(const uint32_t* __restrict__ in, size_t n, uint32_t* __restrict__ out,
+                                                             uint32_t* __restrict__ tile_sums) {
+    __shared__ uint32_t sh[SCAN_THREADS];
+    const size_t base = (size_t)blockIdx.x * SCAN_TILE + (size_t)threadIdx.x * SCAN_PER;
+    uint32_t v[SCAN_PER], run = 0;
+#pragma unroll
+    for (int k = 0; k < SCAN_PER; k++) { v[k] = base + k < n ? in[base + k] : 0; run += v[k]; }
+    uint32_t total;
+    uint32_t pre = cta_exclusive_scan(run, sh, &total);
+#pragma unroll
+    for (int k = 0; k < SCAN_PER; k++) { if (base + k < n) out[base + k] = pre; pre += v[k]; }
+    if (threadIdx.x == 0) tile_sums[blockIdx.x] = total;
+}
+__global__ void __launch_bounds__(SCAN_THREADS) k_scan_tile_sums(uint32_t* __restrict__ tile_sums, size_t ntiles, uint32_t* __restrict__ out_total) {
+    __shared__ uint32_t sh[SCAN_THREADS];
+    uint32_t carry = 0;
+    for (size_t b = 0; b < ntiles; b += SCAN_THREADS) {                     // in place, exclusive
+        const size_t i = b + threadIdx.x;
+        const uint32_t v = i < ntiles ? tile_sums[i] : 0;
+        uint32_t total;
+        const uint32_t pre = cta_exclusive_scan(v, sh, &total);
+        if (i < ntiles) tile_sums[i] = carry + pre;
+        carry += total;
+    }
+    if (threadIdx.x == 0) *out_total = carry;
+}
+__global__ void k_scan_add(uint32_t* __restrict__ out, size_t n, const uint32_t* __restrict__ tile_sums) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) out[i] += tile_sums[i / SCAN_TILE];
+}
+
+// cursor[t] starts at the transposed row's first slot; every valid entry takes the next one
+__global__ void k_csr_transpose_scatter(CsrArgs m, uint32_t* __restrict__ cursor, uint32_t* __restrict__ t_cols,
+                                        uint32_t* __restrict__ t_vals) {
+    const size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= m.nnz) return;
+    const uint32_t c = __ldg(m.cols + e);
+    if (c >= m.nvars) return;
+    const uint32_t slot = atomicAdd(cursor + reindex_by_subdomain(c, m.input_size, m.period), 1u);   // < its row's end ≤ nnz
+    t_cols[slot] = csr_row_of(m.row_ptr, m.nrows, (uint32_t)e);
+    const uint4* src = reinterpret_cast<const uint4*>(m.vals + e * 8);
+    uint4* dst = reinterpret_cast<uint4*>(t_vals + (size_t)slot * 8);
+    dst[0] = __ldg(src); dst[1] = __ldg(src + 1);
+}
+
+// the shared validation of both entry points: everything the kernels index by must fit in u32 and in its domain
+static int csr_index_args(CsrArgs* m, const void* d_row_ptr, size_t nrows, const void* d_cols, const void* d_vals, size_t nnz,
+                          size_t nvars, size_t input_size, uint32_t lg_variable) {
+    if (!d_row_ptr || (nnz && (!d_cols || !d_vals)) || lg_variable > 31) return (int)cudaErrorInvalidValue;
+    const size_t V = (size_t)1 << lg_variable;
+    if (input_size == 0 || (input_size & (input_size - 1)) || V <= input_size) return (int)cudaErrorInvalidValue;   // domain.rs:327-329
+    if (nvars > V || nrows >= ((size_t)1 << 32) || nnz >= ((size_t)1 << 32)) return (int)cudaErrorInvalidValue;
+    *m = CsrArgs{(const uint32_t*)d_row_ptr, (const uint32_t*)d_cols, (const uint32_t*)d_vals, (uint32_t)nrows, (uint32_t)nnz,
+                 (uint32_t)nvars, (uint32_t)input_size, (uint32_t)(V / input_size)};
+    return 0;
+}
+// reads the bad flag back (synchronising the stream) and frees the scratch
+static int csr_finish(int rc, uint8_t* scratch, const int* bad, cudaStream_t stream) {
+    int h_bad = 0;
+    if (rc == 0) rc = (int)cudaMemcpyAsync(&h_bad, bad, sizeof(int), cudaMemcpyDeviceToHost, stream);
+    cudaFreeAsync(scratch, stream);
+    if (rc == 0) rc = (int)cudaStreamSynchronize(stream);
+    if (rc == 0 && h_bad) rc = (int)cudaErrorInvalidValue;
+    return rc;
+}
+
+int varuna_matrix_evals_device(void* d_row, void* d_col, void* d_row_col_val, const void* d_row_ptr, size_t nrows, const void* d_cols,
+                               const void* d_vals, size_t nnz, size_t nvars, size_t input_size, uint32_t lg_constraint,
+                               uint32_t lg_variable, uint32_t lg_non_zero, cudaStream_t stream) {
+    CsrArgs m;
+    int rc = csr_index_args(&m, d_row_ptr, nrows, d_cols, d_vals, nnz, nvars, input_size, lg_variable);
+    if (rc != 0) return rc;
+    if (!d_row || !d_col || !d_row_col_val || lg_constraint > 31 || lg_non_zero > 31) return (int)cudaErrorInvalidValue;
+    if (nrows > ((size_t)1 << lg_constraint) || nnz > ((size_t)1 << lg_non_zero)) return (int)cudaErrorInvalidValue;
+    const uint32_t lg_max = lg_constraint > lg_variable ? lg_constraint : lg_variable;
+    const void* tw = nullptr;
+    int lgN = 0;
+    if ((rc = ntt_get_twiddles((int)lg_max, &tw, &lgN)) != 0) return rc;
+    uint8_t* scratch = nullptr;
+    cudaError_t e = pool_alloc(&scratch, 256, stream);
+    if (e != cudaSuccess) return (int)e;
+    int* bad = (int*)scratch;
+    rc = (int)cudaMemsetAsync(bad, 0, sizeof(int), stream);
+    const size_t K = (size_t)1 << lg_non_zero;
+    if (rc == 0) {
+        k_matrix_evals<<<(unsigned)((K + 255) / 256), 256, 0, stream>>>(m, K, (const uint32_t*)tw, lgN, (int)lg_constraint, (int)lg_variable,
+                                                                        (uint32_t*)d_row, (uint32_t*)d_col, (uint32_t*)d_row_col_val, bad);
+        count_launch();
+        rc = (int)cudaGetLastError();
+    }
+    return csr_finish(rc, scratch, bad, stream);
+}
+
+int csr_transpose_device(void* d_t_row_ptr, void* d_t_cols, void* d_t_vals, const void* d_row_ptr, size_t nrows, const void* d_cols,
+                         const void* d_vals, size_t nnz, size_t nvars, size_t input_size, uint32_t lg_variable, cudaStream_t stream) {
+    CsrArgs m;
+    int rc = csr_index_args(&m, d_row_ptr, nrows, d_cols, d_vals, nnz, nvars, input_size, lg_variable);
+    if (rc != 0) return rc;
+    if (!d_t_row_ptr || (nnz && (!d_t_cols || !d_t_vals))) return (int)cudaErrorInvalidValue;
+    const size_t V = (size_t)1 << lg_variable, ntiles = (V + SCAN_TILE - 1) / SCAN_TILE;
+    // scratch: [0] bad flag | counts[V] | cursor[V] | tile sums[ntiles]
+    const size_t off_counts = 256, off_cursor = off_counts + ((V * 4 + 255) & ~(size_t)255),
+                 off_tiles = off_cursor + ((V * 4 + 255) & ~(size_t)255), total = off_tiles + ntiles * 4;
+    uint8_t* scratch = nullptr;
+    cudaError_t e = pool_alloc(&scratch, total, stream);
+    if (e != cudaSuccess) return (int)e;
+    int* bad = (int*)scratch;
+    uint32_t *counts = (uint32_t*)(scratch + off_counts), *cursor = (uint32_t*)(scratch + off_cursor), *tiles = (uint32_t*)(scratch + off_tiles);
+    uint32_t* t_row_ptr = (uint32_t*)d_t_row_ptr;
+    rc = (int)cudaMemsetAsync(scratch, 0, off_cursor, stream);              // bad flag and counts
+    if (rc == 0) {
+        const unsigned egrid = (unsigned)((nnz + 255) / 256 > 0 ? (nnz + 255) / 256 : 1);
+        k_csr_col_histogram<<<egrid, 256, 0, stream>>>(m, counts, bad);
+        k_scan_tiles<<<(unsigned)ntiles, SCAN_THREADS, 0, stream>>>(counts, V, t_row_ptr, tiles);
+        k_scan_tile_sums<<<1, SCAN_THREADS, 0, stream>>>(tiles, ntiles, t_row_ptr + V);
+        k_scan_add<<<(unsigned)((V + 255) / 256), 256, 0, stream>>>(t_row_ptr, V, tiles);
+        count_launch(4);
+        rc = (int)cudaMemcpyAsync(cursor, t_row_ptr, V * 4, cudaMemcpyDeviceToDevice, stream);
+        if (rc == 0 && nnz) {
+            k_csr_transpose_scatter<<<egrid, 256, 0, stream>>>(m, cursor, (uint32_t*)d_t_cols, (uint32_t*)d_t_vals);
+            count_launch();
+        }
+        if (rc == 0) rc = (int)cudaGetLastError();
+    }
+    return csr_finish(rc, scratch, bad, stream);
 }
 
 }  // namespace b200

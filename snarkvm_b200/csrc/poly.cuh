@@ -29,6 +29,18 @@ int fr_vec_scalar_op_device(void* d_out, const void* d_a, const void* scalar_mon
 // out[i] = ω_n^i, i < n = 2^lg (EvaluationDomain::elements, fft/domain.rs:307-309)
 int domain_elements_device(void* d_out, uint32_t lg, cudaStream_t stream);
 
+// Varuna indexer over a CSR matrix (row_ptr nrows + 1 u32, cols nnz u32 < nvars, vals Montgomery Fr); input_size = |I| (a power of
+// two), the domains are R = 2^lg_constraint ≥ nrows, C = 2^lg_variable > |I| with C ≥ nvars, K = 2^lg_non_zero ≥ nnz.  A column
+// ≥ nvars or a row_ptr not running from 0 to nnz returns cudaErrorInvalidValue.  Both synchronise the stream.
+// matrix_evals (ahp/matrices.rs:138-195): row / col / row_col_val evaluations on K, 2^lg_non_zero Montgomery Fr each.
+int varuna_matrix_evals_device(void* d_row, void* d_col, void* d_row_col_val, const void* d_row_ptr, size_t nrows, const void* d_cols,
+                               const void* d_vals, size_t nnz, size_t nvars, size_t input_size, uint32_t lg_constraint,
+                               uint32_t lg_variable, uint32_t lg_non_zero, cudaStream_t stream);
+// transpose (ahp/matrices.rs:249-270) as CSR over the reindexed variable domain: t_row_ptr 2^lg_variable + 1 u32, t_cols nnz u32
+// (row indices of the input), t_vals nnz Montgomery Fr; the order of the entries inside a transposed row is unspecified.
+int csr_transpose_device(void* d_t_row_ptr, void* d_t_cols, void* d_t_vals, const void* d_row_ptr, size_t nrows, const void* d_cols,
+                         const void* d_vals, size_t nnz, size_t nvars, size_t input_size, uint32_t lg_variable, cudaStream_t stream);
+
 // Group FFT over G1 (DomainCoeff = G1Projective, fft/domain.rs:169-221 generic path): n = 2^lg affine points in, affine points
 // out (natural order both sides).  direction 1 = inverse (includes n^{-1}): UniversalParams::lagrange_basis
 // (polycommit/kzg10/data_structures.rs:68-72).

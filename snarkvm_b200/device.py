@@ -392,6 +392,46 @@ def sparse_matvec(row_ptr: torch.Tensor, cols: torch.Tensor, vals: torch.Tensor,
     return out
 
 
+def _csr_args(row_ptr: torch.Tensor, cols: torch.Tensor, vals: torch.Tensor):
+    if row_ptr.dtype != torch.int32 or cols.dtype != torch.int32:
+        raise TypeError("row_ptr and cols must be int32 tensors")
+    nnz = cols.numel()
+    if _nbytes(vals) != nnz * 32:
+        raise ValueError("one 32-byte value per column index")
+    return (_check(row_ptr, "row_ptr"), row_ptr.numel() - 1, _check(cols, "cols") if nnz else None, _check(vals, "vals") if nnz else None,
+            nnz)
+
+
+def varuna_matrix_evals(row_ptr: torch.Tensor, cols: torch.Tensor, vals: torch.Tensor, nvars: int, input_size: int, lg_constraint: int,
+                        lg_variable: int, lg_non_zero: int):
+    """matrix_evals (snark/varuna/ahp/matrices.rs:138-195) of a CSR matrix (row_ptr int32 [nrows + 1], cols int32 [nnz], vals [nnz, 4]
+    i64 Montgomery) → (row, col, row_col_val), [2^lg_non_zero, 4] i64 Montgomery each, padded with (1, 1, 0).  A column ≥ nvars
+    raises CudaError."""
+    rp, nrows, cp, vp, nnz = _csr_args(row_ptr, cols, vals)
+    K = 1 << lg_non_zero
+    row, col, rcv = (torch.empty((K, 4), dtype=torch.int64, device=row_ptr.device) for _ in range(3))
+    with torch.cuda.device(row_ptr.device):
+        _lib.check(_lib.lib().snarkvm_b200_varuna_matrix_evals_device(row.data_ptr(), col.data_ptr(), rcv.data_ptr(), rp, nrows, cp, vp, nnz,
+                                                                       nvars, input_size, lg_constraint, lg_variable, lg_non_zero, _stream()))
+    return row, col, rcv
+
+
+def csr_transpose(row_ptr: torch.Tensor, cols: torch.Tensor, vals: torch.Tensor, nvars: int, input_size: int, lg_variable: int):
+    """transpose (snark/varuna/ahp/matrices.rs:249-270) over the variable domain → (t_row_ptr int32 [2^lg_variable + 1], t_cols int32
+    [nnz] row indices, t_vals [nnz, 4] i64); entries inside a transposed row come in no fixed order.  A column ≥ nvars raises
+    CudaError."""
+    rp, nrows, cp, vp, nnz = _csr_args(row_ptr, cols, vals)
+    dev = row_ptr.device
+    t_row_ptr = torch.empty((1 << lg_variable) + 1, dtype=torch.int32, device=dev)
+    t_cols = torch.empty(nnz, dtype=torch.int32, device=dev)
+    t_vals = torch.empty((nnz, 4), dtype=torch.int64, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(_lib.lib().snarkvm_b200_csr_transpose_device(t_row_ptr.data_ptr(), t_cols.data_ptr() if nnz else None,
+                                                                 t_vals.data_ptr() if nnz else None, rp, nrows, cp, vp, nnz, nvars,
+                                                                 input_size, lg_variable, _stream()))
+    return t_row_ptr, t_cols, t_vals
+
+
 def poly_divide_by_linear(p: torch.Tensor, point_mont) -> torch.Tensor:
     """Quotient of p / (x − point), the KZG witness polynomial (kzg10/mod.rs:220-241) → CUDA tensor [m − 1, 4] i64, not trimmed."""
     z = _fr_host(point_mont)

@@ -3,7 +3,9 @@
 Device-side mirror of /root/reference/algorithms/src/snark/varuna for the part of `prove_batch` (varuna.rs:336-620) that is
 bulk field arithmetic — the five `AHPForR1CS::prover_*_round` functions and the indexer's arithmetization:
 
-    ahp/indexer/indexer.rs:121-200, ahp/matrices.rs:138-190, 239-254   Circuit            (domains, row / col / row_col_val on K, transposes)
+    ahp/indexer/indexer.rs:121-200, ahp/matrices.rs:138-195, 249-270   Circuit            (domains, row / col / row_col_val on K, transposes)
+    ahp/matrices.rs:211-240                        Circuit.index_polynomials (MatrixArithmetization::new)
+    varuna.rs:72-134, 226-233                      circuit_setup        (the verifying key's twelve index commitments)
     ahp/prover/round_functions/mod.rs:43-192, ahp/prover/state.rs:107-178   init_prover   (z_A, z_B, z_C by sparse mat-vec, x_poly)
     ahp/prover/round_functions/first.rs:129-160    prover_first_round   (w)
     ahp/prover/round_functions/third.rs:207-234    calculate_assignments (z)
@@ -21,6 +23,8 @@ Polynomials are CUDA tensors [m, 4] int64 (Montgomery Fr, low degree first, NOT 
 `trimmed()` gives the reference's canonical form on the host).
 """
 from __future__ import annotations
+
+from dataclasses import dataclass
 
 import numpy as np
 import torch
@@ -116,28 +120,23 @@ def apply_randomized_selector(poly: torch.Tensor, combiner: int, target: Evaluat
     return h, xg
 
 
-def reindex_by_subdomain(variable_size: int, input_size: int, index: np.ndarray) -> np.ndarray:
-    """EvaluationDomain::reindex_by_subdomain (fft/domain.rs:322-344), vectorised"""
-    if variable_size <= input_size:
-        raise ValueError("other.size() must be smaller than self.size()")
-    period = variable_size // input_size
-    index = np.asarray(index, dtype=np.int64)
-    i = index - input_size
-    x = period - 1
-    return np.where(index < input_size, index * period, i + i // x + 1)
-
-
 class Matrix:
     """A sparse R1CS matrix in CSR form on the device: row_ptr int32 [nrows + 1], cols int32 [nnz] (variable indices: public first,
-    then private — into_matrix_helper, ahp/matrices.rs:39-63), vals [nnz, 4] int64 Montgomery."""
+    then private — into_matrix_helper, ahp/matrices.rs:39-63), vals [nnz, 4] int64 Montgomery.  The arrays are uploaded once; no
+    host copy is kept."""
 
     def __init__(self, row_ptr: np.ndarray, cols: np.ndarray, vals_mont: np.ndarray, dev):
-        self.row_ptr_h = np.ascontiguousarray(row_ptr, dtype=np.int64)
-        self.cols_h = np.ascontiguousarray(cols, dtype=np.int64)
         self.nrows, self.nnz = len(row_ptr) - 1, len(cols)
-        self.row_ptr = torch.from_numpy(self.row_ptr_h.astype(np.int32)).to(dev)
-        self.cols = torch.from_numpy(self.cols_h.astype(np.int32)).to(dev)
+        self.row_ptr = torch.from_numpy(np.ascontiguousarray(row_ptr, dtype=np.int32)).to(dev)
+        self.cols = torch.from_numpy(np.ascontiguousarray(cols, dtype=np.int32)).to(dev)
         self.vals = torch.from_numpy(np.ascontiguousarray(vals_mont, dtype=np.uint64).reshape(-1, 4).view(np.int64)).to(dev)
+
+    @classmethod
+    def from_device(cls, row_ptr: torch.Tensor, cols: torch.Tensor, vals: torch.Tensor) -> "Matrix":
+        m = cls.__new__(cls)
+        m.nrows, m.nnz = row_ptr.numel() - 1, cols.numel()
+        m.row_ptr, m.cols, m.vals = row_ptr, cols, vals
+        return m
 
 
 class MatrixEvals:
@@ -147,12 +146,45 @@ class MatrixEvals:
         self.row, self.col, self.row_col_val, self.domain = row, col, row_col_val, domain
 
 
+_domain_size = EvaluationDomain.compute_size_of_domain            # fft/domain.rs:151-154
+
+
+@dataclass(frozen=True)
+class CircuitInfo:
+    """ahp/indexer/circuit_info.rs: the six counts index_helper records (ahp/indexer/indexer.rs:169-176)"""
+    num_public_inputs: int
+    num_public_and_private_variables: int
+    num_constraints: int
+    num_non_zero_a: int
+    num_non_zero_b: int
+    num_non_zero_c: int
+
+    def max_degree(self, zk: bool = False) -> int:
+        """CircuitInfo::max_degree → AHPForR1CS::max_degree (circuit_info.rs:43-46, ahp/ahp.rs:85-107); zk_bound is 1 in the hiding
+        mode, 0 otherwise"""
+        zk_bound = 1 if zk else 0
+        r = _domain_size(self.num_constraints)
+        v = _domain_size(self.num_public_and_private_variables)
+        k = _domain_size(max(self.num_non_zero_a, self.num_non_zero_b, self.num_non_zero_c))
+        return max(2 * r + 2 * zk_bound - 2, 2 * v + 2 * zk_bound - 2, v + 3 if zk else 0, v, r, k - 1)
+
+    def degree_bounds(self) -> list:
+        """AHPForR1CS::get_degree_bounds (ahp/ahp.rs:110-121): the bounds of g_1, g_a, g_b, g_c"""
+        return [_domain_size(n) - 2 for n in (self.num_public_and_private_variables, self.num_non_zero_a, self.num_non_zero_b,
+                                               self.num_non_zero_c)]
+
+
+# the twelve index polynomials in the order of their labels circuit_{id}_{name}_{matrix} sorted as strings (varuna.rs:116), which
+# is the same for every circuit id
+INDEX_POLYNOMIAL_NAMES = tuple(f"{p}_{m}" for p in ("col", "row", "row_col", "row_col_val") for m in "abc")
+
+
 class Circuit:
     """AHPForR1CS::index_helper (ahp/indexer/indexer.rs:121-200) for the non-hiding mode: the caller has already padded the public
-    variables to a power of two (pad_input_for_indexer_and_prover, ahp/matrices.rs:85-100)."""
+    variables to a power of two (pad_input_for_indexer_and_prover, ahp/matrices.rs:85-100).  The evaluations on K and the
+    transposes are built on the device from the CSR arrays (device.varuna_matrix_evals, device.csr_transpose)."""
 
     def __init__(self, a: Matrix, b: Matrix, c: Matrix, num_public: int, num_variables: int):
-        dev = a.vals.device
         self.a, self.b, self.c = a, b, c
         self.num_public, self.num_variables, self.num_constraints = num_public, num_variables, a.nrows
         if num_public & (num_public - 1):
@@ -160,36 +192,63 @@ class Circuit:
         self.constraint_domain = EvaluationDomain.new(self.num_constraints)
         self.variable_domain = EvaluationDomain.new(num_variables)
         self.input_domain = EvaluationDomain.new(num_public)
+        if self.variable_domain.size <= self.input_domain.size:          # reindex_by_subdomain (fft/domain.rs:327-329)
+            raise ValueError("other.size() must be smaller than self.size()")
         self.non_zero_domains = [EvaluationDomain.new(m.nnz) for m in (a, b, c)]
         self.max_non_zero_domain = max(self.non_zero_domains, key=lambda d: d.size)
-        r_el = device.domain_elements(self.constraint_domain.log_size_of_group, dev)
-        c_el = device.domain_elements(self.variable_domain.log_size_of_group, dev)
-        one = torch.from_numpy(_mont(1).view(np.int64)).to(dev)
+        self.info = CircuitInfo(num_public, num_variables, self.num_constraints, a.nnz, b.nnz, c.nnz)
+        lg_r, lg_c = self.constraint_domain.log_size_of_group, self.variable_domain.log_size_of_group
         self.ariths, self.transposes = [], []
         for m, K in zip((a, b, c), self.non_zero_domains):
-            entry_rows = np.repeat(np.arange(m.nrows, dtype=np.int64), np.diff(m.row_ptr_h))
-            entry_cols = reindex_by_subdomain(self.variable_domain.size, self.input_domain.size, m.cols_h)
-            # matrix_evals (ahp/matrices.rs:138-190)
-            row = one.repeat(K.size, 1)
-            col = one.repeat(K.size, 1)
-            rcv = _zeros(K.size, dev)
-            if m.nnz:
-                row[: m.nnz] = r_el[torch.from_numpy(entry_rows).to(dev)]
-                col[: m.nnz] = c_el[torch.from_numpy(entry_cols).to(dev)]
-                rc = device.fr_vec_op(row[: m.nnz].contiguous(), col[: m.nnz].contiguous(), device.FR_MUL)
-                rcv[: m.nnz] = device.fr_vec_op(m.vals, rc, device.FR_MUL)
+            row, col, rcv = device.varuna_matrix_evals(m.row_ptr, m.cols, m.vals, num_variables, self.input_domain.size, lg_r, lg_c,
+                                                       K.log_size_of_group)
             self.ariths.append(MatrixEvals(row, col, rcv, K))
-            # transpose (ahp/matrices.rs:239-254) as CSR over the variable domain's indices; entries keep the row-major order
-            order = np.argsort(entry_cols, kind="stable")
-            counts = np.bincount(entry_cols, minlength=self.variable_domain.size)
-            t_ptr = np.concatenate([[0], np.cumsum(counts)])
-            t_vals = m.vals[torch.from_numpy(order).to(dev)] if m.nnz else m.vals
-            tm = Matrix.__new__(Matrix)
-            tm.nrows, tm.nnz = self.variable_domain.size, m.nnz
-            tm.row_ptr = torch.from_numpy(t_ptr.astype(np.int32)).to(dev)
-            tm.cols = torch.from_numpy(entry_rows[order].astype(np.int32)).to(dev)
-            tm.vals = t_vals.contiguous()
-            self.transposes.append(tm)
+            self.transposes.append(Matrix.from_device(*device.csr_transpose(m.row_ptr, m.cols, m.vals, num_variables,
+                                                                            self.input_domain.size, lg_c)))
+
+    def index_polynomials(self) -> dict:
+        """MatrixArithmetization::new (ahp/matrices.rs:211-240) for A, B, C: the iFFT over each matrix's K of row, col, row_col
+        (= row∘col, padding 1·1 = 1) and row_col_val → {name: [|K|, 4] i64 Montgomery coefficients} in INDEX_POLYNOMIAL_NAMES order"""
+        out = {}
+        for m, arith in zip("abc", self.ariths):
+            K = arith.domain
+            out[f"row_{m}"] = K.ifft(arith.row)
+            out[f"col_{m}"] = K.ifft(arith.col)
+            out[f"row_col_{m}"] = K.ifft_in_place(device.fr_vec_op(arith.row, arith.col, device.FR_MUL))
+            out[f"row_col_val_{m}"] = K.ifft(arith.row_col_val)
+        return {name: out[name] for name in INDEX_POLYNOMIAL_NAMES}
+
+
+@dataclass
+class CircuitVerifyingKey:
+    """snark/varuna/data_structures/circuit_verifying_key.rs without the circuit id: the index counts and the twelve index commitments
+    (normalised projective uint64[12, 18]) in INDEX_POLYNOMIAL_NAMES order"""
+    circuit_info: CircuitInfo
+    circuit_commitments: np.ndarray
+
+
+@dataclass
+class CircuitProvingKey:
+    """snark/varuna/data_structures/circuit_proving_key.rs: the verifying key, the indexed circuit and its committer key"""
+    circuit_verifying_key: CircuitVerifyingKey
+    circuit: Circuit
+    committer_key: object
+
+
+def circuit_setup(circuit: Circuit, pp_powers_of_beta_g: torch.Tensor, pp_powers_of_beta_times_gamma_g: torch.Tensor, zk: bool = False):
+    """VarunaSNARK::circuit_setup → batch_circuit_setup for one circuit (varuna.rs:72-134, 226-233): trim the universal parameters to
+    the circuit's max_degree and degree bounds, commit the twelve index polynomials in ONE pass (no degree bound, no hiding) and return
+    (CircuitProvingKey, CircuitVerifyingKey).  The SRS is (β^i·G, γβ^i·G) as sonic_pc.CommitterKey.trim takes it."""
+    from .sonic_pc import CommitterKey, LabeledPolynomial, SonicKZG10
+    info = circuit.info
+    max_degree = info.max_degree(zk)
+    if pp_powers_of_beta_g.shape[0] < max_degree + 1:                  # download_powers_for(0..max_degree), varuna.rs:85-87
+        raise ValueError(f"the SRS holds {pp_powers_of_beta_g.shape[0]} powers; the circuit needs {max_degree + 1}")
+    ck = CommitterKey.trim(pp_powers_of_beta_g, pp_powers_of_beta_times_gamma_g, max_degree, (), 1, info.degree_bounds())
+    polys = circuit.index_polynomials()
+    comms, _rands = SonicKZG10.commit(ck, [LabeledPolynomial(name, p) for name, p in polys.items()])
+    vk = CircuitVerifyingKey(info, comms)
+    return CircuitProvingKey(vk, circuit, ck), vk
 
 
 class Prover:
