@@ -134,7 +134,7 @@ void write_infinity(void* out144) {
 // exactly where the reference's own plugin finishes, snarkvm.cu:290-295).  out144s: njobs × 144 B of HOST memory.
 int msm_jobs_impl(void* out144s, const MsmPlan& plan, const MsmBases* bases, int nbases, const uint32_t* table, size_t table_n,
                   const MsmSegment* segs, int nsegs, int njobs, cudaStream_t stream) {
-    const size_t sets = table ? 1 : (size_t)plan.nwin;
+    const size_t sets = table ? 1 : (size_t)plan.nsets;
     const size_t npts = (size_t)njobs * sets;
     uint32_t* d_buf = nullptr;
     cudaError_t e = pool_alloc(&d_buf, npts * 192 + 256, stream);
@@ -161,7 +161,7 @@ int msm_jobs_impl(void* out144s, const MsmPlan& plan, const MsmBases* bases, int
     memcpy(&flags, sums.data() + npts, 4);
     if (flags & 1u) return (int)cudaErrorInvalidValue;           // a scalar ≥ 2^253: not a canonical Fr, let the caller fall back
     auto finish = [&](int j) {
-        host::Xyzz total = table ? sums[(size_t)j] : host::horner_windows(sums.data() + (size_t)j * sets, plan.nwin, plan.c);
+        host::Xyzz total = table ? sums[(size_t)j] : host::horner_windows(sums.data() + (size_t)j * sets, plan.nwin, plan.c, plan.top_sets());
         host::xyzz_to_normalised_projective(total, (uint64_t*)((uint8_t*)out144s + (size_t)j * 144));
     };
     if (njobs <= 2) { for (int j = 0; j < njobs; j++) finish(j); }
@@ -674,7 +674,7 @@ snarkvm_error_t snarkvm_msm(void* out, const void* points, size_t npoints, const
         std::vector<size_t> sum_off{0};                                   // in XYZZ points
         for (int k = 0; k < chunks; k++) {
             plans.push_back(msm_make_plan(bounds[k + 1] - bounds[k]));
-            sum_off.push_back(sum_off.back() + (size_t)plans.back().nwin);
+            sum_off.push_back(sum_off.back() + (size_t)plans.back().nsets);
         }
         std::vector<cudaEvent_t> ev((size_t)chunks + 1, nullptr);
         for (auto& e : ev) if (rc == 0) rc = (int)cudaEventCreateWithFlags(&e, cudaEventDisableTiming);
@@ -711,7 +711,7 @@ snarkvm_error_t snarkvm_msm(void* out, const void* points, size_t npoints, const
         }
         if (rc == 0) {
             host::Xyzz total = host::xyzz_inf();
-            for (int k = 0; k < chunks; k++) host::xyzz_add(total, host::horner_windows(sums.data() + sum_off[k], plans[k].nwin, plans[k].c));
+            for (int k = 0; k < chunks; k++) host::xyzz_add(total, host::horner_windows(sums.data() + sum_off[k], plans[k].nwin, plans[k].c, plans[k].top_sets()));
             host::xyzz_to_normalised_projective(total, result);
         }
     }
@@ -737,14 +737,14 @@ int snarkvm_b200_polymul_device(void* d_out, size_t pcount, const void* const* d
 }
 
 int snarkvm_b200_msm_plan(size_t npoints, int* c, int* nwin, uint32_t* cap) {
-    MsmPlan p = msm_make_plan(npoints);
+    MsmPlan p = msm_make_plan(npoints, false);
     if (c) *c = p.c;
     if (nwin) *nwin = p.nwin;
     if (cap) *cap = p.cap;
     return 0;
 }
 
-int snarkvm_b200_msm_plan_levels(size_t npoints) { return msm_make_plan(npoints).levels; }
+int snarkvm_b200_msm_plan_levels(size_t npoints) { return msm_make_plan(npoints, false).levels; }
 
 int snarkvm_b200_msm_device(void* out144, const void* d_points, size_t npoints, const void* d_scalars, size_t stride,
                             void* stream) {
@@ -810,7 +810,7 @@ int snarkvm_b200_msm_window_sums_plan_device(void* d_window_sums, uint32_t* d_fl
                                              size_t npoints, const void* d_scalars, size_t stride, void* stream_v) {
     if (!d_window_sums || stride < 104 || (stride & 7) || plan_npoints == 0 || npoints > plan_npoints) return (int)cudaErrorInvalidValue;
     cudaStream_t stream = (cudaStream_t)stream_v;
-    MsmPlan plan = msm_make_plan(plan_npoints);
+    MsmPlan plan = msm_make_plan(plan_npoints, false);
     uint32_t* own_flags = nullptr;
     int rc = 0;
     if (!d_flags) { rc = (int)pool_alloc(&own_flags, 256, stream); if (rc) return rc; d_flags = own_flags; }
@@ -828,7 +828,7 @@ int snarkvm_b200_msm_window_sums_host(void* d_window_sums, uint32_t* d_flags, si
                                       const void* h_scalars, size_t stride, void* stream_v) {
     if (!d_window_sums || stride < 104 || (stride & 7) || plan_npoints == 0 || npoints > plan_npoints) return (int)cudaErrorInvalidValue;
     cudaStream_t stream = (cudaStream_t)stream_v;
-    MsmPlan plan = msm_make_plan(plan_npoints);
+    MsmPlan plan = msm_make_plan(plan_npoints, false);
     uint32_t* own_flags = nullptr;
     int rc = 0;
     if (!d_flags) { rc = (int)pool_alloc(&own_flags, 256, stream); if (rc) return rc; d_flags = own_flags; }
@@ -1079,7 +1079,7 @@ static int msm_g2_impl(void* out288, const void* d_points, size_t npoints, const
     if (!out288) return (int)cudaErrorInvalidValue;
     if (npoints == 0) { host::Xyzz2 inf = host::xyzz_inf_t<host::Fq2>(); host::xyzz_to_normalised_projective(inf, (uint64_t*)out288); return 0; }
     if (!d_points || !d_scalars || stride < 200 || (stride & 7)) return (int)cudaErrorInvalidValue;
-    MsmPlan plan = msm_make_plan(npoints);
+    MsmPlan plan = msm_make_plan(npoints, false);
     const size_t nw = (size_t)plan.nwin;
     uint32_t* d_buf = nullptr;
     cudaError_t e = pool_alloc(&d_buf, nw * 384 + 256, stream);

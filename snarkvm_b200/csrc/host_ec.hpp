@@ -195,12 +195,14 @@ inline Xyzz xyzz_from_projective(const uint64_t in[18]) {
 // (Measured and dropped: a Jacobian doubling chain, 2M + 5S against XYZZ's 5M + 4S, and a dedicated squaring.  On the host the
 // 13 additions of the Jacobian doubling and the less regular code cost what the two saved products gain: 620 vs 640 ns per
 // doubling; the squaring with 57 word products ran at 60 ns against 50 ns for the row loop.)
-// Σ_w 2^{c·w} · window_sum[w]  (Horner from the top window; batched.rs:404-413, standard.rs:107-117)
-template <class F> inline XyzzT<F> horner_windows(const XyzzT<F>* sums, int nwin, int c) {
+// Σ_w 2^{c·w} · window_sum[w]  (Horner from the top window; batched.rs:404-413, standard.rs:107-117).  Every window but the top
+// one is c bits wide; the top window's sum comes in `top_sets` parts, sums[nwin − 1 …] (its bucket sets, MsmPlan).
+template <class F> inline XyzzT<F> horner_windows(const XyzzT<F>* sums, int nwin, int c, int top_sets = 1) {
     XyzzT<F> total = xyzz_inf_t<F>();
     for (int w = nwin - 1; w >= 0; w--) {
         for (int k = 0; k < c; k++) xyzz_dbl(total);
         xyzz_add(total, sums[w]);
+        if (w == nwin - 1) for (int s = 1; s < top_sets; s++) xyzz_add(total, sums[w + s]);
     }
     return total;
 }

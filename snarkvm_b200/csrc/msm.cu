@@ -9,6 +9,7 @@
 #include <vector>
 #include <cstdio>
 #include <cstdlib>
+#include <cstring>
 #include <cub/device/device_scan.cuh>
 
 #define FF_CALL_MUL 1
@@ -72,16 +73,55 @@ static int plan_log2(size_t x) {
     return l;
 }
 
-MsmPlan msm_make_plan(size_t npoints) {
+// "w,w,…" or "w*k,…" (k windows of w bits): every width but the last equal, the last one wide enough that the top digit of a
+// scalar below 2^253 stays non-negative.  Returns false (and leaves p alone) for anything else.
+static bool parse_window_widths(const char* s, MsmPlan& p) {
+    std::vector<int> w;
+    while (*s) {
+        char* end = nullptr;
+        long v = strtol(s, &end, 10);
+        if (end == s || v < 2 || v > 24) return false;
+        long k = 1;
+        s = end;
+        if (*s == '*') { k = strtol(s + 1, &end, 10); if (end == s + 1 || k < 1 || k > 128) return false; s = end; }
+        for (long i = 0; i < k && w.size() <= 128; i++) w.push_back((int)v);
+        if (*s == ',') s++;
+        else if (*s) return false;
+    }
+    if (w.size() < 2 || w.size() > 128) return false;
+    for (size_t i = 1; i + 1 < w.size(); i++) if (w[i] != w[0]) return false;
+    const int c = w[0], nwin = (int)w.size(), c_top = w.back();
+    if ((nwin - 1) * c >= 253 || (nwin - 1) * c + c_top < 254) return false;          // top raw ≤ 2^(253 − bit) ≤ 2^(c_top − 1)
+    const int top_sets = c_top > c ? 1 << (c_top - c) : 1;
+    if (top_sets > 64) return false;
+    p.c = c; p.nwin = nwin; p.c_top = c_top; p.nsets = nwin - 1 + top_sets;
+    p.nbuckets = 1u << (c - 1);
+    return true;
+}
+
+MsmPlan msm_make_plan(size_t npoints, bool mixed) {
     MsmPlan p;
     int lg = plan_log2(npoints);
     // Window bits from a sweep (tools/tune_msm.py): wider windows mean fewer
     // bucket additions (n·W) but more buckets to reduce and shorter, more divergent bucket runs.
     int c = lg <= 8 ? 4 : lg <= 12 ? lg - 4 : lg <= 18 ? 11 : lg == 19 ? 13 : lg == 20 ? 15 : lg <= 22 ? 16 : 17;
-    if (const char* e = getenv("SNARKVM_B200_MSM_C")) { int v = atoi(e); if (v >= 2 && v <= 24) c = v; }
+    const char* ec = getenv("SNARKVM_B200_MSM_C");
+    if (ec) { int v = atoi(ec); if (v >= 2 && v <= 24) c = v; }
     p.c = c;
     p.nwin = 253 / c + 1;
     p.nbuckets = 1u << (c - 1);
+    p.c_top = c;
+    p.nsets = p.nwin;
+    // Mixed layouts (tools/sweep_msm_windows.py, DESIGN §4): from 2^24, 13 windows of 18 bits and a 20-bit top window — 14
+    // windows instead of 15, every bucket set 2^17 buckets, the top window's digits (≤ 305 881 below r) in four sets.  At 2^22
+    // and 2^23 the uniform plans stay ahead (the larger reduction and sort cost more than the 1/15 fewer additions save).
+    // SNARKVM_B200_MSM_C asks for a uniform plan; SNARKVM_B200_MSM_WINDOWS names a layout ("18*13,20"), or "0" for the uniform one.
+    if (mixed) {
+        const char* ew = getenv("SNARKVM_B200_MSM_WINDOWS");
+        if (ew && *ew && strcmp(ew, "0") != 0) parse_window_widths(ew, p);
+        else if (!ew && !ec && lg >= 24) parse_window_widths("18*13,20", p);
+        c = p.c;
+    }
     // Aim for ≥ ~300k work items so 132 SMs × (2 × 256-thread CTAs) see several waves, but keep
     // items long enough (≥ 16 points) that the per-item overhead stays in the noise.
     size_t total = npoints * (size_t)p.nwin;
@@ -131,8 +171,10 @@ MsmPlan msm_make_plan_batch(size_t max_n, size_t total_n) {
 // this scalar vector's first point in the call's dense base array.  MONT: the scalars are Montgomery Fr (polynomial
 // coefficients) and are converted here (to_bigint, kzg10/mod.rs:469-474).  Scalars with bits 253..255 set are outside
 // what nwin windows cover: they raise bit 0 of *flags and the caller returns an error instead of a wrong point.
+// Windows below the top one have c_low bits, the top one c_top (MsmPlan); the top window's digits run past nbuckets into the
+// sets that follow its first one.
 template <bool SCATTER, bool MONT>
-__global__ void __launch_bounds__(256) k_digits(const uint32_t* __restrict__ scalars, size_t n, int c, int nwin,
+__global__ void __launch_bounds__(256) k_digits(const uint32_t* __restrict__ scalars, size_t n, int c_low, int c_top, int nwin,
                                                 uint32_t nbuckets, uint32_t* __restrict__ counters /* hist or cursors */,
                                                 uint32_t* __restrict__ sorted, size_t flat /* 0, or the table's points per window */,
                                                 uint32_t slot_base, uint32_t index_base, uint32_t* __restrict__ flags) {
@@ -153,15 +195,16 @@ __global__ void __launch_bounds__(256) k_digits(const uint32_t* __restrict__ sca
         for (int k = 0; k < 8; k++) s[k] = x.v[k];
     }
     if (!SCATTER && (s[7] >> 29)) atomicOr(flags, 1u);
-    const uint32_t half = 1u << (c - 1);
     uint32_t carry = 0;
     for (int w = 0; w < nwin; w++) {
-        int bit = w * c;
+        const int c = w == nwin - 1 ? c_top : c_low;
+        int bit = w * c_low;
         // dynamic register-array indexing would spill: select the two words with a small switch-free scan
         int wi = bit >> 5, sh = bit & 31;
         uint32_t lo = 0, hi = 0;
 #pragma unroll
         for (int k = 0; k < 8; k++) { if (k == wi) lo = s[k]; if (k == wi + 1) hi = s[k]; }
+        const uint32_t half = 1u << (c - 1);
         uint32_t raw = (__funnelshift_r(lo, hi, sh) & ((1u << c) - 1u)) + carry;
         uint32_t neg = raw > half ? 1u : 0u;
         uint32_t mag = neg ? (1u << c) - raw : raw;
@@ -216,7 +259,8 @@ static constexpr uint32_t REC_NONE = 0xffffffffu;
 // feeds the job's single bucket set.
 template <bool MONT, bool FLAT>
 __global__ void __launch_bounds__(256) k_scatter_records(const uint32_t* __restrict__ scalars, size_t n, const uint8_t* __restrict__ points,
-                                                         size_t stride, const uint32_t* __restrict__ table, size_t table_n, int c, uint32_t nbuckets,
+                                                         size_t stride, const uint32_t* __restrict__ table, size_t table_n, int c_low, int c_top,
+                                                         int nwin, uint32_t nbuckets,
                                                          uint32_t* __restrict__ cursors, uint32_t slot_base, int w_lo, int w_hi,
                                                          const uint32_t* __restrict__ pos_base_ptr, uint4* __restrict__ dense0) {
     __shared__ uint4 sh_rec[256 * 9];                       // per point: x (3 × 16 B), y (3), −y (3)
@@ -256,15 +300,16 @@ __global__ void __launch_bounds__(256) k_scatter_records(const uint32_t* __restr
             stage(pt.x, pt.y, pt.inf);
         }
     }
-    const uint32_t half = 1u << (c - 1);
     uint32_t carry = 0;
     // One window at a time (issuing the cursor atomics of 8 windows back to back before one barrier was measured slower at
     // 2^24 — co-resident CTAs in different phases already overlap).
     for (int w = 0; w < w_hi; w++) {
-        const int bit = w * c, wi = bit >> 5, sh = bit & 31;
+        const int c = w == nwin - 1 ? c_top : c_low;          // (k_digits)
+        const int bit = w * c_low, wi = bit >> 5, sh = bit & 31;
         uint32_t lo = 0, hi = 0;
 #pragma unroll
         for (int k = 0; k < 8; k++) { if (k == wi) lo = s[k]; if (k == wi + 1) hi = s[k]; }
+        const uint32_t half = 1u << (c - 1);
         const uint32_t raw = (__funnelshift_r(lo, hi, sh) & ((1u << c) - 1u)) + carry;
         const uint32_t neg = raw > half ? 1u : 0u;
         const uint32_t mag = neg ? (1u << c) - raw : raw;
@@ -607,8 +652,9 @@ FF_DEV int pair_classify_global(const PairDesc& d, const uint32_t* __restrict__ 
 template <bool GATHER, int MINB>
 __global__ void __launch_bounds__(PAIR_THREADS, MINB) k_pair_level2(const uint32_t* __restrict__ records /* level 0: dense bases / table; above: dense_in */,
                                                          const uint2* __restrict__ desc, const uint32_t* __restrict__ total_ptr,
-                                                         uint32_t T, uint32_t* __restrict__ prefix, uint32_t* __restrict__ dense_out,
+                                                         uint32_t T_bound, uint32_t* __restrict__ prefix, uint32_t* __restrict__ dense_out,
                                                          uint32_t* __restrict__ sm_slots) {
+    (void)T_bound;
     extern __shared__ uint4 pair2_smem[];
     __shared__ uint32_t sh_slot;
     uint32_t* sh_inv = reinterpret_cast<uint32_t*>(pair2_smem);                       // 128 × 48 B
@@ -622,6 +668,12 @@ __global__ void __launch_bounds__(PAIR_THREADS, MINB) k_pair_level2(const uint32
     __syncthreads();
     const int inv_warp = (int)(sh_slot & 3u);
     const uint32_t total = __ldg(total_ptr);
+    // Steps per lane from the level's ACTUAL output count: the host sizes the grid (whole waves) from an upper bound, Σ cnt/2 +
+    // #buckets, which overshoots by up to half a bucket per bucket — 11 % at the last of five levels at 2^24 points, more with
+    // more buckets — and every lane walks all T steps, so T from the bound made the whole grid that much slower.  Any partition
+    // works for Montgomery's trick and the outputs do not depend on it.
+    const uint64_t lanes = (uint64_t)gridDim.x * PAIR_THREADS;
+    const uint32_t T = total > lanes ? (uint32_t)((total + lanes - 1) / lanes) : 1u;      // ≤ T_bound
     const uint64_t w0_64 = ((uint64_t)blockIdx.x * (PAIR_THREADS / 32) + (uint32_t)warp) * 32ull * T + (uint32_t)lane;   // this lane's first output
     uint32_t nv = 0;                                                                   // steps that exist for this lane
     if (w0_64 < total) { const uint64_t left = (total - w0_64 + 31) / 32; nv = left < T ? (uint32_t)left : T; }
@@ -815,6 +867,21 @@ FF_DEV XYZZ bucket_sum(const uint32_t* __restrict__ partial, const uint32_t* __r
     return s;
 }
 
+// Digit offset of the buckets of set `set` of a launch (MsmPlan::set_digit_offset): the sets of the launch are sets set0, set0 + 1, …
+// of the call, per_job of them per sum, and set k ≥ 1 above the top window's first set `top_first` holds the digits k·nbuckets + b + 1.
+// Its window sum is Σ_b (k·nbuckets + b + 1)·S_b = (the usual Σ_b (b + 1)·S_b) + k·nbuckets·Σ_b S_b.  Uniform plans: all zero.
+struct SetOffsets {
+    uint32_t set0, per_job, top_first, nbuckets;
+    FF_DEV uint32_t of(uint32_t set) const {
+        const uint32_t s = (set0 + set) % per_job;
+        return s > top_first ? (s - top_first) * nbuckets : 0u;
+    }
+};
+static SetOffsets set_offsets(const MsmPlan& plan, bool flat, uint32_t set0) {
+    if (flat) return SetOffsets{0u, 1u, 0u, 0u};
+    return SetOffsets{set0, (uint32_t)plan.nsets, (uint32_t)plan.nwin - 1u, plan.nbuckets};
+}
+
 // Thread j of window w owns bucket values [lo, hi] = [j·K + 1, (j+1)·K]:
 //   running = Σ S_b ; acc = Σ (b − lo + 1)·S_b   (top-down running sum, batched.rs:356-361)
 //   out = acc + (lo − 1)·running = Σ b·S_b over the chunk.
@@ -827,7 +894,8 @@ template <bool PAIRS>
 __global__ void __launch_bounds__(128) k_bucket_reduce(const uint32_t* __restrict__ partial, const uint32_t* __restrict__ item_start,
                                                         uint32_t nbuckets, uint32_t chunk, uint32_t chunks_per_window,
                                                         uint32_t nwin, uint32_t* __restrict__ out,
-                                                        const uint32_t* __restrict__ partial_b = nullptr, int folds = 0) {
+                                                        const uint32_t* __restrict__ partial_b = nullptr, int folds = 0,
+                                                        SetOffsets so = SetOffsets{0u, 1u, 0u, 0u}) {
     uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= chunks_per_window * nwin) return;
     uint32_t w = t / chunks_per_window, j = t % chunks_per_window;
@@ -850,7 +918,8 @@ __global__ void __launch_bounds__(128) k_bucket_reduce(const uint32_t* __restric
         running.store(out + ((size_t)t * 2 + 1) * XYZZ_WORDS);
         return;
     }
-    if (lo != 0u) acc.add(running.mul_u32(lo));               // bucket value of index lo is lo+1 ⇒ (lo+1−1)·running
+    const uint32_t lo_off = lo + so.of(w);                   // bucket value of index lo is lo+1 (+ the set's digit offset)
+    if (lo_off != 0u) acc.add(running.mul_u32(lo_off));
     acc.store(out + (size_t)t * XYZZ_WORDS);
 }
 
@@ -954,7 +1023,8 @@ __global__ void __launch_bounds__(128) k_bucket_reduce_warp(const uint32_t* __re
     }
 }
 // window sum = Σ_j acc_j + 32·Σ_j j·run_j over the set's chunks (chunks ≤ 32)
-__global__ void __launch_bounds__(32) k_window_combine_warp(const uint32_t* __restrict__ in, uint32_t chunks, uint32_t* __restrict__ out) {
+__global__ void __launch_bounds__(32) k_window_combine_warp(const uint32_t* __restrict__ in, uint32_t chunks, uint32_t* __restrict__ out,
+                                                            SetOffsets so) {
     const uint32_t set = blockIdx.x, lane = threadIdx.x;
     XYZZ a = XYZZ::infinity(), r = XYZZ::infinity();
     if (lane < chunks) {
@@ -969,6 +1039,8 @@ __global__ void __launch_bounds__(32) k_window_combine_warp(const uint32_t* __re
         for (int k = 0; k < 5; k++) w.dbl();
         total.add(w);
     }
+    const uint32_t off = so.of(set);
+    if (off != 0u) { const XYZZ run = warp_sum_xyzz(r); total.add(run.mul_u32(off)); }
     if (lane == 0) total.store(out + (size_t)set * XYZZ_WORDS);
 }
 
@@ -1162,8 +1234,19 @@ __global__ void __launch_bounds__(128) k_combine_level_quadseq(const uint32_t* _
 }
 // window sum of a set from its m0 ≤ 64 entries (each spanning 2^lgw0 buckets): one CTA per set, 8:1 per level through
 // shared memory
+// k·a (double-and-add from the top bit) by one quad
+FF_DEV XYZZ quad_mul_u32(const XYZZ& a, uint32_t k, const Quad& Q) {
+    XYZZ r = XYZZ::infinity();
+#pragma unroll 1
+    for (int b = 31 - __clz(k); b >= 0; b--) {
+        r = quad_dbl(r, Q);
+        if ((k >> b) & 1u) r = quad_add(r, a, Q);
+    }
+    return r;
+}
 static constexpr int COMBINE_QUAD_MAX_WARPS = 8;
-__global__ void __launch_bounds__(32 * COMBINE_QUAD_MAX_WARPS) k_window_combine_quad(const uint32_t* __restrict__ in, uint32_t m0, int lgw0, uint32_t* __restrict__ out) {
+__global__ void __launch_bounds__(32 * COMBINE_QUAD_MAX_WARPS) k_window_combine_quad(const uint32_t* __restrict__ in, uint32_t m0, int lgw0, uint32_t* __restrict__ out,
+                                                                                      SetOffsets so) {
     __shared__ __align__(16) uint32_t sm[COMBINE_QUAD_MAX_WARPS][2][XYZZ_WORDS];
     const uint32_t set = blockIdx.x, warp = threadIdx.x >> 5;
     const Quad Q = Quad::here();
@@ -1178,7 +1261,12 @@ __global__ void __launch_bounds__(32 * COMBINE_QUAD_MAX_WARPS) k_window_combine_
             XYZZ a = XYZZ::infinity(), r = XYZZ::infinity();
             if (j < m) { a = load_xyzz_plain(src + (size_t)j * 2 * XYZZ_WORDS); r = load_xyzz_plain(src + ((size_t)j * 2 + 1) * XYZZ_WORDS); }
             A = combine_fold_quad(a, r, lgw, Q, run);
-            if (groups == 1u && (threadIdx.x & 31u) == 0u) A.store(out + (size_t)set * XYZZ_WORDS);
+            if (groups == 1u) {
+                // slot 0 holds the set's Σ S_b in `run`: add the digit offset's multiple of it (the top window's upper sets)
+                const uint32_t off = so.of(set);
+                if (off != 0u && Q.slot == 0) A = quad_add(A, quad_mul_u32(run, off, Q), Q);
+                if ((threadIdx.x & 31u) == 0u) A.store(out + (size_t)set * XYZZ_WORDS);
+            }
         }
         if (groups == 1u) break;
         __syncthreads();                                                // the previous level's entries have been read
@@ -1354,8 +1442,10 @@ int msm_core(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, co
              const uint32_t* table, size_t table_n, const MsmSegment* segs, int nsegs, int njobs, cudaStream_t stream) {
     int rc = 0;
     const bool flat = table != nullptr;
-    const uint32_t sets_per_job = flat ? 1u : (uint32_t)plan.nwin;   // bucket sets to reduce per job
+    const uint32_t sets_per_job = flat ? 1u : (uint32_t)plan.nsets;  // bucket sets to reduce per job
+    const uint32_t wins_per_job = flat ? 1u : (uint32_t)plan.nwin;   // windows per job, each ≤ one scalar's worth of entries
     if (njobs < 1 || nsegs < 1 || (!flat && nbases < 1)) return (int)cudaErrorInvalidValue;
+    if (plan.nsets < plan.nwin || plan.nwin < 1 || (flat && plan.nsets != plan.nwin)) return (int)cudaErrorInvalidValue;
     const uint64_t nsets64 = (uint64_t)njobs * sets_per_job;
     const uint64_t TB64 = nsets64 * plan.nbuckets;
     if (TB64 >= (1ull << 31)) return (int)cudaErrorInvalidValue;
@@ -1402,28 +1492,37 @@ int msm_core(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, co
         }
     }
 
-    // Everything after the bucket sort runs per GROUP of whole bucket sets, so the dense scratch of the pair levels
-    // (≈ 180 B per entry with the level-0 records) stays inside the budget of the device's cached scratch: on an 80 GB H100,
-    // 2^24 points → all 15 windows in one group (44 GB), a 2^26-point shard three windows at a time.  Fewer groups mean
-    // fewer, larger pair-level launches (H100 SXM, 700 W: 116 ms of kernels in one group against 121 ms in two).
+    // Everything after the bucket sort runs per GROUP of whole windows (all bucket sets of a window together), so the dense
+    // scratch of the pair levels (≈ 180 B per entry with the level-0 records) stays inside the budget of the device's cached
+    // scratch: on an 80 GB H100, 2^24 points → all windows in one group (≈ 42 GB for 14), a 2^26-point shard three windows at a
+    // time.  Fewer groups mean fewer, larger pair-level launches (H100 SXM, 700 W: 116 ms of kernels in one group against 121 ms
+    // in two).  A window holds at most one entry per scalar whatever the number of its sets.
     size_t budget = 0;
     if ((rc = scratch_group_budget(&budget)) != 0) return rc;
     if (const char* e = getenv("SNARKVM_B200_MSM_SCRATCH_GB")) { long v = atol(e); if (v >= 1) budget = (size_t)v << 30; }
     if (const char* e = getenv("SNARKVM_B200_MSM_SCRATCH_MB")) { long v = atol(e); if (v >= 1) budget = (size_t)v << 20; }      // tests: force many groups
-    uint32_t gw = nsets;
+    const uint32_t nwins = (uint32_t)njobs * wins_per_job;
+    uint32_t gu = nwins;                                          // windows per group
     if (levels > 0) {
         // per entry: dense_a 48 + prefix 24 + descriptors 4, plus the 96-byte level-0 records (dense_b reuses them: level 0
         // is their last reader) rounded up to 180 for the item partials and per-bucket arrays; or dense_b 24 + the 4-byte index
-        size_t per_set = set_cap * (size_t)(records ? 180 : 104) + 1;
-        size_t fit = budget / per_set;
+        size_t per_win = set_cap * (size_t)(records ? 180 : 104) + 1;
+        size_t fit = budget / per_win;
         if (fit < 1) fit = 1;
-        if (fit < gw) {
-            const uint32_t ngroups = (uint32_t)((nsets + fit - 1) / fit);          // equal groups (15 sets in 3 groups: 5 + 5 + 5, not 7 + 7 + 1)
-            gw = (nsets + ngroups - 1) / ngroups;
+        if (fit < gu) {
+            const uint32_t ngroups = (uint32_t)((nwins + fit - 1) / fit);          // equal groups (15 windows in 3 groups: 5 + 5 + 5, not 7 + 7 + 1)
+            gu = (nwins + ngroups - 1) / ngroups;
         }
     }
+    // first bucket set of window u of the call (job-major; a window's sets are contiguous, the top window's come last in its job)
+    auto set_of = [&](uint32_t u) { return (u / wins_per_job) * sets_per_job + u % wins_per_job; };
+    uint32_t gw = 0;                                              // bucket sets of the largest group
+    for (uint32_t u0 = 0; u0 < nwins; u0 += gu) {
+        const uint32_t s = set_of(u0 + (nwins - u0 < gu ? nwins - u0 : gu)) - set_of(u0);
+        if (s > gw) gw = s;
+    }
     const uint32_t TBg = gw * plan.nbuckets;                      // buckets of the largest group
-    size_t entries_g = set_cap * (size_t)gw;                      // most entries a group can hold
+    size_t entries_g = set_cap * (size_t)gu;                      // most entries a group can hold
     if (entries_g > max_entries) entries_g = max_entries;
     if (records && entries_g >= 0x7fffffffull) return (int)cudaErrorInvalidValue;      // record positions carry the sign in bit 31
     // small problems take the shuffle-based latency path (see k_bucket_reduce_warp)
@@ -1565,11 +1664,11 @@ int msm_core(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, co
                     const uint32_t* sc = (const uint32_t*)sg.d_scalars;
                     const size_t fl = flat ? table_n : 0;
                     if (pass == 0) {
-                        if (sg.mont) k_digits<false, true><<<grid, 256, 0, stream>>>(sc, sg.n, plan.c, plan.nwin, plan.nbuckets, hist, nullptr, fl, slot_base, sg.base0, d_flags);
-                        else k_digits<false, false><<<grid, 256, 0, stream>>>(sc, sg.n, plan.c, plan.nwin, plan.nbuckets, hist, nullptr, fl, slot_base, sg.base0, d_flags);
+                        if (sg.mont) k_digits<false, true><<<grid, 256, 0, stream>>>(sc, sg.n, plan.c, plan.c_top, plan.nwin, plan.nbuckets, hist, nullptr, fl, slot_base, sg.base0, d_flags);
+                        else k_digits<false, false><<<grid, 256, 0, stream>>>(sc, sg.n, plan.c, plan.c_top, plan.nwin, plan.nbuckets, hist, nullptr, fl, slot_base, sg.base0, d_flags);
                     } else {
-                        if (sg.mont) k_digits<true, true><<<grid, 256, 0, stream>>>(sc, sg.n, plan.c, plan.nwin, plan.nbuckets, cursors, sorted, fl, slot_base, sg.base0, d_flags);
-                        else k_digits<true, false><<<grid, 256, 0, stream>>>(sc, sg.n, plan.c, plan.nwin, plan.nbuckets, cursors, sorted, fl, slot_base, sg.base0, d_flags);
+                        if (sg.mont) k_digits<true, true><<<grid, 256, 0, stream>>>(sc, sg.n, plan.c, plan.c_top, plan.nwin, plan.nbuckets, cursors, sorted, fl, slot_base, sg.base0, d_flags);
+                        else k_digits<true, false><<<grid, 256, 0, stream>>>(sc, sg.n, plan.c, plan.c_top, plan.nwin, plan.nbuckets, cursors, sorted, fl, slot_base, sg.base0, d_flags);
                     }
                     count_launch();
                 }
@@ -1592,11 +1691,13 @@ int msm_core(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, co
                 at += bases[i].n;
             }
         }
-        for (uint32_t w0 = 0; w0 < nsets; w0 += gw) {
-            const uint32_t wn = nsets - w0 < gw ? nsets - w0 : gw;                                // bucket sets in this group
+        for (uint32_t u0 = 0; u0 < nwins; u0 += gu) {
+            const uint32_t un = nwins - u0 < gu ? nwins - u0 : gu;                                // windows in this group
+            const uint32_t w0 = set_of(u0), wn = set_of(u0 + un) - w0;                            // its bucket sets
             const uint32_t tb = wn * plan.nbuckets;
             const uint32_t* bs = bucket_start + (size_t)w0 * plan.nbuckets;                       // tb + 1 absolute offsets into `sorted`
-            size_t entries = set_cap * (size_t)wn;                                                // bound on the group's entries
+            const SetOffsets so = set_offsets(plan, flat, w0);
+            size_t entries = set_cap * (size_t)un;                                                // bound on the group's entries
             if (entries > max_entries) entries = max_entries;
             if (large_hot) CUDA_TRY(cudaMemsetAsync(hot_dev, 0, 4, stream));
             size_t items_bound = 1;                                                                // ≥ item count of any single bucket
@@ -1628,26 +1729,27 @@ int msm_core(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, co
                     for (int i = 0; i < nsegs; i++) {
                         const MsmSegment& sg = segs[i];
                         if (sg.n == 0) continue;
-                        // windows of this segment inside the group: its job's bucket sets are [job·sets, (job+1)·sets)
-                        const int64_t first = (int64_t)sg.job * sets_per_job;
+                        // windows of this segment inside the group: its job's windows are [job·wins, (job+1)·wins)
+                        const int64_t first = (int64_t)sg.job * wins_per_job;
                         int w_lo, w_hi;
                         if (flat) {                                                                   // one set per job: all windows or none
-                            if (first < (int64_t)w0 || first >= (int64_t)w0 + wn) continue;
+                            if (first < (int64_t)u0 || first >= (int64_t)u0 + un) continue;
                             w_lo = 0; w_hi = plan.nwin;
                         } else {
-                            const int64_t lo_w = (int64_t)w0 - first, hi_w = (int64_t)w0 + wn - first;
+                            const int64_t lo_w = (int64_t)u0 - first, hi_w = (int64_t)u0 + un - first;
                             w_lo = lo_w < 0 ? 0 : (int)lo_w; w_hi = hi_w > plan.nwin ? plan.nwin : (int)hi_w;
                             if (w_lo >= w_hi) continue;
                         }
                         const unsigned grid = (unsigned)((sg.n + 255) / 256);
                         const uint32_t slot_base = sg.job * sets_per_job * plan.nbuckets;
                         const uint32_t* sc = (const uint32_t*)sg.d_scalars;
+                        const int ct = plan.c_top, nw = plan.nwin;
                         if (flat) {
-                            if (sg.mont) k_scatter_records<true, true><<<grid, 256, 0, stream>>>(sc, sg.n, nullptr, 0, table, table_n, plan.c, plan.nbuckets, cursors, slot_base, w_lo, w_hi, bs, (uint4*)dense0);
-                            else k_scatter_records<false, true><<<grid, 256, 0, stream>>>(sc, sg.n, nullptr, 0, table, table_n, plan.c, plan.nbuckets, cursors, slot_base, w_lo, w_hi, bs, (uint4*)dense0);
+                            if (sg.mont) k_scatter_records<true, true><<<grid, 256, 0, stream>>>(sc, sg.n, nullptr, 0, table, table_n, plan.c, ct, nw, plan.nbuckets, cursors, slot_base, w_lo, w_hi, bs, (uint4*)dense0);
+                            else k_scatter_records<false, true><<<grid, 256, 0, stream>>>(sc, sg.n, nullptr, 0, table, table_n, plan.c, ct, nw, plan.nbuckets, cursors, slot_base, w_lo, w_hi, bs, (uint4*)dense0);
                         } else {
-                            if (sg.mont) k_scatter_records<true, false><<<grid, 256, 0, stream>>>(sc, sg.n, seg_points[i], seg_stride[i], nullptr, 0, plan.c, plan.nbuckets, cursors, slot_base, w_lo, w_hi, bs, (uint4*)dense0);
-                            else k_scatter_records<false, false><<<grid, 256, 0, stream>>>(sc, sg.n, seg_points[i], seg_stride[i], nullptr, 0, plan.c, plan.nbuckets, cursors, slot_base, w_lo, w_hi, bs, (uint4*)dense0);
+                            if (sg.mont) k_scatter_records<true, false><<<grid, 256, 0, stream>>>(sc, sg.n, seg_points[i], seg_stride[i], nullptr, 0, plan.c, ct, nw, plan.nbuckets, cursors, slot_base, w_lo, w_hi, bs, (uint4*)dense0);
+                            else k_scatter_records<false, false><<<grid, 256, 0, stream>>>(sc, sg.n, seg_points[i], seg_stride[i], nullptr, 0, plan.c, ct, nw, plan.nbuckets, cursors, slot_base, w_lo, w_hi, bs, (uint4*)dense0);
                         }
                         count_launch();
                     }
@@ -1769,14 +1871,14 @@ int msm_core(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, co
                     count_launch();
                     ent = red_b; m = groups; lgw += 3;
                 }
-                k_window_combine_quad<<<wn, 32u * ((m + 7u) / 8u), 0, stream>>>(ent, m, lgw, group_sums);
+                k_window_combine_quad<<<wn, 32u * ((m + 7u) / 8u), 0, stream>>>(ent, m, lgw, group_sums, so);
                 count_launch(2);
                 continue;
             }
             if (warp_reduce) {
                 const uint32_t wchunks = (plan.nbuckets + 31u) / 32u;
                 k_bucket_reduce_warp<<<(wn * wchunks * 32u + 127u) / 128u, 128, 0, stream>>>(final_partial, final_start, plan.nbuckets, wchunks, wn, red_a);
-                k_window_combine_warp<<<wn, 32, 0, stream>>>(red_a, wchunks, group_sums);
+                k_window_combine_warp<<<wn, 32, 0, stream>>>(red_a, wchunks, group_sums, so);
                 count_launch(2);
                 continue;
             }
@@ -1802,11 +1904,12 @@ int msm_core(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, co
                     uint32_t* done = other; other = (uint32_t*)ent; ent = done;
                     m = groups; lgw += 3;
                 }
-                k_window_combine_quad<<<wn, 32u * ((m + 7u) / 8u), 0, stream>>>(ent, m, lgw, group_sums);
+                k_window_combine_quad<<<wn, 32u * ((m + 7u) / 8u), 0, stream>>>(ent, m, lgw, group_sums, so);
                 count_launch();
                 continue;
             }
-            k_bucket_reduce<false><<<(nthreads + 127) / 128, 128, 0, stream>>>(final_partial, final_start, plan.nbuckets, chunk, chunks_per_set, wn, red_a);
+            k_bucket_reduce<false><<<(nthreads + 127) / 128, 128, 0, stream>>>(final_partial, final_start, plan.nbuckets, chunk, chunks_per_set, wn, red_a,
+                                                                                 nullptr, 0, so);
             count_launch(1);
             // tree over the per-chunk sums: groups of `tree` until one point per bucket set remains
             uint32_t per_row = chunks_per_set;
@@ -1843,17 +1946,18 @@ int msm_exclusive_scan(void* tmp, size_t tmp_bytes, const uint32_t* in, uint32_t
 }
 int msm_sort_indices(const MsmPlan& plan, const void* d_scalars, size_t n, int mont, uint32_t* hist, uint32_t* bucket_start, uint32_t* cursors,
                      uint32_t* sorted, void* cub_tmp, size_t cub_bytes, uint32_t* d_flags, cudaStream_t stream) {
+    if (plan.nsets != plan.nwin || plan.c_top != plan.c) return (int)cudaErrorInvalidValue;        // G2 takes the uniform plans
     const uint32_t TB = (uint32_t)plan.nwin * plan.nbuckets;
     int rc = (int)cudaMemsetAsync(hist, 0, (size_t)(TB + 1) * 4, stream);
     if (rc) return rc;
     const unsigned grid = (unsigned)((n + 255) / 256);
     const uint32_t* sc = (const uint32_t*)d_scalars;
-    if (mont) k_digits<false, true><<<grid, 256, 0, stream>>>(sc, n, plan.c, plan.nwin, plan.nbuckets, hist, nullptr, 0, 0u, 0u, d_flags);
-    else k_digits<false, false><<<grid, 256, 0, stream>>>(sc, n, plan.c, plan.nwin, plan.nbuckets, hist, nullptr, 0, 0u, 0u, d_flags);
+    if (mont) k_digits<false, true><<<grid, 256, 0, stream>>>(sc, n, plan.c, plan.c_top, plan.nwin, plan.nbuckets, hist, nullptr, 0, 0u, 0u, d_flags);
+    else k_digits<false, false><<<grid, 256, 0, stream>>>(sc, n, plan.c, plan.c_top, plan.nwin, plan.nbuckets, hist, nullptr, 0, 0u, 0u, d_flags);
     if ((rc = msm_exclusive_scan(cub_tmp, cub_bytes, hist, bucket_start, (size_t)TB + 1, stream)) != 0) return rc;
     if ((rc = (int)cudaMemcpyAsync(cursors, bucket_start, (size_t)(TB + 1) * 4, cudaMemcpyDeviceToDevice, stream)) != 0) return rc;
-    if (mont) k_digits<true, true><<<grid, 256, 0, stream>>>(sc, n, plan.c, plan.nwin, plan.nbuckets, cursors, sorted, 0, 0u, 0u, d_flags);
-    else k_digits<true, false><<<grid, 256, 0, stream>>>(sc, n, plan.c, plan.nwin, plan.nbuckets, cursors, sorted, 0, 0u, 0u, d_flags);
+    if (mont) k_digits<true, true><<<grid, 256, 0, stream>>>(sc, n, plan.c, plan.c_top, plan.nwin, plan.nbuckets, cursors, sorted, 0, 0u, 0u, d_flags);
+    else k_digits<true, false><<<grid, 256, 0, stream>>>(sc, n, plan.c, plan.c_top, plan.nwin, plan.nbuckets, cursors, sorted, 0, 0u, 0u, d_flags);
     count_launch(3);
     return (int)cudaGetLastError();
 }
@@ -1885,6 +1989,8 @@ MsmPlan msm_make_plan_precomputed(size_t npoints) {
     p.c = c;
     p.nwin = 253 / c + 1;
     p.nbuckets = 1u << (c - 1);
+    p.c_top = c;
+    p.nsets = p.nwin;
     size_t total = npoints * (size_t)p.nwin;
     size_t cap = total / 300000 + 1;
     if (cap < 16) cap = 16;

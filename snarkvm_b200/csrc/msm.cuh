@@ -24,15 +24,31 @@
 
 namespace b200 {
 
+// Window layout: windows 0 … nwin−2 have c bits each, the top window (bits (nwin−1)·c …) has c_top bits.  Every window is a
+// signed-digit window (digit ∈ [−2^(w−1), 2^(w−1)] for a w-bit window, the carry passed upwards); the top window is wide
+// enough that a scalar below 2^253 never makes its digit negative, so no carry leaves it.  A window's buckets are cut into
+// bucket SETS of nbuckets = 2^(c−1) buckets: one set per window below the top, top_sets() = 2^(c_top−1) / nbuckets for the top
+// window, whose set k holds the digits k·nbuckets + 1 … (k+1)·nbuckets (its window sum carries the k·nbuckets offset).
+// The uniform plans are c_top = c, nsets = nwin (nwin = 253 / c + 1).
 struct MsmPlan {
-    int c;              // window bits
-    int nwin;           // number of windows = 253 / c + 1 (room for the signed-digit carry)
-    uint32_t nbuckets;  // 2^(c-1) buckets per window (bucket value 1 .. 2^(c-1))
+    int c;              // bits of every window but the top one
+    int nwin;           // number of windows
+    uint32_t nbuckets;  // 2^(c-1) buckets per bucket set (bucket value 1 .. 2^(c-1))
     uint32_t cap;       // max points per work item
     int levels;         // batched-affine pair levels run before the XYZZ accumulation (0 = gather + XYZZ only)
+    int c_top;          // bits of the top window (= c in the uniform plans)
+    int nsets;          // bucket sets per sum: nwin − 1 + top_sets()
+
+    int top_sets() const { return nsets - nwin + 1; }
+    int window_bit(int w) const { return w * c; }                                        // first scalar bit of window w
+    int window_bits(int w) const { return w == nwin - 1 ? c_top : c; }
+    uint32_t window_buckets(int w) const { return 1u << (window_bits(w) - 1); }          // largest digit magnitude
+    int window_first_set(int w) const { return w; }                                      // its sets are contiguous from here
+    uint32_t set_digit_offset(int s) const { return s >= nwin ? (uint32_t)(s - nwin + 1) * nbuckets : 0u; }
 };
 
-MsmPlan msm_make_plan(size_t npoints);
+// mixed = false: always a uniform plan (the sharded window-sum calls, whose callers fold the sums as Σ 2^{c·w}·S_w, and G2)
+MsmPlan msm_make_plan(size_t npoints, bool mixed = true);
 MsmPlan msm_make_plan_batch(size_t max_n, size_t total_n);
 
 // One MSM call = `njobs` independent sums over one resident base set.
