@@ -222,6 +222,22 @@ SNARKVM_API int snarkvm_b200_csr_transpose_device(void* d_t_row_ptr, void* d_t_c
 /* DensePolynomial::evaluate (fft/polynomial/dense.rs:98-114): out = sum c_i * point^i; out and point are 32-byte HOST buffers. */
 SNARKVM_API int snarkvm_b200_poly_evaluate_device(void* out_mont_host, const void* d_coeffs, size_t m, const void* point_mont_host,
                                                   void* stream);
+/* The circuit id's byte stream of one CSR matrix (Circuit::hash, snark/varuna/ahp/indexer/circuit.rs:109-121, which feeds it to
+ * Blake2s): serialize_uncompressed of Vec<Vec<(Fr, usize)>> — [u64 nrows] then per row [u64 len][len x (32 B canonical LE value,
+ * u64 LE column)] — written to d_out (out_bytes = 8 + 8 * nrows + 40 * nnz, 8-byte aligned).  Same CSR layout as
+ * snarkvm_b200_varuna_matrix_evals_device.  A wrong out_bytes, nnz > 0 with no rows or a misaligned d_out return cudaErrorInvalidValue
+ * before any launch; a row_ptr that is not non-decreasing from 0 to nnz returns cudaErrorInvalidValue after the pass.  Synchronises. */
+SNARKVM_API int snarkvm_b200_csr_serialize_device(void* d_out, size_t out_bytes, const void* d_row_ptr, size_t nrows, const void* d_cols,
+                                                  const void* d_vals, size_t nnz, void* stream);
+/* d_out (n Montgomery Fr) = sum_j c_j * p_j over nterms <= 12 polynomials of different lengths, in one pass (the `+= (c, &p)` sequence
+ * of LinearCombination polynomials, bit for bit).  d_polys, lens and coeffs_mont_host (nterms x 32 B) are HOST arrays; lens[j] <= n.
+ * nterms > 12 or lens[j] > n return cudaErrorInvalidValue before any launch. */
+SNARKVM_API int snarkvm_b200_fr_lincomb_device(void* d_out, size_t n, const void* const* d_polys, const size_t* lens, const void* coeffs_mont_host,
+                                               uint32_t nterms, void* stream);
+/* MatrixEvals::evaluate (snark/varuna/ahp/matrices.rs:114-126): out_mont_host (4 x 32 B HOST) = sum l*row, sum l*col, sum l*row*col,
+ * sum l*row_col_val over n Montgomery Fr in HBM, l being the Lagrange coefficients of K at a point.  Synchronises the stream. */
+SNARKVM_API int snarkvm_b200_matrix_evals_dot_device(void* out_mont_host, const void* d_row, const void* d_col, const void* d_row_col_val,
+                                                     const void* d_lagrange, size_t n, void* stream);
 
 /* Fr Montgomery <-> canonical, n elements in HBM (to_bigint / from_bigint, fields/src/fp_256.rs:362-413). */
 SNARKVM_API int snarkvm_b200_fr_from_mont_device(void* d_out, const void* d_in, size_t n, void* stream);

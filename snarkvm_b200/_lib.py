@@ -33,6 +33,7 @@ SYMBOLS = (
     "snarkvm_b200_sonic_commit_batch_device", "snarkvm_b200_generator_mul_device", "snarkvm_b200_selftest_host_copy",
     "snarkvm_b200_test_field_op_device", "snarkvm_b200_test_curve_op_device", "snarkvm_b200_test_field_op_host",
     "snarkvm_b200_varuna_matrix_evals_device", "snarkvm_b200_csr_transpose_device",
+    "snarkvm_b200_csr_serialize_device", "snarkvm_b200_fr_lincomb_device", "snarkvm_b200_matrix_evals_dot_device",
 )
 
 
@@ -113,6 +114,9 @@ def lib():
     L.snarkvm_b200_domain_elements_device.argtypes = [vp, u32, vp]
     L.snarkvm_b200_varuna_matrix_evals_device.argtypes = [vp, vp, vp, vp, sz, vp, vp, sz, sz, sz, u32, u32, u32, vp]
     L.snarkvm_b200_csr_transpose_device.argtypes = [vp, vp, vp, vp, sz, vp, vp, sz, sz, sz, u32, vp]
+    L.snarkvm_b200_csr_serialize_device.argtypes = [vp, sz, vp, sz, vp, vp, sz, vp]
+    L.snarkvm_b200_fr_lincomb_device.argtypes = [vp, sz, vp, vp, vp, u32, vp]
+    L.snarkvm_b200_matrix_evals_dot_device.argtypes = [vp, vp, vp, vp, vp, sz, vp]
     L.snarkvm_b200_msm_batch_device.argtypes = [vp, vp, sz, vp, vp, sz, vp]
     L.snarkvm_b200_msm_window_sums_plan_device.argtypes = [vp, vp, sz, vp, sz, vp, sz, vp]
     L.snarkvm_b200_kzg_commit_batch_hiding_device.argtypes = [vp, vp, sz, vp, vp, vp, vp, vp, sz, vp]

@@ -1167,6 +1167,18 @@ int snarkvm_b200_csr_transpose_device(void* d_t_row_ptr, void* d_t_cols, void* d
 int snarkvm_b200_poly_evaluate_device(void* out_mont_host, const void* d_coeffs, size_t m, const void* point_mont_host, void* stream) {
     return poly_evaluate_device(out_mont_host, d_coeffs, m, point_mont_host, (cudaStream_t)stream);
 }
+int snarkvm_b200_csr_serialize_device(void* d_out, size_t out_bytes, const void* d_row_ptr, size_t nrows, const void* d_cols,
+                                      const void* d_vals, size_t nnz, void* stream) {
+    return csr_serialize_device(d_out, out_bytes, d_row_ptr, nrows, d_cols, d_vals, nnz, (cudaStream_t)stream);
+}
+int snarkvm_b200_fr_lincomb_device(void* d_out, size_t n, const void* const* d_polys, const size_t* lens, const void* coeffs_mont_host,
+                                   uint32_t nterms, void* stream) {
+    return fr_lincomb_device(d_out, n, d_polys, lens, coeffs_mont_host, nterms, (cudaStream_t)stream);
+}
+int snarkvm_b200_matrix_evals_dot_device(void* out_mont_host, const void* d_row, const void* d_col, const void* d_row_col_val,
+                                         const void* d_lagrange, size_t n, void* stream) {
+    return matrix_evals_dot_device(out_mont_host, d_row, d_col, d_row_col_val, d_lagrange, n, (cudaStream_t)stream);
+}
 
 int snarkvm_b200_fr_from_mont_device(void* d_out, const void* d_in, size_t n, void* stream) {
     return fr_from_mont_device(d_out, d_in, n, (cudaStream_t)stream);

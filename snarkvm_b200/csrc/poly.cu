@@ -6,6 +6,9 @@
 //   poly_divide_by_vanishing_device    — fft/polynomial/dense.rs:162-169 → fft/polynomial/mod.rs:222-256 with the
 //                                        divisor x^n − 1
 //   poly_evaluate_device               — DensePolynomial::evaluate (fft/polynomial/dense.rs:98-114)
+//   csr_serialize_device               — the circuit id's byte stream (snark/varuna/ahp/indexer/circuit.rs:109-121)
+//   fr_lincomb_device                  — a LinearCombination of polynomials in one pass (snark/varuna/varuna.rs:256-272)
+//   matrix_evals_dot_device            — MatrixEvals::evaluate (snark/varuna/ahp/matrices.rs:114-126)
 //
 // Every result is a canonical Fr value, so any correct evaluation order is bit-identical to the reference's.
 #include "poly.cuh"
@@ -170,8 +173,11 @@ __global__ void __launch_bounds__(EVAL_THREADS) k_poly_eval_partial(const uint32
     Fr s = cta_sum(acc, reinterpret_cast<uint32_t*>(sh4));
     if (threadIdx.x == 0) s.store(partial + (size_t)blockIdx.x * 8);
 }
+// CTA b adds in[b·count … (b + 1)·count) into out[b]: one CTA per row of partials
 __global__ void __launch_bounds__(EVAL_THREADS) k_fr_sum(const uint32_t* __restrict__ in, size_t count, uint32_t* __restrict__ out) {
     __shared__ uint4 sh4[EVAL_THREADS * 2];
+    in += (size_t)blockIdx.x * count * 8;
+    out += (size_t)blockIdx.x * 8;
     Fr acc = Fr::zero();
     for (size_t i = threadIdx.x; i < count; i += EVAL_THREADS) acc = acc + Fr::load_ldg(in + i * 8);
     Fr s = cta_sum(acc, reinterpret_cast<uint32_t*>(sh4));
@@ -659,6 +665,149 @@ int csr_transpose_device(void* d_t_row_ptr, void* d_t_cols, void* d_t_vals, cons
         if (rc == 0) rc = (int)cudaGetLastError();
     }
     return csr_finish(rc, scratch, bad, stream);
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// The circuit id's byte stream (Circuit::hash, snark/varuna/ahp/indexer/circuit.rs:109-121): a Matrix = Vec<Vec<(Fr, usize)>>
+// through serialize_uncompressed (utilities/src/serialize/impls.rs: u64 LE length prefixes, usize as u64 LE; Fr as its 32 LE
+// canonical bytes with empty flags, fields/src/macros.rs:190-245):
+//     [u64 nrows] then, per row r, [u64 len_r][len_r × (32 B value, u64 column)]
+// Row r's header sits at 8 + 8·r + 40·row_ptr[r] and entry e of row r at 16 + 8·r + 40·e, so every thread knows its address: one
+// thread per entry (Montgomery → canonical fused in) and one per row header.  A row_ptr that is not non-decreasing from 0 to nnz
+// raises the bad flag; its row header is then not written, and no thread writes outside the 8 + 8·nrows + 40·nnz bytes.
+// ---------------------------------------------------------------------------------------------------------------------
+__global__ void k_csr_serialize(CsrArgs m, uint8_t* __restrict__ out, int* __restrict__ bad) {
+    const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    csr_check_bounds(m, bad);
+    if (t < m.nnz) {
+        const uint32_t e = (uint32_t)t, r = csr_row_of(m.row_ptr, m.nrows, e);
+        uint64_t* dst = reinterpret_cast<uint64_t*>(out + 16 + 8 * (size_t)r + 40 * (size_t)e);
+        const Fr v = Fr::load_ldg(m.vals + (size_t)e * 8).from_mont();
+#pragma unroll
+        for (int i = 0; i < 4; i++) dst[i] = (uint64_t)v.v[2 * i] | (uint64_t)v.v[2 * i + 1] << 32;
+        dst[4] = __ldg(m.cols + e);
+    } else if (t < (size_t)m.nnz + m.nrows) {
+        const uint32_t r = (uint32_t)(t - m.nnz), e0 = __ldg(m.row_ptr + r), e1 = __ldg(m.row_ptr + r + 1);
+        if (e0 > e1 || e1 > m.nnz) { *bad = 1; return; }
+        *reinterpret_cast<uint64_t*>(out + 8 + 8 * (size_t)r + 40 * (size_t)e0) = e1 - e0;
+    } else if (t == (size_t)m.nnz + m.nrows) {
+        *reinterpret_cast<uint64_t*>(out) = m.nrows;
+    }
+}
+
+int csr_serialize_device(void* d_out, size_t out_bytes, const void* d_row_ptr, size_t nrows, const void* d_cols, const void* d_vals, size_t nnz,
+                         cudaStream_t stream) {
+    if (!d_out || !d_row_ptr || (nnz && (!d_cols || !d_vals))) return (int)cudaErrorInvalidValue;
+    if (nrows >= ((size_t)1 << 32) || nnz >= ((size_t)1 << 32) || out_bytes != 8 + 8 * nrows + 40 * nnz) return (int)cudaErrorInvalidValue;
+    if ((nnz && !nrows) || ((uintptr_t)d_out & 7)) return (int)cudaErrorInvalidValue;
+    const CsrArgs m{(const uint32_t*)d_row_ptr, (const uint32_t*)d_cols, (const uint32_t*)d_vals, (uint32_t)nrows, (uint32_t)nnz, 0, 0, 0};
+    uint8_t* scratch = nullptr;
+    cudaError_t e = pool_alloc(&scratch, 256, stream);
+    if (e != cudaSuccess) return (int)e;
+    int* bad = (int*)scratch;
+    int rc = (int)cudaMemsetAsync(bad, 0, sizeof(int), stream);
+    if (rc == 0) {
+        const size_t threads = nnz + nrows + 1;
+        k_csr_serialize<<<(unsigned)((threads + 255) / 256), 256, 0, stream>>>(m, (uint8_t*)d_out, bad);
+        count_launch();
+        rc = (int)cudaGetLastError();
+    }
+    return csr_finish(rc, scratch, bad, stream);
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// out = Σ_j c_j·p_j over up to LINCOMB_MAX polynomials of different lengths in one pass: each output coefficient is read-modified
+// once instead of once per term (the poly_axpy loop).  A term whose coefficient is one adds p_j without the product; zero
+// coefficients and empty terms are dropped on the host.  Field sums are exact, so the result is the axpy sequence's bit for bit.
+// ---------------------------------------------------------------------------------------------------------------------
+static constexpr int LINCOMB_MAX = 12;
+struct LincombArgs {
+    const uint32_t* p[LINCOMB_MAX];
+    uint64_t len[LINCOMB_MAX];
+    FrArg c[LINCOMB_MAX];
+    uint32_t nterms;
+};
+__global__ void k_fr_lincomb(uint32_t* __restrict__ out, size_t n, LincombArgs a) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    Fr acc = Fr::zero();
+    for (uint32_t j = 0; j < a.nterms; j++) {
+        if (i >= a.len[j]) continue;
+        const Fr x = Fr::load_ldg(a.p[j] + i * 8), c = fr_from_arg(a.c[j]);
+        acc = acc + (c == Fr::one() ? x : c * x);
+    }
+    acc.store(out + i * 8);
+}
+
+int fr_lincomb_device(void* d_out, size_t n, const void* const* d_polys, const size_t* lens, const void* coeffs_mont_host, uint32_t nterms,
+                      cudaStream_t stream) {
+    if (nterms > LINCOMB_MAX || (nterms && (!d_polys || !lens || !coeffs_mont_host))) return (int)cudaErrorInvalidValue;
+    if (n && !d_out) return (int)cudaErrorInvalidValue;
+    LincombArgs a{};
+    for (uint32_t j = 0; j < nterms; j++) {
+        if (lens[j] > n || (lens[j] && !d_polys[j])) return (int)cudaErrorInvalidValue;
+        FrArg c;
+        memcpy(c.v, (const uint8_t*)coeffs_mont_host + 32 * (size_t)j, 32);
+        bool zero = true;
+        for (int k = 0; k < 8; k++) zero &= c.v[k] == 0;
+        if (lens[j] == 0 || zero) continue;
+        a.p[a.nterms] = (const uint32_t*)d_polys[j];
+        a.len[a.nterms] = lens[j];
+        a.c[a.nterms] = c;
+        a.nterms++;
+    }
+    if (n == 0) return 0;
+    k_fr_lincomb<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>((uint32_t*)d_out, n, a);
+    count_launch();
+    return (int)cudaGetLastError();
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// MatrixEvals::evaluate (snark/varuna/ahp/matrices.rs:114-126): with the Lagrange coefficients l of K at a point, the four inner
+// products Σ l·row, Σ l·col, Σ l·row·col, Σ l·row_col_val — the matrix's four index polynomials at that point.  row·col is formed
+// on the fly (the device index keeps no row_col vector).  Stage 1: one launch over the whole matrix, grid-stride, every CTA
+// reduces its four partials in shared memory; stage 2: one CTA per product adds the per-CTA partials.
+// ---------------------------------------------------------------------------------------------------------------------
+static constexpr unsigned DOT_MAX_CTAS = 1024;
+__global__ void __launch_bounds__(EVAL_THREADS) k_matrix_evals_dot(const uint32_t* __restrict__ row, const uint32_t* __restrict__ col,
+                                                                    const uint32_t* __restrict__ rcv, const uint32_t* __restrict__ lag,
+                                                                    size_t n, uint32_t* __restrict__ partial /* [4][gridDim.x] */) {
+    __shared__ uint4 sh4[EVAL_THREADS * 2];
+    Fr s[4] = {Fr::zero(), Fr::zero(), Fr::zero(), Fr::zero()};
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+        const Fr l = Fr::load_ldg(lag + i * 8), lr = l * Fr::load_ldg(row + i * 8), c = Fr::load_ldg(col + i * 8);
+        s[0] = s[0] + lr;
+        s[1] = s[1] + l * c;
+        s[2] = s[2] + lr * c;
+        s[3] = s[3] + l * Fr::load_ldg(rcv + i * 8);
+    }
+#pragma unroll
+    for (int k = 0; k < 4; k++) {
+        const Fr t = cta_sum(s[k], reinterpret_cast<uint32_t*>(sh4));
+        if (threadIdx.x == 0) t.store(partial + ((size_t)k * gridDim.x + blockIdx.x) * 8);
+        __syncthreads();
+    }
+}
+
+int matrix_evals_dot_device(void* out_mont_host, const void* d_row, const void* d_col, const void* d_row_col_val, const void* d_lagrange,
+                            size_t n, cudaStream_t stream) {
+    if (!out_mont_host) return (int)cudaErrorInvalidValue;
+    if (n == 0) { memset(out_mont_host, 0, 4 * 32); return 0; }
+    if (!d_row || !d_col || !d_row_col_val || !d_lagrange) return (int)cudaErrorInvalidValue;
+    size_t blocks = (n + EVAL_THREADS - 1) / EVAL_THREADS;
+    if (blocks > DOT_MAX_CTAS) blocks = DOT_MAX_CTAS;
+    uint32_t* scratch = nullptr;                             // partials [4][blocks], then the four sums
+    cudaError_t e = pool_alloc(&scratch, (4 * blocks + 4) * 32, stream);
+    if (e != cudaSuccess) return (int)e;
+    k_matrix_evals_dot<<<(unsigned)blocks, EVAL_THREADS, 0, stream>>>((const uint32_t*)d_row, (const uint32_t*)d_col,
+                                                                      (const uint32_t*)d_row_col_val, (const uint32_t*)d_lagrange, n, scratch);
+    k_fr_sum<<<4, EVAL_THREADS, 0, stream>>>(scratch, blocks, scratch + 4 * blocks * 8);
+    count_launch(2);
+    int rc = (int)cudaGetLastError();
+    if (rc == 0) rc = (int)cudaMemcpyAsync(out_mont_host, scratch + 4 * blocks * 8, 4 * 32, cudaMemcpyDeviceToHost, stream);
+    cudaFreeAsync(scratch, stream);
+    if (rc == 0) rc = (int)cudaStreamSynchronize(stream);
+    return rc;
 }
 
 }  // namespace b200

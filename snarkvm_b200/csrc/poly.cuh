@@ -41,6 +41,20 @@ int varuna_matrix_evals_device(void* d_row, void* d_col, void* d_row_col_val, co
 int csr_transpose_device(void* d_t_row_ptr, void* d_t_cols, void* d_t_vals, const void* d_row_ptr, size_t nrows, const void* d_cols,
                          const void* d_vals, size_t nnz, size_t nvars, size_t input_size, uint32_t lg_variable, cudaStream_t stream);
 
+// The circuit id's byte stream of a CSR matrix (Circuit::hash, ahp/indexer/circuit.rs:109-121): serialize_uncompressed of
+// Vec<Vec<(Fr, usize)>> — [u64 nrows], per row [u64 len][len × (32 B canonical value, u64 column)] — into out_bytes = 8 + 8·nrows +
+// 40·nnz bytes of HBM (8-byte aligned).  A row_ptr not non-decreasing from 0 to nnz returns cudaErrorInvalidValue.  Synchronises.
+int csr_serialize_device(void* d_out, size_t out_bytes, const void* d_row_ptr, size_t nrows, const void* d_cols, const void* d_vals, size_t nnz,
+                         cudaStream_t stream);
+// out (n Montgomery Fr) = Σ_j c_j·p_j for nterms ≤ 12 polynomials: d_polys / lens / coeffs are HOST arrays (device pointers,
+// lengths ≤ n, 32-byte Montgomery coefficients); coefficients past a polynomial's length count as zero
+int fr_lincomb_device(void* d_out, size_t n, const void* const* d_polys, const size_t* lens, const void* coeffs_mont_host, uint32_t nterms,
+                      cudaStream_t stream);
+// MatrixEvals::evaluate (ahp/matrices.rs:114-126): out (4 × 32 B Montgomery, HOST) = Σ l·row, Σ l·col, Σ l·row·col, Σ l·row_col_val
+// over n elements; synchronises the stream
+int matrix_evals_dot_device(void* out_mont_host, const void* d_row, const void* d_col, const void* d_row_col_val, const void* d_lagrange,
+                            size_t n, cudaStream_t stream);
+
 // Group FFT over G1 (DomainCoeff = G1Projective, fft/domain.rs:169-221 generic path): n = 2^lg affine points in, affine points
 // out (natural order both sides).  direction 1 = inverse (includes n^{-1}): UniversalParams::lagrange_basis
 // (polycommit/kzg10/data_structures.rs:68-72).

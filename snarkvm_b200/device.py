@@ -432,6 +432,56 @@ def csr_transpose(row_ptr: torch.Tensor, cols: torch.Tensor, vals: torch.Tensor,
     return t_row_ptr, t_cols, t_vals
 
 
+def csr_serialize(row_ptr: torch.Tensor, cols: torch.Tensor, vals: torch.Tensor) -> torch.Tensor:
+    """The circuit id's byte stream of one CSR matrix (Circuit::hash, snark/varuna/ahp/indexer/circuit.rs:109-121):
+    serialize_uncompressed of Vec<Vec<(Fr, usize)>> → CUDA uint8 tensor of 8 + 8·nrows + 40·nnz bytes.  A row_ptr that is not
+    non-decreasing from 0 to nnz raises CudaError."""
+    rp, nrows, cp, vp, nnz = _csr_args(row_ptr, cols, vals)
+    nbytes = 8 + 8 * nrows + 40 * nnz
+    out = torch.empty(nbytes // 8, dtype=torch.int64, device=row_ptr.device)          # int64 storage: 8-byte aligned
+    with torch.cuda.device(row_ptr.device):
+        _lib.check(_lib.lib().snarkvm_b200_csr_serialize_device(out.data_ptr(), nbytes, rp, nrows, cp, vp, nnz, _stream()))
+    return out.view(torch.uint8)
+
+
+LINCOMB_MAX_TERMS = 12
+
+
+def fr_lincomb(polys: list, coeffs_mont: list) -> torch.Tensor:
+    """Σ_j coeffs_j·polys_j in one pass over up to 12 Montgomery coefficient tensors of different lengths → CUDA tensor
+    [max length, 4] i64, bit-identical to the `poly_axpy` sequence (sonic_pc.py)"""
+    if len(polys) != len(coeffs_mont) or not polys:
+        raise ValueError("one coefficient per polynomial, at least one polynomial")
+    if len(polys) > LINCOMB_MAX_TERMS:
+        raise ValueError(f"at most {LINCOMB_MAX_TERMS} polynomials")
+    lens = [_nbytes(p) // 32 for p in polys]
+    n = max(lens)
+    dev = polys[0].device
+    out = torch.empty((n, 4), dtype=torch.int64, device=dev)
+    k = len(polys)
+    ptrs = (ctypes.c_void_p * k)(*[(_check(p, "poly") if m else None) for p, m in zip(polys, lens)])
+    szs = (ctypes.c_size_t * k)(*lens)
+    cs = np.ascontiguousarray(np.stack([_fr_host(c) for c in coeffs_mont]))
+    with torch.cuda.device(dev):
+        _lib.check(_lib.lib().snarkvm_b200_fr_lincomb_device(out.data_ptr() if n else None, n, ctypes.cast(ptrs, ctypes.c_void_p),
+                                                              ctypes.cast(szs, ctypes.c_void_p), cs.ctypes.data, k, _stream()))
+    return out
+
+
+def matrix_evals_dot(row: torch.Tensor, col: torch.Tensor, row_col_val: torch.Tensor, lagrange: torch.Tensor) -> np.ndarray:
+    """MatrixEvals::evaluate (snark/varuna/ahp/matrices.rs:114-126): Σ l·row, Σ l·col, Σ l·row·col, Σ l·row_col_val over K →
+    uint64[4, 4] Montgomery on the host"""
+    n = _nbytes(lagrange) // 32
+    for t in (row, col, row_col_val):
+        if _nbytes(t) != n * 32:
+            raise ValueError("length mismatch")
+    out = np.zeros((4, 4), dtype=np.uint64)
+    with torch.cuda.device(lagrange.device):
+        args = [_check(t, name) if n else None for t, name in ((row, "row"), (col, "col"), (row_col_val, "row_col_val"), (lagrange, "lagrange"))]
+        _lib.check(_lib.lib().snarkvm_b200_matrix_evals_dot_device(out.ctypes.data, *args, n, _stream()))
+    return out
+
+
 def poly_divide_by_linear(p: torch.Tensor, point_mont) -> torch.Tensor:
     """Quotient of p / (x − point), the KZG witness polynomial (kzg10/mod.rs:220-241) → CUDA tensor [m − 1, 4] i64, not trimmed."""
     z = _fr_host(point_mont)

@@ -6,6 +6,10 @@ bulk field arithmetic — the five `AHPForR1CS::prover_*_round` functions and th
     ahp/indexer/indexer.rs:121-200, ahp/matrices.rs:138-195, 249-270   Circuit            (domains, row / col / row_col_val on K, transposes)
     ahp/matrices.rs:211-240                        Circuit.index_polynomials (MatrixArithmetization::new)
     varuna.rs:72-134, 226-233                      circuit_setup        (the verifying key's twelve index commitments)
+    ahp/indexer/circuit.rs:109-121                 Circuit.id           (Blake2s of the index counts and the serialized matrices)
+    varuna.rs:236-276                              prove_vk             (the verifying-key certificate)
+    ahp/indexer/indexer.rs:232-260                 Circuit.evaluate_index_polynomials
+    varuna.rs:280-331                              verify_vk            (up to the final pairing)
     ahp/prover/round_functions/mod.rs:43-192, ahp/prover/state.rs:107-178   init_prover   (z_A, z_B, z_C by sparse mat-vec, x_poly)
     ahp/prover/round_functions/first.rs:129-160    prover_first_round   (w)
     ahp/prover/round_functions/third.rs:207-234    calculate_assignments (z)
@@ -24,6 +28,8 @@ Polynomials are CUDA tensors [m, 4] int64 (Montgomery Fr, low degree first, NOT 
 """
 from __future__ import annotations
 
+import hashlib
+import struct
 from dataclasses import dataclass
 
 import numpy as np
@@ -138,6 +144,12 @@ class Matrix:
         m.row_ptr, m.cols, m.vals = row_ptr, cols, vals
         return m
 
+    def serialize(self) -> torch.Tensor:
+        """the matrix's part of the circuit id's byte stream (serialize_uncompressed of Vec<Vec<(Fr, usize)>>), built on the device
+        → CUDA uint8 tensor of 8 + 8·nrows + 40·nnz bytes.  It equals the reference's bytes when every row holds its entries as
+        into_matrix_helper leaves them (ahp/matrices.rs:39-63): columns increasing, no repeats, no zero values."""
+        return device.csr_serialize(self.row_ptr, self.cols, self.vals)
+
 
 class MatrixEvals:
     """ahp/matrices.rs:102-136: row, col, row_col_val evaluations on the non-zero domain K"""
@@ -172,6 +184,11 @@ class CircuitInfo:
         """AHPForR1CS::get_degree_bounds (ahp/ahp.rs:110-121): the bounds of g_1, g_a, g_b, g_c"""
         return [_domain_size(n) - 2 for n in (self.num_public_and_private_variables, self.num_non_zero_a, self.num_non_zero_b,
                                                self.num_non_zero_c)]
+
+    def to_bytes_le(self) -> bytes:
+        """the six counts as u64 LE (ToBytes, circuit_info.rs:49-58; the derived serialize_uncompressed writes the same bytes)"""
+        return struct.pack("<6Q", self.num_public_inputs, self.num_public_and_private_variables, self.num_constraints,
+                           self.num_non_zero_a, self.num_non_zero_b, self.num_non_zero_c)
 
 
 # the twelve index polynomials in the order of their labels circuit_{id}_{name}_{matrix} sorted as strings (varuna.rs:116), which
@@ -218,13 +235,43 @@ class Circuit:
             out[f"row_col_val_{m}"] = K.ifft(arith.row_col_val)
         return {name: out[name] for name in INDEX_POLYNOMIAL_NAMES}
 
+    def id(self) -> bytes:
+        """Circuit::hash (ahp/indexer/circuit.rs:109-121): Blake2s-256 of CircuitInfo and of A, B, C serialized uncompressed.  Each
+        matrix's stream is built on the device and fed to the hash on its own (no single host blob).  Computed once, then cached."""
+        if self._id is None:
+            h = hashlib.blake2s(digest_size=32)
+            h.update(self.info.to_bytes_le())
+            for m in (self.a, self.b, self.c):
+                h.update(m.serialize().cpu().numpy().data)
+            self._id = h.digest()
+        return self._id
+
+    _id = None
+
+    def evaluate_index_polynomials(self, point: int, combiners) -> int:
+        """AHPForR1CS::evaluate_index_polynomials (ahp/indexer/indexer.rs:232-260): Σ_i combiners_i·p_i(point) over the twelve index
+        polynomials in INDEX_POLYNOMIAL_NAMES (= label) order, from their evaluations on K through the Lagrange coefficients of each
+        matrix's K at the point (a point inside K included, fft/domain.rs:258-292); no polynomial is interpolated."""
+        combiners = [int(c) % R_MOD for c in combiners]
+        if len(combiners) != len(INDEX_POLYNOMIAL_NAMES):
+            raise ValueError(f"{len(combiners)} combiners for {len(INDEX_POLYNOMIAL_NAMES)} index polynomials")
+        evals = {}
+        dev = self.a.row_ptr.device
+        for m, arith in zip("abc", self.ariths):
+            lag = arith.domain.evaluate_all_lagrange_coefficients(point, dev)
+            dots = device.matrix_evals_dot(arith.row, arith.col, arith.row_col_val, lag)
+            for name, v in zip(("row", "col", "row_col", "row_col_val"), dots):
+                evals[f"{name}_{m}"] = _fr_mont_to_int(v)
+        return sum(c * evals[name] for c, name in zip(combiners, INDEX_POLYNOMIAL_NAMES)) % R_MOD
+
 
 @dataclass
 class CircuitVerifyingKey:
-    """snark/varuna/data_structures/circuit_verifying_key.rs without the circuit id: the index counts and the twelve index commitments
-    (normalised projective uint64[12, 18]) in INDEX_POLYNOMIAL_NAMES order"""
+    """snark/varuna/data_structures/circuit_verifying_key.rs: the index counts, the twelve index commitments (normalised projective
+    uint64[12, 18]) in INDEX_POLYNOMIAL_NAMES order and the circuit id (Circuit.id(), 32 bytes; None when setup was not asked for it)"""
     circuit_info: CircuitInfo
     circuit_commitments: np.ndarray
+    id: bytes | None = None
 
 
 @dataclass
@@ -235,10 +282,12 @@ class CircuitProvingKey:
     committer_key: object
 
 
-def circuit_setup(circuit: Circuit, pp_powers_of_beta_g: torch.Tensor, pp_powers_of_beta_times_gamma_g: torch.Tensor, zk: bool = False):
+def circuit_setup(circuit: Circuit, pp_powers_of_beta_g: torch.Tensor, pp_powers_of_beta_times_gamma_g: torch.Tensor, zk: bool = False,
+                  with_id: bool = False):
     """VarunaSNARK::circuit_setup → batch_circuit_setup for one circuit (varuna.rs:72-134, 226-233): trim the universal parameters to
     the circuit's max_degree and degree bounds, commit the twelve index polynomials in ONE pass (no degree bound, no hiding) and return
-    (CircuitProvingKey, CircuitVerifyingKey).  The SRS is (β^i·G, γβ^i·G) as sonic_pc.CommitterKey.trim takes it."""
+    (CircuitProvingKey, CircuitVerifyingKey).  The SRS is (β^i·G, γβ^i·G) as sonic_pc.CommitterKey.trim takes it.  `with_id` also
+    fills the verifying key's circuit id (Circuit.id(): a host Blake2s pass over the matrices' byte streams)."""
     from .sonic_pc import CommitterKey, LabeledPolynomial, SonicKZG10
     info = circuit.info
     max_degree = info.max_degree(zk)
@@ -247,8 +296,78 @@ def circuit_setup(circuit: Circuit, pp_powers_of_beta_g: torch.Tensor, pp_powers
     ck = CommitterKey.trim(pp_powers_of_beta_g, pp_powers_of_beta_times_gamma_g, max_degree, (), 1, info.degree_bounds())
     polys = circuit.index_polynomials()
     comms, _rands = SonicKZG10.commit(ck, [LabeledPolynomial(name, p) for name, p in polys.items()])
-    vk = CircuitVerifyingKey(info, comms)
+    vk = CircuitVerifyingKey(info, comms, circuit.id() if with_id else None)
     return CircuitProvingKey(vk, circuit, ck), vk
+
+
+@dataclass
+class Certificate:
+    """snark/varuna/data_structures/certificate.rs: the BatchLCProof of prove_vk, one non-hiding KZG proof `w` (normalised projective
+    uint64[18]) at the one query point"""
+    w: np.ndarray
+
+
+def _certificate_point(challenges) -> tuple:
+    """the twelve values squeeze_nonnative_field_elements(12) yields → (point, combiners): the last is the point, the combiners are
+    one followed by the first eleven (varuna.rs:248-255, 296-300)"""
+    challenges = [int(c) % R_MOD for c in challenges]
+    if len(challenges) != len(INDEX_POLYNOMIAL_NAMES):
+        raise ValueError(f"{len(challenges)} challenges; a certificate takes {len(INDEX_POLYNOMIAL_NAMES)}")
+    return challenges[-1], [1] + challenges[:-1]
+
+
+def prove_vk(pk: CircuitProvingKey, challenges, opening_challenges) -> Certificate:
+    """VarunaSNARK::prove_vk (varuna.rs:236-276) after the sponge: open Σ c_i·p_i over the twelve index polynomials (c = [1] +
+    challenges[:11] in label order) at z = challenges[11].  The combination is one fr_lincomb pass; the opening is
+    SonicKZG10.batch_open of `circuit_check` with empty randomness, which consumes `opening_challenges` (its combination challenge,
+    then the discarded randomizer) as open_combinations would."""
+    from .sonic_pc import LabeledPolynomial, Randomness, SonicKZG10
+    point, combiners = _certificate_point(challenges)
+    polys = list(pk.circuit.index_polynomials().values())
+    combined = device.fr_lincomb(polys, [_mont(c) for c in combiners])
+    (w, _random_v), = SonicKZG10.batch_open(pk.committer_key, [LabeledPolynomial("circuit_check", combined)],
+                                            [("circuit_check", ("challenge", point))], [Randomness()], iter(opening_challenges))
+    return Certificate(w)
+
+
+@dataclass
+class VerifyingKeyCheck:
+    """verify_vk up to its pairing.  `matches`: the circuit's info and id equal the verifying key's (the reference stops with
+    CircuitNotFound otherwise; the other fields are still computed here).  The certificate is valid iff `matches` and
+    e(lhs, H) = e(w, β·H)."""
+    matches: bool
+    evaluation: int
+    lhs: np.ndarray
+    w: np.ndarray
+
+
+def _affine(projective: np.ndarray) -> np.ndarray:
+    """normalised projective image (X, Y, Z = one or (0, one, 0)) → the 104-byte Affine image (x, y, infinity flag, padding)"""
+    limbs = np.ascontiguousarray(projective, dtype=np.uint64).reshape(18)
+    out = np.zeros(104, dtype=np.uint8)
+    out[:96] = limbs[:12].view(np.uint8)
+    out[96] = 1 if not limbs[12:].any() else 0
+    return out
+
+
+def verify_vk(circuit: Circuit, vk: CircuitVerifyingKey, certificate: Certificate, challenges, opening_challenge: int) -> VerifyingKeyCheck:
+    """VarunaSNARK::verify_vk (varuna.rs:280-331) up to the pairing.  The circuit is already indexed (Circuit).  The evaluation v
+    comes from evaluate_index_polynomials; check_combinations → batch_check → accumulate_elems for one point with randomizer one
+    (sonic_pc/mod.rs:344-411, 477-544, 582-635) reduces to lhs = ξ·C_lc − ξ·v·G + z·W with C_lc = Σ c_i·C_i, ξ = opening_challenge:
+    ONE 14-point MSM over the twelve commitments, G and W.  check_elems' pairing equation is then e(lhs, H) = e(W, β·H).  G is the
+    universal verifier's g, the SRS's first power, which is the G1 generator in the mainnet setup and in synthetic_srs."""
+    point, combiners = _certificate_point(challenges)
+    xi = int(opening_challenge) % R_MOD
+    matches = circuit.info == vk.circuit_info and vk.id is not None and circuit.id() == vk.id
+    evaluation = circuit.evaluate_index_polynomials(point, combiners)
+    dev = circuit.a.row_ptr.device
+    g = device.generator_mul(torch.from_numpy(np.array([[1, 0, 0, 0]], dtype=np.uint64).view(np.int64)).to(dev))
+    comms = torch.from_numpy(np.stack([_affine(c) for c in vk.circuit_commitments])).to(dev)
+    bases = torch.cat([comms, g, torch.from_numpy(_affine(certificate.w)[None]).to(dev)])           # C_0 … C_11, G, W
+    scalars = [xi * c % R_MOD for c in combiners] + [(-xi * evaluation) % R_MOD, point]
+    sc = np.array([[(s >> (64 * i)) & (2**64 - 1) for i in range(4)] for s in scalars], dtype=np.uint64)
+    lhs = device.msm(bases, torch.from_numpy(sc.view(np.int64)).to(dev))
+    return VerifyingKeyCheck(matches, evaluation, lhs, certificate.w)
 
 
 class Prover:
