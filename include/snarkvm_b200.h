@@ -171,7 +171,7 @@ SNARKVM_API int snarkvm_b200_sonic_commit_batch_device(void* out144s, size_t str
                                                        const void* const* d_gamma_bases, const void* const* d_blinding_mont,
                                                        const size_t* nblinding, size_t count, void* stream);
 
-/* MSM scratch budget of the current device (bytes): the limit concurrent calls share (55 % of the device unless
+/* MSM scratch budget of the current device (bytes): the limit concurrent calls share (60 % of the device unless
  * SNARKVM_B200_SCRATCH_LIMIT_GB is set; callers that do not fit wait instead of failing), what is in flight, and the high-water mark. */
 SNARKVM_API int snarkvm_b200_msm_scratch_stats(size_t* limit_bytes, size_t* in_use_bytes, size_t* peak_bytes);
 /* change the limit at run time (also resets the high-water mark) */

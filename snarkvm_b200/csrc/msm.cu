@@ -251,18 +251,49 @@ FF_DEV void store_dense(uint32_t* p, const DensePoint& d) {
 // 32 DRAM lines per LDGSTS instruction, MIO and scoreboard stalls with only 4 warps per scheduler to hide them), the
 // scatter writes the RECORDS themselves: point i is read once, and for every window its 96-byte (x, ±y) image goes to the
 // slot the bucket cursor hands out.  Level 0 then reads a dense, already signed array exactly like the levels above it.
-// The CTA stages its 256 points (x, y, −y) in shared memory and writes each window's records cooperatively, six
-// consecutive lanes per record, so a store instruction touches 6 lines instead of 32.
-// Windows [w_lo, w_hi) of this segment belong to the current group of bucket sets; positions are relative to *pos_base.
-static constexpr uint32_t REC_NONE = 0xffffffffu;
+// The CTA stages its 256 points (x, y, −y) in shared memory and writes each window's records cooperatively, consecutive
+// lanes per record, so a store instruction touches 4–6 lines instead of 32.
+// rec_words = BASE_WORDS (plain bases, calls of at least REC_LINE_MIN_ENTRIES entries): every record is one whole, aligned
+// 128-byte line (x, ±y, 32 B of zeros) written by eight lanes.  At the 96-byte stride (DENSE_WORDS, six lanes) a record covers
+// half of a 64-byte unit that the next slot of its bucket fills later from another CTA; in a large call the halves rarely
+// meet in L2, and the partial writes cost more than the 33 % extra bytes (H100 SXM at 400 W, 2^24 points, 14 windows: the
+// stores alone take 16.6 ms at 96 B and 13.5 ms at 128 B; DESIGN §4).
 // FLAT (precomputed tables): window w of point i takes record w·table_n + i of the table (staged per window) and every window
 // feeds the job's single bucket set.
+// Windows [w_lo, w_hi) of this segment belong to the current group of bucket sets; positions are relative to *pos_base.
+static constexpr uint32_t REC_NONE = 0xffffffffu;
+// Below this many entries per call, 128-byte records lose to 96-byte ones.  The stores alone per record
+// (tools/scatter_probe.py, H100 SXM at 400 W, 14 windows): 96-byte records are 15–23 % faster at 2^14–2^16 points, the two
+// tie at 2^18 points (3.7 M entries), and 128-byte records are 16–18 % faster from 2^20 points.  The default plans run pair
+// levels from 2^19 points (≥ 10 M entries); smaller calls get here only with forced levels.  The tables' records (FLAT)
+// always keep 96 B: one job's table scratch cannot be split into groups and already fills most of the device next to the
+// tables.
+static constexpr size_t REC_LINE_MIN_ENTRIES = (size_t)1 << 22;
+// one window's records of the CTA's 256 points, LANES 16-byte granules per record (6, or 8 with the zero tail).
+// The whole lines are stored evict-first (st.global.cs): nothing reads them before level 0, long after they have left L2,
+// and with ordinary stores 30 GB of records push the bucket cursors (2.2 M × 4 B at 2^24) out of L2, where every cursor
+// atomic needs them (H100 SXM at 700 W, 2^24 points: the scatter 16.4 → 14.2 ms; the stores alone stay at 13.5 ms).  The
+// 96-byte records keep ordinary stores: their two halves of a 64-byte unit must meet in L2.
+template <uint32_t LANES>
+FF_DEV void emit_records(const uint4* sh_rec, const uint32_t* my_pos, uint32_t tid, uint4* __restrict__ dense0) {
+    for (uint32_t k = tid; k < 256u * LANES; k += 256u) {
+        const uint32_t r = k / LANES, part = k - LANES * r;
+        const uint32_t pp = my_pos[r];
+        if (pp == REC_NONE) continue;
+        const uint32_t src = part < 3u ? part : ((pp >> 31) ? 3u : 0u) + part;       // x0..2 | y0..2 or (−y)0..2
+        const uint4 v = part < 6u ? sh_rec[r * 9u + src] : make_uint4(0u, 0u, 0u, 0u);
+        uint4* d = dense0 + (size_t)(pp & 0x7fffffffu) * LANES + part;
+        if (LANES == 8u) __stcs(d, v);
+        else *d = v;
+    }
+}
 template <bool MONT, bool FLAT>
 __global__ void __launch_bounds__(256) k_scatter_records(const uint32_t* __restrict__ scalars, size_t n, const uint8_t* __restrict__ points,
                                                          size_t stride, const uint32_t* __restrict__ table, size_t table_n, int c_low, int c_top,
                                                          int nwin, uint32_t nbuckets,
                                                          uint32_t* __restrict__ cursors, uint32_t slot_base, int w_lo, int w_hi,
-                                                         const uint32_t* __restrict__ pos_base_ptr, uint4* __restrict__ dense0) {
+                                                         const uint32_t* __restrict__ pos_base_ptr, uint4* __restrict__ dense0,
+                                                         uint32_t rec_words) {
     __shared__ uint4 sh_rec[256 * 9];                       // per point: x (3 × 16 B), y (3), −y (3)
     __shared__ uint32_t sh_pos[2][256];
     const uint32_t tid = threadIdx.x;
@@ -327,13 +358,8 @@ __global__ void __launch_bounds__(256) k_scatter_records(const uint32_t* __restr
         uint32_t* my_pos = sh_pos[w & 1];
         my_pos[tid] = pos;
         __syncthreads();                                    // also orders the staging of sh_rec before the reads
-        for (uint32_t k = tid; k < 256u * 6u; k += 256u) {
-            const uint32_t r = k / 6u, part = k - 6u * r;
-            const uint32_t pp = my_pos[r];
-            if (pp == REC_NONE) continue;
-            const uint32_t src = part < 3u ? part : ((pp >> 31) ? 3u : 0u) + part;       // x0..2 | y0..2 or (−y)0..2
-            dense0[(size_t)(pp & 0x7fffffffu) * 6u + part] = sh_rec[r * 9u + src];
-        }
+        if (!FLAT && rec_words == (uint32_t)BASE_WORDS) emit_records<8>(sh_rec, my_pos, tid, dense0);
+        else emit_records<6>(sh_rec, my_pos, tid, dense0);
         // the next window writes the other half of sh_pos; its barrier orders this window's reads before the window after
     }
 }
@@ -613,22 +639,24 @@ FF_DEV PairDesc pair_load_desc(int64_t j, uint32_t nv, const uint2* __restrict__
     d.p = v.x; d.q = v.y; d.valid = true;
     return d;
 }
+// in_words: stride of the dense inputs — the call's record stride at level 0 (BASE_WORDS or DENSE_WORDS, see
+// REC_LINE_MIN_ENTRIES), DENSE_WORDS above
 template <bool GATHER>
-FF_DEV const uint32_t* pair_src(const PairDesc& d, int which, const uint32_t* __restrict__ records) {
+FF_DEV const uint32_t* pair_src(const PairDesc& d, int which, const uint32_t* __restrict__ records, uint32_t in_words) {
     if (GATHER) return records + (size_t)((which ? d.q : d.p) & 0x7fffffffu) * BASE_WORDS;
-    return records + (size_t)(d.p + (uint32_t)which) * DENSE_WORDS;
+    return records + (size_t)(d.p + (uint32_t)which) * in_words;
 }
 // copies of step operands into ring stage `st` of `chunks` 16-byte chunks per lane: backward (FULL) x1 y1 x2 y2 in 12 chunks,
 // forward x1 x2 in 6 chunks
 template <bool GATHER, bool FULL>
-FF_DEV void pair_issue(const PairDesc& d, uint4* ring, int st, int lane, const uint32_t* __restrict__ records, int chunks) {
+FF_DEV void pair_issue(const PairDesc& d, uint4* ring, int st, int lane, const uint32_t* __restrict__ records, uint32_t in_words, int chunks) {
     if (d.valid) {
         const uint32_t dst = smem_addr_u32(ring + (size_t)st * (size_t)(chunks * 32) + lane);
-        const uint32_t* p = pair_src<GATHER>(d, 0, records);
+        const uint32_t* p = pair_src<GATHER>(d, 0, records, in_words);
 #pragma unroll
         for (int k = 0; k < (FULL ? 6 : 3); k++) cp_async16(dst + (uint32_t)k * 512u, p + 4 * k);
         if (d.q != PAIR_NONE) {
-            const uint32_t* q = pair_src<GATHER>(d, 1, records);
+            const uint32_t* q = pair_src<GATHER>(d, 1, records, in_words);
 #pragma unroll
             for (int k = 0; k < (FULL ? 6 : 3); k++) cp_async16(dst + (uint32_t)((FULL ? 6 : 3) + k) * 512u, q + 4 * k);
         }
@@ -637,9 +665,9 @@ FF_DEV void pair_issue(const PairDesc& d, uint4* ring, int st, int lane, const u
 }
 // full classification of one pair from global memory (rare path of the forward pass: equal x, or an x that is 0)
 template <bool GATHER>
-FF_DEV int pair_classify_global(const PairDesc& d, const uint32_t* __restrict__ records, Fq& den) {
-    DensePoint P = load_dense(pair_src<GATHER>(d, 0, records));
-    DensePoint Q = load_dense(pair_src<GATHER>(d, 1, records));
+FF_DEV int pair_classify_global(const PairDesc& d, const uint32_t* __restrict__ records, uint32_t in_words, Fq& den) {
+    DensePoint P = load_dense(pair_src<GATHER>(d, 0, records, in_words));
+    DensePoint Q = load_dense(pair_src<GATHER>(d, 1, records, in_words));
     if (GATHER) { if ((d.p >> 31) && !P.inf) P.y = P.y.neg(); if ((d.q >> 31) && !Q.inf) Q.y = Q.y.neg(); }
     return classify_pair(P, Q, true, den);
 }
@@ -651,7 +679,7 @@ FF_DEV int pair_classify_global(const PairDesc& d, const uint32_t* __restrict__ 
 // MINB = resident CTAs per SM the kernel is compiled for: 4 (128 registers) or 3 (168 registers, no spills).
 template <bool GATHER, int MINB>
 __global__ void __launch_bounds__(PAIR_THREADS, MINB) k_pair_level2(const uint32_t* __restrict__ records /* level 0: dense bases / table; above: dense_in */,
-                                                         const uint2* __restrict__ desc, const uint32_t* __restrict__ total_ptr,
+                                                         uint32_t in_words, const uint2* __restrict__ desc, const uint32_t* __restrict__ total_ptr,
                                                          uint32_t T_bound, uint32_t* __restrict__ prefix, uint32_t* __restrict__ dense_out,
                                                          uint32_t* __restrict__ sm_slots) {
     (void)T_bound;
@@ -689,12 +717,12 @@ __global__ void __launch_bounds__(PAIR_THREADS, MINB) k_pair_level2(const uint32
     {
         constexpr int PF = 3;                                                   // steps of lead; PF + 1 stages of 6 chunks
         PairDesc q0 = pair_load_desc(0, nv, dlane), q1 = pair_load_desc(1, nv, dlane), q2 = pair_load_desc(2, nv, dlane);
-        pair_issue<GATHER, false>(q0, ring, 0, lane, records, 6);
-        pair_issue<GATHER, false>(q1, ring, 1, lane, records, 6);
-        pair_issue<GATHER, false>(q2, ring, 2, lane, records, 6);
+        pair_issue<GATHER, false>(q0, ring, 0, lane, records, in_words, 6);
+        pair_issue<GATHER, false>(q1, ring, 1, lane, records, in_words, 6);
+        pair_issue<GATHER, false>(q2, ring, 2, lane, records, in_words, 6);
         PairDesc ahead = pair_load_desc(PF, nv, dlane);
         for (uint32_t j = 0; j < T; j++) {
-            pair_issue<GATHER, false>(ahead, ring, (int)((j + PF) & 3u), lane, records, 6);       // step j+3 (descriptor loaded a step ago)
+            pair_issue<GATHER, false>(ahead, ring, (int)((j + PF) & 3u), lane, records, in_words, 6);       // step j+3 (descriptor loaded a step ago)
             const PairDesc cur = q0;
             q0 = q1; q1 = q2; q2 = ahead;
             ahead = pair_load_desc((int64_t)j + PF + 1, nv, dlane);                              // not touched until the next iteration
@@ -705,7 +733,7 @@ __global__ void __launch_bounds__(PAIR_THREADS, MINB) k_pair_level2(const uint32
                 Fq x1 = ring_fq(slot_p), x2 = ring_fq(slot_p + 3 * 32);
                 if (x1 == x2 || x1.is_zero() || x2.is_zero()) {
                     Fq den;
-                    if (pair_classify_global<GATHER>(cur, records, den) >= PAIR_ADD) d = den;
+                    if (pair_classify_global<GATHER>(cur, records, in_words, den) >= PAIR_ADD) d = den;
                 } else {
                     d = x2 - x1;
                 }
@@ -719,11 +747,11 @@ __global__ void __launch_bounds__(PAIR_THREADS, MINB) k_pair_level2(const uint32
     // ---------------- backward: one inverse per pair, then the affine addition ----------------
     {
         PairDesc cur = pair_load_desc((int64_t)T - 1, nv, dlane);
-        pair_issue<GATHER, true>(cur, ring, 0, lane, records, 12);
+        pair_issue<GATHER, true>(cur, ring, 0, lane, records, in_words, 12);
         PairDesc nxt = pair_load_desc((int64_t)T - 2, nv, dlane);
         for (uint32_t k = 0; k < T; k++) {
             const uint32_t j = T - 1 - k;
-            pair_issue<GATHER, true>(nxt, ring, (int)((k + 1) & 1u), lane, records, 12);
+            pair_issue<GATHER, true>(nxt, ring, (int)((k + 1) & 1u), lane, records, in_words, 12);
             PairDesc nn = pair_load_desc((int64_t)j - 2, nv, dlane);
             Fq pf = Fq::one();
             if (cur.valid && j != 0) pf = Fq::load(plane + (size_t)(j - 1) * (32 * 12));     // behind the first multiplication
@@ -1306,10 +1334,11 @@ struct DeviceScratch {
 };
 static DeviceScratch g_scratch[64];
 
-// Default scratch budget and pool release threshold: 55 % of the device.  On an 80 GB H100 that keeps the 44 GB of a
-// one-group 2^24-point MSM cached between calls; a call whose scratch exceeds the threshold has its memory unmapped and
-// mapped again on every call (one 49 GB group: 348 ms per call against 116 ms of kernels, H100 SXM at 700 W).
-static size_t default_scratch_bytes(size_t total) { return total / 20 * 11; }
+// Default scratch budget and pool release threshold: 60 % of the device.  On an 80 GB H100 that keeps the 48 GB of a
+// one-group 2^24-point MSM with 128-byte level-0 records cached between calls; a call whose scratch exceeds the threshold
+// has its memory unmapped and mapped again on every call (one 49 GB group: 348 ms per call against 116 ms of kernels, H100
+// SXM at 700 W).
+static size_t default_scratch_bytes(size_t total) { return total / 5 * 3; }
 
 static int scratch_init(DeviceScratch& ds, int dev) {
     if (ds.ready) return 0;
@@ -1469,11 +1498,12 @@ int msm_core(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, co
     if (flat && table_n * (size_t)plan.nwin >= (1ull << 31)) return (int)cudaErrorInvalidValue;
     const int levels = plan.levels;
     const size_t set_cap = flat ? max_job_n * (size_t)plan.nwin : max_job_n;   // most entries one bucket set (or one bucket) can hold
-    // pair levels over plain bases: the sort scatters 96-byte records (k_scatter_records) and every level is dense;
-    // tables (flat) and the XYZZ-only path keep the index sort + gather
+    // pair levels: the sort scatters level-0 records (k_scatter_records) and every level is dense; the XYZZ-only path keeps
+    // the index sort + gather
     bool records = levels > 0;
     if (const char* e = getenv("SNARKVM_B200_MSM_RECORDS")) records = records && atoi(e) != 0;
     if (const char* e = getenv("SNARKVM_B200_MSM_PAIR_V1")) { if (atoi(e) != 0) records = false; }      // the round-1 kernel gathers
+    const uint32_t rec_words = !flat && max_entries >= REC_LINE_MIN_ENTRIES ? BASE_WORDS : DENSE_WORDS;   // level-0 record stride
     // a scalar segment must lie inside one base array (the record scatter reads its points through one pointer)
     std::vector<const uint8_t*> seg_points((size_t)nsegs, nullptr);
     std::vector<size_t> seg_stride((size_t)nsegs, 0);
@@ -1493,9 +1523,9 @@ int msm_core(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, co
     }
 
     // Everything after the bucket sort runs per GROUP of whole windows (all bucket sets of a window together), so the dense
-    // scratch of the pair levels (≈ 180 B per entry with the level-0 records) stays inside the budget of the device's cached
-    // scratch: on an 80 GB H100, 2^24 points → all windows in one group (≈ 42 GB for 14), a 2^26-point shard three windows at a
-    // time.  Fewer groups mean fewer, larger pair-level launches (H100 SXM, 700 W: 116 ms of kernels in one group against 121 ms
+    // scratch of the pair levels (≈ 212 B per entry with 128-byte level-0 records) stays inside the budget of the device's
+    // cached scratch: on an 80 GB H100, 2^24 points → all windows in one group (49 GB for 14), a 2^26-point shard three
+    // windows at a time.  Fewer groups mean fewer, larger pair-level launches (H100 SXM, 700 W: 116 ms of kernels in one group against 121 ms
     // in two).  A window holds at most one entry per scalar whatever the number of its sets.
     size_t budget = 0;
     if ((rc = scratch_group_budget(&budget)) != 0) return rc;
@@ -1504,9 +1534,10 @@ int msm_core(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, co
     const uint32_t nwins = (uint32_t)njobs * wins_per_job;
     uint32_t gu = nwins;                                          // windows per group
     if (levels > 0) {
-        // per entry: dense_a 48 + prefix 24 + descriptors 4, plus the 96-byte level-0 records (dense_b reuses them: level 0
-        // is their last reader) rounded up to 180 for the item partials and per-bucket arrays; or dense_b 24 + the 4-byte index
-        size_t per_win = set_cap * (size_t)(records ? 180 : 104) + 1;
+        // per entry: dense_a 48 + prefix 24 + descriptors 4, plus the level-0 records (dense_b reuses them: level 0 is their
+        // last reader), 96 or 128 B (rec_words), with 8 B for the item partials and per-bucket arrays;
+        // or dense_b 24 + the 4-byte index
+        size_t per_win = set_cap * (size_t)(records ? 84 + 4 * rec_words : 104) + 1;
         size_t fit = budget / per_win;
         if (fit < 1) fit = 1;
         if (fit < gu) {
@@ -1627,14 +1658,14 @@ int msm_core(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, co
         red_b = a.take<uint32_t>((size_t)gw * (chunks_per_set / tree + 1 > 2 * ((plan.nbuckets + 63u) / 64u) + 2 ? chunks_per_set / tree + 1 : 2 * ((plan.nbuckets + 63u) / 64u) + 2) * XYZZ_WORDS);
         cub_tmp = a.take<uint8_t>(cub_bytes);
         if (!flat && !records) dense_bases = a.take<uint32_t>(total_bases * (size_t)BASE_WORDS);
-        if (records) dense0 = a.take<uint32_t>(entries_g * (size_t)DENSE_WORDS);
+        if (records) dense0 = a.take<uint32_t>(entries_g * (size_t)rec_words);
         if (levels > 0) {
             off_a = a.take<uint32_t>((size_t)TBg + 1);
             off_b = a.take<uint32_t>((size_t)TBg + 1);
             dense_a = a.take<uint32_t>(dense_cap_a * DENSE_WORDS);
-            // level 1 writes its outputs over the level-0 records: only level 0 reads them, and the next group's scatter
-            // runs after this group's accumulation in stream order
-            if (levels > 1) dense_b = records && dense_cap_b <= entries_g ? dense0 : a.take<uint32_t>(dense_cap_b * DENSE_WORDS);
+            // level 1 writes its outputs (96-byte points) over the level-0 records: only level 0 reads them, and the next
+            // group's scatter runs after this group's accumulation in stream order
+            if (levels > 1) dense_b = records && dense_cap_b * DENSE_WORDS <= entries_g * (size_t)rec_words ? dense0 : a.take<uint32_t>(dense_cap_b * DENSE_WORDS);
             prefix = a.take<uint32_t>(dense_cap_a * 12);
             desc = a.take<uint2>(dense_cap_a);
             sm_slots = a.take<uint32_t>(256);
@@ -1745,11 +1776,11 @@ int msm_core(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, co
                         const uint32_t* sc = (const uint32_t*)sg.d_scalars;
                         const int ct = plan.c_top, nw = plan.nwin;
                         if (flat) {
-                            if (sg.mont) k_scatter_records<true, true><<<grid, 256, 0, stream>>>(sc, sg.n, nullptr, 0, table, table_n, plan.c, ct, nw, plan.nbuckets, cursors, slot_base, w_lo, w_hi, bs, (uint4*)dense0);
-                            else k_scatter_records<false, true><<<grid, 256, 0, stream>>>(sc, sg.n, nullptr, 0, table, table_n, plan.c, ct, nw, plan.nbuckets, cursors, slot_base, w_lo, w_hi, bs, (uint4*)dense0);
+                            if (sg.mont) k_scatter_records<true, true><<<grid, 256, 0, stream>>>(sc, sg.n, nullptr, 0, table, table_n, plan.c, ct, nw, plan.nbuckets, cursors, slot_base, w_lo, w_hi, bs, (uint4*)dense0, rec_words);
+                            else k_scatter_records<false, true><<<grid, 256, 0, stream>>>(sc, sg.n, nullptr, 0, table, table_n, plan.c, ct, nw, plan.nbuckets, cursors, slot_base, w_lo, w_hi, bs, (uint4*)dense0, rec_words);
                         } else {
-                            if (sg.mont) k_scatter_records<true, false><<<grid, 256, 0, stream>>>(sc, sg.n, seg_points[i], seg_stride[i], nullptr, 0, plan.c, ct, nw, plan.nbuckets, cursors, slot_base, w_lo, w_hi, bs, (uint4*)dense0);
-                            else k_scatter_records<false, false><<<grid, 256, 0, stream>>>(sc, sg.n, seg_points[i], seg_stride[i], nullptr, 0, plan.c, ct, nw, plan.nbuckets, cursors, slot_base, w_lo, w_hi, bs, (uint4*)dense0);
+                            if (sg.mont) k_scatter_records<true, false><<<grid, 256, 0, stream>>>(sc, sg.n, seg_points[i], seg_stride[i], nullptr, 0, plan.c, ct, nw, plan.nbuckets, cursors, slot_base, w_lo, w_hi, bs, (uint4*)dense0, rec_words);
+                            else k_scatter_records<false, false><<<grid, 256, 0, stream>>>(sc, sg.n, seg_points[i], seg_stride[i], nullptr, 0, plan.c, ct, nw, plan.nbuckets, cursors, slot_base, w_lo, w_hi, bs, (uint4*)dense0, rec_words);
                         }
                         count_launch();
                     }
@@ -1786,12 +1817,13 @@ int msm_core(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, co
                         const unsigned dgrid = (unsigned)((bound + 255) / 256);
                         if (l == 0 && !records) {
                             k_pair_desc<true><<<dgrid, 256, 0, stream>>>(sorted, off_in, off_out, tb, desc, nullptr);
-                            if (pair_minb == 3) k_pair_level2<true, 3><<<lgrid, 128, PAIR2_SMEM, stream>>>(gather_src, desc, off_out + tb, (uint32_t)T, prefix, dense_out, sm_slots);
-                            else k_pair_level2<true, 4><<<lgrid, 128, PAIR2_SMEM, stream>>>(gather_src, desc, off_out + tb, (uint32_t)T, prefix, dense_out, sm_slots);
+                            if (pair_minb == 3) k_pair_level2<true, 3><<<lgrid, 128, PAIR2_SMEM, stream>>>(gather_src, BASE_WORDS, desc, off_out + tb, (uint32_t)T, prefix, dense_out, sm_slots);
+                            else k_pair_level2<true, 4><<<lgrid, 128, PAIR2_SMEM, stream>>>(gather_src, BASE_WORDS, desc, off_out + tb, (uint32_t)T, prefix, dense_out, sm_slots);
                         } else {
                             k_pair_desc<false><<<dgrid, 256, 0, stream>>>(nullptr, off_in, off_out, tb, desc, l == 0 ? bs : nullptr);
-                            if (pair_minb == 3) k_pair_level2<false, 3><<<lgrid, 128, PAIR2_SMEM, stream>>>(dense_in, desc, off_out + tb, (uint32_t)T, prefix, dense_out, sm_slots);
-                            else k_pair_level2<false, 4><<<lgrid, 128, PAIR2_SMEM, stream>>>(dense_in, desc, off_out + tb, (uint32_t)T, prefix, dense_out, sm_slots);
+                            const uint32_t in_words = l == 0 ? rec_words : (uint32_t)DENSE_WORDS;
+                            if (pair_minb == 3) k_pair_level2<false, 3><<<lgrid, 128, PAIR2_SMEM, stream>>>(dense_in, in_words, desc, off_out + tb, (uint32_t)T, prefix, dense_out, sm_slots);
+                            else k_pair_level2<false, 4><<<lgrid, 128, PAIR2_SMEM, stream>>>(dense_in, in_words, desc, off_out + tb, (uint32_t)T, prefix, dense_out, sm_slots);
                         }
                         count_launch(1);
                     }

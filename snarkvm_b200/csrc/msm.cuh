@@ -119,7 +119,7 @@ int test_curve_op_device(int group, int op, void* d_out, const void* d_a, const 
 int xyzz_sum_ranks_device(uint32_t* d_out, const uint32_t* d_in, int nranks, int count, cudaStream_t stream);
 
 // Allocation from the library's private stream-ordered pool of the current device (release threshold = the scratch budget:
-// 55 % of the device unless SNARKVM_B200_SCRATCH_LIMIT_GB says otherwise); free with cudaFreeAsync.  The default pool is untouched.
+// 60 % of the device unless SNARKVM_B200_SCRATCH_LIMIT_GB says otherwise); free with cudaFreeAsync.  The default pool is untouched.
 int pool_alloc_raw(void** p, size_t bytes, cudaStream_t stream);
 template <class T> inline cudaError_t pool_alloc(T** p, size_t bytes, cudaStream_t stream) { return (cudaError_t)pool_alloc_raw((void**)p, bytes, stream); }
 // MSM scratch budget of the current device: bytes allowed in flight, in flight now, and the high-water mark
