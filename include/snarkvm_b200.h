@@ -239,6 +239,63 @@ SNARKVM_API int snarkvm_b200_fr_lincomb_device(void* d_out, size_t n, const void
 SNARKVM_API int snarkvm_b200_matrix_evals_dot_device(void* out_mont_host, const void* d_row, const void* d_col, const void* d_row_col_val,
                                                      const void* d_lagrange, size_t n, void* stream);
 
+/* Many circuits per call (VarunaSNARK::batch_circuit_setup, varuna.rs:72-134; a deployment's setup and certificates, one circuit
+ * per function).  Each entry point below does in ONE pass what the one-matrix entry point above does per matrix; the results are
+ * bit-identical to a loop of those calls.  Segment tables are HOST arrays; the device pointers in them follow the layouts above. */
+
+/* In-place transforms, transform i of 2^lgs[i] Fr at d_data[i] (HOST array of device pointers), natural order, one direction and
+ * type for all.  Each result equals snarkvm_b200_ntt_device's.  Transforms of equal size share their launches (one launch per pass
+ * for all of them); the sizes may be mixed, from 2^0 up. */
+SNARKVM_API int snarkvm_b200_ntt_batch_device(void* const* d_data, const uint32_t* lgs, size_t count, int ntt_direction, int ntt_type,
+                                              void* stream);
+
+/* One CSR matrix of a segmented indexer call (the arguments of snarkvm_b200_varuna_matrix_evals_device).  d_out: row, col and
+ * row_col_val (2^lg_non_zero Fr each) for matrix_evals; d_out[0] alone receives the 8 + 8 * nrows + 40 * nnz bytes (8-byte
+ * aligned) of the byte stream for csr_serialize, which reads only the CSR arrays, nrows and nnz. */
+typedef struct {
+    const void* d_row_ptr;
+    const void* d_cols;
+    const void* d_vals;
+    uint64_t nrows, nnz, nvars, input_size;
+    uint32_t lg_constraint, lg_variable, lg_non_zero, reserved;
+    void* d_out[3];
+} snarkvm_b200_csr_segment_t;
+/* matrix_evals of every segment in one launch and one synchronisation.  Argument errors return cudaErrorInvalidValue before any
+ * launch.  A bad column or row_ptr in any segment returns cudaErrorInvalidValue after the pass, and *bad_segment (HOST, may be
+ * NULL) receives the index of the first such segment (-1 otherwise); outputs are then unspecified. */
+SNARKVM_API int snarkvm_b200_varuna_matrix_evals_batch_device(const snarkvm_b200_csr_segment_t* segs, size_t count, int64_t* bad_segment,
+                                                              void* stream);
+/* The circuit id's byte stream of every segment in one launch and one synchronisation; errors as above. */
+SNARKVM_API int snarkvm_b200_csr_serialize_batch_device(const snarkvm_b200_csr_segment_t* segs, size_t count, int64_t* bad_segment,
+                                                        void* stream);
+
+/* One output of a segmented linear combination: d_out (n Fr) = sum_j coeffs_mont[j] * d_polys[j], lens[j] <= n, nterms <= 12. */
+typedef struct {
+    void* d_out;
+    uint64_t n;
+    const void* d_polys[12];
+    uint64_t lens[12];
+    uint8_t coeffs_mont[12][32];
+    uint32_t nterms, reserved;
+} snarkvm_b200_lincomb_segment_t;
+/* every segment's combination in one launch (snarkvm_b200_fr_lincomb_device per segment, bit for bit) */
+SNARKVM_API int snarkvm_b200_fr_lincomb_batch_device(const snarkvm_b200_lincomb_segment_t* segs, size_t count, void* stream);
+
+/* One matrix of a segmented MatrixEvals::evaluate: its row, col and row_col_val on K (n = |K| Fr each, n a power of two) and the
+ * point (32 B Montgomery). */
+typedef struct {
+    const void* d_row;
+    const void* d_col;
+    const void* d_row_col_val;
+    uint64_t n;
+    uint8_t point_mont[32];
+} snarkvm_b200_evals_segment_t;
+/* For every segment: the Lagrange coefficients of its K at its point (fft/domain.rs:258-292, a point inside K included) and the four
+ * inner products of snarkvm_b200_matrix_evals_dot_device with them.  All denominators share one batch inversion; one
+ * synchronisation.  out_mont_host: count x 4 x 32 B HOST. */
+SNARKVM_API int snarkvm_b200_matrix_evals_at_points_device(void* out_mont_host, const snarkvm_b200_evals_segment_t* segs, size_t count,
+                                                           void* stream);
+
 /* Fr Montgomery <-> canonical, n elements in HBM (to_bigint / from_bigint, fields/src/fp_256.rs:362-413). */
 SNARKVM_API int snarkvm_b200_fr_from_mont_device(void* d_out, const void* d_in, size_t n, void* stream);
 SNARKVM_API int snarkvm_b200_fr_to_mont_device(void* d_out, const void* d_in, size_t n, void* stream);

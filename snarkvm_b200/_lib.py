@@ -34,7 +34,29 @@ SYMBOLS = (
     "snarkvm_b200_test_field_op_device", "snarkvm_b200_test_curve_op_device", "snarkvm_b200_test_field_op_host",
     "snarkvm_b200_varuna_matrix_evals_device", "snarkvm_b200_csr_transpose_device",
     "snarkvm_b200_csr_serialize_device", "snarkvm_b200_fr_lincomb_device", "snarkvm_b200_matrix_evals_dot_device",
+    "snarkvm_b200_ntt_batch_device", "snarkvm_b200_varuna_matrix_evals_batch_device", "snarkvm_b200_csr_serialize_batch_device",
+    "snarkvm_b200_fr_lincomb_batch_device", "snarkvm_b200_matrix_evals_at_points_device",
 )
+
+
+class CsrSegment(ctypes.Structure):
+    """snarkvm_b200_csr_segment_t"""
+    _fields_ = [("d_row_ptr", ctypes.c_void_p), ("d_cols", ctypes.c_void_p), ("d_vals", ctypes.c_void_p),
+                ("nrows", ctypes.c_uint64), ("nnz", ctypes.c_uint64), ("nvars", ctypes.c_uint64), ("input_size", ctypes.c_uint64),
+                ("lg_constraint", ctypes.c_uint32), ("lg_variable", ctypes.c_uint32), ("lg_non_zero", ctypes.c_uint32),
+                ("reserved", ctypes.c_uint32), ("d_out", ctypes.c_void_p * 3)]
+
+
+class LincombSegment(ctypes.Structure):
+    """snarkvm_b200_lincomb_segment_t"""
+    _fields_ = [("d_out", ctypes.c_void_p), ("n", ctypes.c_uint64), ("d_polys", ctypes.c_void_p * 12), ("lens", ctypes.c_uint64 * 12),
+                ("coeffs_mont", (ctypes.c_uint8 * 32) * 12), ("nterms", ctypes.c_uint32), ("reserved", ctypes.c_uint32)]
+
+
+class EvalsSegment(ctypes.Structure):
+    """snarkvm_b200_evals_segment_t"""
+    _fields_ = [("d_row", ctypes.c_void_p), ("d_col", ctypes.c_void_p), ("d_row_col_val", ctypes.c_void_p), ("n", ctypes.c_uint64),
+                ("point_mont", ctypes.c_uint8 * 32)]
 
 
 class CudaError(RuntimeError):
@@ -117,6 +139,11 @@ def lib():
     L.snarkvm_b200_csr_serialize_device.argtypes = [vp, sz, vp, sz, vp, vp, sz, vp]
     L.snarkvm_b200_fr_lincomb_device.argtypes = [vp, sz, vp, vp, vp, u32, vp]
     L.snarkvm_b200_matrix_evals_dot_device.argtypes = [vp, vp, vp, vp, vp, sz, vp]
+    L.snarkvm_b200_ntt_batch_device.argtypes = [vp, vp, sz, i32, i32, vp]
+    L.snarkvm_b200_varuna_matrix_evals_batch_device.argtypes = [ctypes.POINTER(CsrSegment), sz, ctypes.POINTER(ctypes.c_int64), vp]
+    L.snarkvm_b200_csr_serialize_batch_device.argtypes = [ctypes.POINTER(CsrSegment), sz, ctypes.POINTER(ctypes.c_int64), vp]
+    L.snarkvm_b200_fr_lincomb_batch_device.argtypes = [ctypes.POINTER(LincombSegment), sz, vp]
+    L.snarkvm_b200_matrix_evals_at_points_device.argtypes = [vp, ctypes.POINTER(EvalsSegment), sz, vp]
     L.snarkvm_b200_msm_batch_device.argtypes = [vp, vp, sz, vp, vp, sz, vp]
     L.snarkvm_b200_msm_window_sums_plan_device.argtypes = [vp, vp, sz, vp, sz, vp, sz, vp]
     L.snarkvm_b200_kzg_commit_batch_hiding_device.argtypes = [vp, vp, sz, vp, vp, vp, vp, vp, sz, vp]

@@ -1179,6 +1179,21 @@ int snarkvm_b200_matrix_evals_dot_device(void* out_mont_host, const void* d_row,
                                          const void* d_lagrange, size_t n, void* stream) {
     return matrix_evals_dot_device(out_mont_host, d_row, d_col, d_row_col_val, d_lagrange, n, (cudaStream_t)stream);
 }
+int snarkvm_b200_ntt_batch_device(void* const* d_data, const uint32_t* lgs, size_t count, int ntt_direction, int ntt_type, void* stream) {
+    return ntt_batch_device(d_data, lgs, count, ntt_direction, ntt_type, (cudaStream_t)stream);
+}
+int snarkvm_b200_varuna_matrix_evals_batch_device(const snarkvm_b200_csr_segment_t* segs, size_t count, int64_t* bad_segment, void* stream) {
+    return varuna_matrix_evals_batch_device(segs, count, bad_segment, (cudaStream_t)stream);
+}
+int snarkvm_b200_csr_serialize_batch_device(const snarkvm_b200_csr_segment_t* segs, size_t count, int64_t* bad_segment, void* stream) {
+    return csr_serialize_batch_device(segs, count, bad_segment, (cudaStream_t)stream);
+}
+int snarkvm_b200_fr_lincomb_batch_device(const snarkvm_b200_lincomb_segment_t* segs, size_t count, void* stream) {
+    return fr_lincomb_batch_device(segs, count, (cudaStream_t)stream);
+}
+int snarkvm_b200_matrix_evals_at_points_device(void* out_mont_host, const snarkvm_b200_evals_segment_t* segs, size_t count, void* stream) {
+    return matrix_evals_at_points_device(out_mont_host, segs, count, (cudaStream_t)stream);
+}
 
 int snarkvm_b200_fr_from_mont_device(void* d_out, const void* d_in, size_t n, void* stream) {
     return fr_from_mont_device(d_out, d_in, n, (cudaStream_t)stream);

@@ -169,10 +169,16 @@ struct PassArgs {
     uint32_t tile0;      // first tile of this launch (a pass may be launched in column ranges)
     int pre;             // 1: multiply input j by coset_lo/hi (forward coset)
     int post;            // 0 none, 1: × n^{-1}, 2: × coset_lo/hi[k] (hi already carries n^{-1})
+    // k_ntt_pass<true>: blockIdx.y is a transform of 2^lg elements at batch[y]; in / out are then the scratch base (transform y's
+    // scratch at in/out + y·2^lg) unless in_batch / out_batch select batch[y]
+    Fr* const* batch;
+    int in_batch, out_batch;
 };
 
 FF_DEV Fr coset_factor(const Fr* lo, const Fr* hi, size_t idx) { return lo[idx & 4095] * hi[idx >> 12]; }
 
+// BATCH: the pointer-table form (ntt_batch_device); the one-transform instantiation compiles without it.
+template <bool BATCH>
 __global__ void __launch_bounds__(256) k_ntt_pass(PassArgs a) {
     // Shared memory holds the tile as two planes of 16-byte halves (low limbs of element i at [i], high limbs at
     // [tile_elems + i]): consecutive threads then touch consecutive 16-byte words — conflict-free LDS/STS.128 — where
@@ -206,6 +212,14 @@ __global__ void __launch_bounds__(256) k_ntt_pass(PassArgs a) {
     const Tile sm{smem_raw, tile_elems, (uint32_t)Q, cols - 1u};
     const size_t tile = (size_t)blockIdx.x + a.tile0;
     const uint32_t tid = threadIdx.x, nthr = blockDim.x;
+    const Fr* src = a.in;
+    Fr* dst = a.out;
+    if (BATCH) {
+        Fr* const x = a.batch[blockIdx.y];
+        const size_t off = (size_t)blockIdx.y << lg;
+        src = a.in_batch ? x : a.in + off;
+        dst = a.out_batch ? x : a.out + off;
+    }
 
     size_t H = 0, low_base = 0, hprime_base = 0;
     if (!a.last) { H = tile >> (L - Q); low_base = (tile & (((size_t)1 << (L - Q)) - 1)) << Q; }
@@ -233,7 +247,7 @@ __global__ void __launch_bounds__(256) k_ntt_pass(PassArgs a) {
             size_t Hrow = t0 ? (size_t)(__brevll((unsigned long long)hp) >> (64 - t0)) : 0;
             idx = (Hrow << S) | d;
         }
-        Fr x = Fr::load(a.in + idx);
+        Fr x = Fr::load(src + idx);
         if (a.pre) x = x * coset_factor(a.coset_lo, a.coset_hi, idx);
         sm.put((d << Q) | c, x);
     }
@@ -332,7 +346,7 @@ __global__ void __launch_bounds__(256) k_ntt_pass(PassArgs a) {
         Fr x = sm.get((d << Q) | c);
         if (a.post == 1) x = x * (*a.ninv);
         else if (a.post == 2) x = x * coset_factor(a.coset_lo, a.coset_hi, k);
-        x.store(a.out + k);
+        x.store(dst + k);
     }
 }
 
@@ -410,16 +424,10 @@ int ntt_make_passes(uint32_t lg, NttPass* out, int* npasses) {
 // Tile t of pass 0 holds columns [t·2^Q, (t+1)·2^Q) of the 2^S × 2^(lg−S) row-major view of the input; tile t of the last pass
 // produces the same column range of the 2^S × 2^t0 view of the (natural-order) output — which is what lets a host-buffer
 // transform upload / download by column ranges underneath those two passes (snarkvm_ntt in api.cu).
-int ntt_launch_pass(void* d_A, void* d_B, uint32_t lg, int direction, int type, int p, size_t tile0, size_t ntiles, cudaStream_t stream) {
-    if (lg > NTT_MAX_LG || (direction != NTT_FORWARD && direction != NTT_INVERSE) || (type != NTT_STANDARD && type != NTT_COSET))
-        return (int)cudaErrorInvalidValue;
-    NttPass passes[8];
-    int P = 0, rc = ntt_make_passes(lg, passes, &P);
-    if (rc) return rc;
-    if (p < 0 || p >= P || tile0 + ntiles > passes[p].tiles || (P > 1 && !d_B)) return (int)cudaErrorInvalidValue;
-    if (ntiles == 0) return 0;
+// Everything of pass p of a 2^lg transform but its buffers (in, out, batch).
+static int pass_args(uint32_t lg, int direction, int type, int p, const NttPass* passes, int P, PassArgs* out) {
     const Fr* tw = nullptr;
-    int lgN = 0;
+    int lgN = 0, rc = 0;
     CosetTables ct{nullptr, nullptr, nullptr};
     const bool inverse = direction == NTT_INVERSE, coset = type == NTT_COSET;
     static std::once_flag smem_once[64];
@@ -428,26 +436,97 @@ int ntt_launch_pass(void* d_A, void* d_B, uint32_t lg, int direction, int type, 
     {
         int dev = 0; cudaGetDevice(&dev);
         std::call_once(smem_once[dev & 63], [] {
-            cudaFuncSetAttribute(k_ntt_pass, cudaFuncAttributeMaxDynamicSharedMemorySize, (1 << TILE_LG) * (int)sizeof(Fr) + (int)tw_smem_bytes(TILE_LG, true));
+            const int smem = (1 << TILE_LG) * (int)sizeof(Fr) + (int)tw_smem_bytes(TILE_LG, true);
+            cudaFuncSetAttribute(k_ntt_pass<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+            cudaFuncSetAttribute(k_ntt_pass<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
         });
     }
-    PassArgs a;
+    PassArgs a{};
     a.tw = tw; a.coset_lo = ct.lo; a.coset_hi = ct.hi; a.ninv = ct.ninv;
     a.lg = (int)lg; a.lgN = lgN; a.t0 = passes[p].t0; a.S = passes[p].S; a.Q = passes[p].Q;
     a.last = (p == P - 1) ? 1 : 0;
     a.inverse = inverse ? 1 : 0;
     a.pre = (p == 0 && coset && !inverse) ? 1 : 0;
     a.post = (a.last && inverse) ? (coset ? 2 : 1) : 0;
+    *out = a;
+    return 0;
+}
+static inline size_t pass_smem(const PassArgs& a) { return ((size_t)1 << (a.S + a.Q)) * sizeof(Fr) + tw_smem_bytes(a.S, a.last != 0); }
+
+int ntt_launch_pass(void* d_A, void* d_B, uint32_t lg, int direction, int type, int p, size_t tile0, size_t ntiles, cudaStream_t stream) {
+    if (lg > NTT_MAX_LG || (direction != NTT_FORWARD && direction != NTT_INVERSE) || (type != NTT_STANDARD && type != NTT_COSET))
+        return (int)cudaErrorInvalidValue;
+    NttPass passes[8];
+    int P = 0, rc = ntt_make_passes(lg, passes, &P);
+    if (rc) return rc;
+    if (p < 0 || p >= P || tile0 + ntiles > passes[p].tiles || (P > 1 && !d_B)) return (int)cudaErrorInvalidValue;
+    if (ntiles == 0) return 0;
+    PassArgs a;
+    if ((rc = pass_args(lg, direction, type, p, passes, P, &a)) != 0) return rc;
     a.in = (p == 0) ? (const Fr*)d_A : (const Fr*)d_B;
     a.out = (P == 1 || a.last) ? (Fr*)d_A : (Fr*)d_B;
     a.tile0 = (uint32_t)tile0;
-    const size_t smem = ((size_t)1 << (a.S + a.Q)) * sizeof(Fr) + tw_smem_bytes(a.S, a.last != 0);
     {
         ProfScope pass_scope(PROF_NTT_PASS, stream);
-        k_ntt_pass<<<(unsigned)ntiles, 256, smem, stream>>>(a);
+        k_ntt_pass<false><<<(unsigned)ntiles, 256, pass_smem(a), stream>>>(a);
     }
     count_launch();
     return (int)cudaGetLastError();
+}
+
+// Transforms of equal size share their launches: blockIdx.y picks the transform from a device-side pointer table, so a size
+// of one pass costs one launch for all its transforms and a larger size one launch per pass (each transform has its own
+// slice of one scratch buffer).  The twiddle table is built once, for the largest size, before any launch.
+static constexpr size_t NTT_BATCH_GRID_Y = 65535;
+int ntt_batch_device(void* const* d_data, const uint32_t* lgs, size_t count, int direction, int type, cudaStream_t stream) {
+    if (count == 0) return 0;
+    if (!d_data || !lgs || (direction != NTT_FORWARD && direction != NTT_INVERSE) || (type != NTT_STANDARD && type != NTT_COSET))
+        return (int)cudaErrorInvalidValue;
+    std::map<uint32_t, std::vector<Fr*>> by_lg;
+    uint32_t lg_max = 0;
+    for (size_t i = 0; i < count; i++) {
+        if (lgs[i] > NTT_MAX_LG || !d_data[i]) return (int)cudaErrorInvalidValue;
+        by_lg[lgs[i]].push_back((Fr*)d_data[i]);
+        if (lgs[i] > lg_max) lg_max = lgs[i];
+    }
+    const Fr* tw = nullptr;
+    int lgN = 0, rc = get_twiddles((int)lg_max, &tw, &lgN);
+    if (rc) return rc;
+    std::vector<Fr*> table;                                   // the pointers of every size, size by size
+    table.reserve(count);
+    for (auto& g : by_lg) table.insert(table.end(), g.second.begin(), g.second.end());
+    Fr** d_table = nullptr;
+    if ((rc = (int)pool_alloc(&d_table, count * sizeof(Fr*), stream)) != 0) return rc;
+    rc = (int)cudaMemcpyAsync(d_table, table.data(), count * sizeof(Fr*), cudaMemcpyHostToDevice, stream);
+    size_t first = 0;
+    for (auto it = by_lg.begin(); rc == 0 && it != by_lg.end(); ++it) {
+        const uint32_t lg = it->first;
+        const size_t n = it->second.size();
+        NttPass passes[8];
+        int P = 0;
+        if ((rc = ntt_make_passes(lg, passes, &P)) != 0) break;
+        Fr* scratch = nullptr;
+        if (P > 1 && (rc = (int)pool_alloc(&scratch, (n << lg) * sizeof(Fr), stream)) != 0) break;
+        for (int p = 0; p < P && rc == 0; p++) {
+            PassArgs a;
+            if ((rc = pass_args(lg, direction, type, p, passes, P, &a)) != 0) break;
+            a.in_batch = p == 0;
+            a.out_batch = P == 1 || a.last;
+            ProfScope pass_scope(PROF_NTT_PASS, stream);
+            for (size_t y0 = 0; y0 < n && rc == 0; y0 += NTT_BATCH_GRID_Y) {
+                const size_t ny = n - y0 < NTT_BATCH_GRID_Y ? n - y0 : NTT_BATCH_GRID_Y;
+                a.batch = d_table + first + y0;
+                a.in = a.out = scratch + (y0 << lg);
+                k_ntt_pass<true><<<dim3((unsigned)passes[p].tiles, (unsigned)ny), 256, pass_smem(a), stream>>>(a);
+                count_launch();
+                rc = (int)cudaGetLastError();
+            }
+        }
+        if (scratch) cudaFreeAsync(scratch, stream);
+        first += n;
+    }
+    cudaFreeAsync(d_table, stream);
+    return rc;
 }
 
 int ntt_device(void* d_inout, uint32_t lg, int direction, int type, void* d_scratch, cudaStream_t stream) {

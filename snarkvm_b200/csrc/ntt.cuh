@@ -26,6 +26,10 @@ enum NttType { NTT_STANDARD = 0, NTT_COSET = 1 };
 // is taken from the stream-ordered pool).  Returns cudaError_t as int.
 int ntt_device(void* d_inout, uint32_t lg, int direction, int type, void* d_scratch, cudaStream_t stream);
 
+// `count` in-place transforms, transform i of 2^lgs[i] elements at d_data[i] (HOST array of device pointers), all with the same
+// direction and type and each with ntt_device's result.  Transforms of equal size share their launches; sizes may be mixed.
+int ntt_batch_device(void* const* d_data, const uint32_t* lgs, size_t count, int direction, int type, cudaStream_t stream);
+
 // One transform = ntt_make_passes(lg) passes; pass p may be launched in tile ranges (see ntt.cu for the tile ↔ column-range map).
 struct NttPass { int t0, S, Q; size_t tiles; };
 int ntt_make_passes(uint32_t lg, NttPass* out /* ≥ 8 entries */, int* npasses);

@@ -13,8 +13,13 @@
 // Every result is a canonical Fr value, so any correct evaluation order is bit-identical to the reference's.
 #include "poly.cuh"
 
+#include <algorithm>
+#include <cstring>
+#include <vector>
+
 #include "ff.cuh"
 #include "msm.cuh"   // count_launch, ensure_pool_configured
+#include "ntt.cuh"   // NTT_MAX_LG
 
 namespace b200 {
 
@@ -490,12 +495,36 @@ FF_DEV void csr_check_bounds(const CsrArgs& m, int* bad) {
     if (blockIdx.x == 0 && threadIdx.x == 0 && (m.row_ptr[0] != 0 || m.row_ptr[m.nrows] != m.nnz)) *bad = 1;
 }
 
-__global__ void k_matrix_evals(CsrArgs m, uint64_t K, const uint32_t* __restrict__ tw, int lgN, int lgR, int lgC,
-                               uint32_t* __restrict__ row_out, uint32_t* __restrict__ col_out, uint32_t* __restrict__ rcv_out,
-                               int* __restrict__ bad) {
-    const size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    csr_check_bounds(m, bad);
-    if (e >= K) return;
+// Segmented launches: thread g of the grid belongs to the last segment whose `first` is ≤ g (segments hold consecutive ranges of
+// the grid; empty ones are skipped by the search).
+template <class Seg> FF_DEV uint32_t seg_of(const Seg* __restrict__ segs, uint32_t nsegs, uint64_t g) {
+    uint32_t lo = 0, hi = nsegs;
+    while (hi - lo > 1) {
+        const uint32_t mid = lo + (hi - lo) / 2;
+        if (segs[mid].first <= g) lo = mid; else hi = mid;
+    }
+    return lo;
+}
+
+struct EvalsSeg {
+    CsrArgs m;
+    uint32_t *row_out, *col_out, *rcv_out;
+    uint64_t first, K;
+    int lgR, lgC;
+};
+// one launch over every matrix's K: entry e of segment j; bad[j] is the segment's flag
+__global__ void k_matrix_evals(const EvalsSeg* __restrict__ segs, uint32_t nsegs, uint64_t total, const uint32_t* __restrict__ tw, int lgN,
+                               int* __restrict__ bad_flags) {
+    const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= total) return;
+    const uint32_t j = seg_of(segs, nsegs, g);
+    const EvalsSeg& s = segs[j];
+    const CsrArgs m = s.m;
+    const size_t e = g - s.first;
+    int* bad = bad_flags + j;
+    uint32_t *row_out = s.row_out, *col_out = s.col_out, *rcv_out = s.rcv_out;
+    const int lgR = s.lgR, lgC = s.lgC;
+    if (e == 0 && (m.row_ptr[0] != 0 || m.row_ptr[m.nrows] != m.nnz)) *bad = 1;
     if (e >= m.nnz) {                                                       // padding (matrices.rs:174-181)
         Fr::one().store(row_out + e * 8); Fr::one().store(col_out + e * 8); Fr::zero().store(rcv_out + e * 8);
         return;
@@ -606,31 +635,76 @@ static int csr_finish(int rc, uint8_t* scratch, const int* bad, cudaStream_t str
     return rc;
 }
 
-int varuna_matrix_evals_device(void* d_row, void* d_col, void* d_row_col_val, const void* d_row_ptr, size_t nrows, const void* d_cols,
-                               const void* d_vals, size_t nnz, size_t nvars, size_t input_size, uint32_t lg_constraint,
-                               uint32_t lg_variable, uint32_t lg_non_zero, cudaStream_t stream) {
-    CsrArgs m;
-    int rc = csr_index_args(&m, d_row_ptr, nrows, d_cols, d_vals, nnz, nvars, input_size, lg_variable);
-    if (rc != 0) return rc;
-    if (!d_row || !d_col || !d_row_col_val || lg_constraint > 31 || lg_non_zero > 31) return (int)cudaErrorInvalidValue;
-    if (nrows > ((size_t)1 << lg_constraint) || nnz > ((size_t)1 << lg_non_zero)) return (int)cudaErrorInvalidValue;
-    const uint32_t lg_max = lg_constraint > lg_variable ? lg_constraint : lg_variable;
-    const void* tw = nullptr;
-    int lgN = 0;
-    if ((rc = ntt_get_twiddles((int)lg_max, &tw, &lgN)) != 0) return rc;
-    uint8_t* scratch = nullptr;
-    cudaError_t e = pool_alloc(&scratch, 256, stream);
+// Scratch of a segmented call: [bad flags, one int per segment | the segment table]; the table is copied up and the flags cleared.
+template <class Seg> static int seg_scratch(const std::vector<Seg>& table, uint8_t** scratch, int** bad, Seg** d_table, cudaStream_t stream) {
+    const size_t nflags = (table.size() * sizeof(int) + 255) & ~(size_t)255;
+    cudaError_t e = pool_alloc(scratch, nflags + table.size() * sizeof(Seg), stream);
     if (e != cudaSuccess) return (int)e;
-    int* bad = (int*)scratch;
-    rc = (int)cudaMemsetAsync(bad, 0, sizeof(int), stream);
-    const size_t K = (size_t)1 << lg_non_zero;
+    *bad = (int*)*scratch;
+    *d_table = (Seg*)(*scratch + nflags);
+    int rc = (int)cudaMemsetAsync(*scratch, 0, nflags, stream);
+    if (rc == 0) rc = (int)cudaMemcpyAsync(*d_table, table.data(), table.size() * sizeof(Seg), cudaMemcpyHostToDevice, stream);
+    return rc;
+}
+// reads every segment's bad flag back (one synchronisation), frees the scratch and names the first bad segment
+static int seg_finish(int rc, uint8_t* scratch, const int* bad, size_t count, int64_t* bad_segment, cudaStream_t stream) {
+    std::vector<int> h_bad(count, 0);
+    if (rc == 0) rc = (int)cudaMemcpyAsync(h_bad.data(), bad, count * sizeof(int), cudaMemcpyDeviceToHost, stream);
+    cudaFreeAsync(scratch, stream);
+    if (rc == 0) rc = (int)cudaStreamSynchronize(stream);
+    if (rc != 0) return rc;
+    for (size_t i = 0; i < count; i++) {
+        if (h_bad[i]) {
+            if (bad_segment) *bad_segment = (int64_t)i;
+            return (int)cudaErrorInvalidValue;
+        }
+    }
+    return 0;
+}
+
+int varuna_matrix_evals_batch_device(const snarkvm_b200_csr_segment_t* segs, size_t count, int64_t* bad_segment, cudaStream_t stream) {
+    if (bad_segment) *bad_segment = -1;
+    if (count == 0) return 0;
+    if (!segs || count >= ((size_t)1 << 31)) return (int)cudaErrorInvalidValue;
+    std::vector<EvalsSeg> table(count);
+    uint64_t total = 0;
+    uint32_t lg_max = 0;
+    for (size_t i = 0; i < count; i++) {
+        const snarkvm_b200_csr_segment_t& s = segs[i];
+        EvalsSeg& t = table[i];
+        int rc = csr_index_args(&t.m, s.d_row_ptr, s.nrows, s.d_cols, s.d_vals, s.nnz, s.nvars, s.input_size, s.lg_variable);
+        if (rc != 0) return rc;
+        if (!s.d_out[0] || !s.d_out[1] || !s.d_out[2] || s.lg_constraint > 31 || s.lg_non_zero > 31) return (int)cudaErrorInvalidValue;
+        if (s.nrows > ((uint64_t)1 << s.lg_constraint) || s.nnz > ((uint64_t)1 << s.lg_non_zero)) return (int)cudaErrorInvalidValue;
+        t.row_out = (uint32_t*)s.d_out[0]; t.col_out = (uint32_t*)s.d_out[1]; t.rcv_out = (uint32_t*)s.d_out[2];
+        t.first = total;
+        t.K = (uint64_t)1 << s.lg_non_zero;
+        t.lgR = (int)s.lg_constraint; t.lgC = (int)s.lg_variable;
+        total += t.K;
+        lg_max = std::max(lg_max, std::max(s.lg_constraint, s.lg_variable));
+    }
+    const void* tw = nullptr;
+    int lgN = 0, rc = ntt_get_twiddles((int)lg_max, &tw, &lgN);
+    if (rc != 0) return rc;
+    uint8_t* scratch = nullptr;
+    int* bad = nullptr;
+    EvalsSeg* d_table = nullptr;
+    rc = seg_scratch(table, &scratch, &bad, &d_table, stream);
+    if (rc != 0 && !scratch) return rc;
     if (rc == 0) {
-        k_matrix_evals<<<(unsigned)((K + 255) / 256), 256, 0, stream>>>(m, K, (const uint32_t*)tw, lgN, (int)lg_constraint, (int)lg_variable,
-                                                                        (uint32_t*)d_row, (uint32_t*)d_col, (uint32_t*)d_row_col_val, bad);
+        k_matrix_evals<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(d_table, (uint32_t)count, total, (const uint32_t*)tw, lgN, bad);
         count_launch();
         rc = (int)cudaGetLastError();
     }
-    return csr_finish(rc, scratch, bad, stream);
+    return seg_finish(rc, scratch, bad, count, bad_segment, stream);
+}
+
+int varuna_matrix_evals_device(void* d_row, void* d_col, void* d_row_col_val, const void* d_row_ptr, size_t nrows, const void* d_cols,
+                               const void* d_vals, size_t nnz, size_t nvars, size_t input_size, uint32_t lg_constraint,
+                               uint32_t lg_variable, uint32_t lg_non_zero, cudaStream_t stream) {
+    const snarkvm_b200_csr_segment_t s{d_row_ptr, d_cols, d_vals, nrows, nnz, nvars, input_size, lg_constraint, lg_variable, lg_non_zero, 0,
+                                       {d_row, d_col, d_row_col_val}};
+    return varuna_matrix_evals_batch_device(&s, 1, nullptr, stream);
 }
 
 int csr_transpose_device(void* d_t_row_ptr, void* d_t_cols, void* d_t_vals, const void* d_row_ptr, size_t nrows, const void* d_cols,
@@ -676,9 +750,20 @@ int csr_transpose_device(void* d_t_row_ptr, void* d_t_cols, void* d_t_vals, cons
 // thread per entry (Montgomery → canonical fused in) and one per row header.  A row_ptr that is not non-decreasing from 0 to nnz
 // raises the bad flag; its row header is then not written, and no thread writes outside the 8 + 8·nrows + 40·nnz bytes.
 // ---------------------------------------------------------------------------------------------------------------------
-__global__ void k_csr_serialize(CsrArgs m, uint8_t* __restrict__ out, int* __restrict__ bad) {
-    const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    csr_check_bounds(m, bad);
+struct SerializeSeg {
+    CsrArgs m;
+    uint8_t* out;
+    uint64_t first;                                     // nnz + nrows + 1 threads per segment
+};
+__global__ void k_csr_serialize(const SerializeSeg* __restrict__ segs, uint32_t nsegs, uint64_t total, int* __restrict__ bad_flags) {
+    const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= total) return;
+    const uint32_t j = seg_of(segs, nsegs, g);
+    const CsrArgs m = segs[j].m;
+    uint8_t* __restrict__ out = segs[j].out;
+    int* bad = bad_flags + j;
+    const size_t t = g - segs[j].first;
+    if (t == 0 && (m.row_ptr[0] != 0 || m.row_ptr[m.nrows] != m.nnz)) *bad = 1;
     if (t < m.nnz) {
         const uint32_t e = (uint32_t)t, r = csr_row_of(m.row_ptr, m.nrows, e);
         uint64_t* dst = reinterpret_cast<uint64_t*>(out + 16 + 8 * (size_t)r + 40 * (size_t)e);
@@ -695,24 +780,41 @@ __global__ void k_csr_serialize(CsrArgs m, uint8_t* __restrict__ out, int* __res
     }
 }
 
-int csr_serialize_device(void* d_out, size_t out_bytes, const void* d_row_ptr, size_t nrows, const void* d_cols, const void* d_vals, size_t nnz,
-                         cudaStream_t stream) {
-    if (!d_out || !d_row_ptr || (nnz && (!d_cols || !d_vals))) return (int)cudaErrorInvalidValue;
-    if (nrows >= ((size_t)1 << 32) || nnz >= ((size_t)1 << 32) || out_bytes != 8 + 8 * nrows + 40 * nnz) return (int)cudaErrorInvalidValue;
-    if ((nnz && !nrows) || ((uintptr_t)d_out & 7)) return (int)cudaErrorInvalidValue;
-    const CsrArgs m{(const uint32_t*)d_row_ptr, (const uint32_t*)d_cols, (const uint32_t*)d_vals, (uint32_t)nrows, (uint32_t)nnz, 0, 0, 0};
+int csr_serialize_batch_device(const snarkvm_b200_csr_segment_t* segs, size_t count, int64_t* bad_segment, cudaStream_t stream) {
+    if (bad_segment) *bad_segment = -1;
+    if (count == 0) return 0;
+    if (!segs || count >= ((size_t)1 << 31)) return (int)cudaErrorInvalidValue;
+    std::vector<SerializeSeg> table(count);
+    uint64_t total = 0;
+    for (size_t i = 0; i < count; i++) {
+        const snarkvm_b200_csr_segment_t& s = segs[i];
+        if (!s.d_out[0] || !s.d_row_ptr || (s.nnz && (!s.d_cols || !s.d_vals))) return (int)cudaErrorInvalidValue;
+        if (s.nrows >= ((uint64_t)1 << 32) || s.nnz >= ((uint64_t)1 << 32)) return (int)cudaErrorInvalidValue;
+        if ((s.nnz && !s.nrows) || ((uintptr_t)s.d_out[0] & 7)) return (int)cudaErrorInvalidValue;
+        table[i].m = CsrArgs{(const uint32_t*)s.d_row_ptr, (const uint32_t*)s.d_cols, (const uint32_t*)s.d_vals, (uint32_t)s.nrows,
+                             (uint32_t)s.nnz, 0, 0, 0};
+        table[i].out = (uint8_t*)s.d_out[0];
+        table[i].first = total;
+        total += s.nnz + s.nrows + 1;
+    }
     uint8_t* scratch = nullptr;
-    cudaError_t e = pool_alloc(&scratch, 256, stream);
-    if (e != cudaSuccess) return (int)e;
-    int* bad = (int*)scratch;
-    int rc = (int)cudaMemsetAsync(bad, 0, sizeof(int), stream);
+    int* bad = nullptr;
+    SerializeSeg* d_table = nullptr;
+    int rc = seg_scratch(table, &scratch, &bad, &d_table, stream);
+    if (rc != 0 && !scratch) return rc;
     if (rc == 0) {
-        const size_t threads = nnz + nrows + 1;
-        k_csr_serialize<<<(unsigned)((threads + 255) / 256), 256, 0, stream>>>(m, (uint8_t*)d_out, bad);
+        k_csr_serialize<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(d_table, (uint32_t)count, total, bad);
         count_launch();
         rc = (int)cudaGetLastError();
     }
-    return csr_finish(rc, scratch, bad, stream);
+    return seg_finish(rc, scratch, bad, count, bad_segment, stream);
+}
+
+int csr_serialize_device(void* d_out, size_t out_bytes, const void* d_row_ptr, size_t nrows, const void* d_cols, const void* d_vals, size_t nnz,
+                         cudaStream_t stream) {
+    if (nrows >= ((size_t)1 << 32) || nnz >= ((size_t)1 << 32) || out_bytes != 8 + 8 * nrows + 40 * nnz) return (int)cudaErrorInvalidValue;
+    const snarkvm_b200_csr_segment_t s{d_row_ptr, d_cols, d_vals, nrows, nnz, 0, 0, 0, 0, 0, 0, {d_out, nullptr, nullptr}};
+    return csr_serialize_batch_device(&s, 1, nullptr, stream);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -720,46 +822,85 @@ int csr_serialize_device(void* d_out, size_t out_bytes, const void* d_row_ptr, s
 // once instead of once per term (the poly_axpy loop).  A term whose coefficient is one adds p_j without the product; zero
 // coefficients and empty terms are dropped on the host.  Field sums are exact, so the result is the axpy sequence's bit for bit.
 // ---------------------------------------------------------------------------------------------------------------------
+// Segmented: every output of a batch (one per circuit) in one launch; thread g writes coefficient g − first of its segment.
 static constexpr int LINCOMB_MAX = 12;
-struct LincombArgs {
+struct LincombSeg {
+    uint32_t* out;
+    uint64_t n, first;
     const uint32_t* p[LINCOMB_MAX];
     uint64_t len[LINCOMB_MAX];
     FrArg c[LINCOMB_MAX];
     uint32_t nterms;
 };
-__global__ void k_fr_lincomb(uint32_t* __restrict__ out, size_t n, LincombArgs a) {
-    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
+__global__ void k_fr_lincomb(const LincombSeg* __restrict__ segs, uint32_t nsegs, uint64_t total) {
+    const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= total) return;
+    const LincombSeg& a = segs[seg_of(segs, nsegs, g)];
+    const size_t i = g - a.first;
     Fr acc = Fr::zero();
     for (uint32_t j = 0; j < a.nterms; j++) {
         if (i >= a.len[j]) continue;
         const Fr x = Fr::load_ldg(a.p[j] + i * 8), c = fr_from_arg(a.c[j]);
         acc = acc + (c == Fr::one() ? x : c * x);
     }
-    acc.store(out + i * 8);
+    acc.store(a.out + i * 8);
+}
+
+int fr_lincomb_batch_device(const snarkvm_b200_lincomb_segment_t* segs, size_t count, cudaStream_t stream) {
+    if (count == 0) return 0;
+    if (!segs || count >= ((size_t)1 << 31)) return (int)cudaErrorInvalidValue;
+    std::vector<LincombSeg> table;
+    uint64_t total = 0;
+    for (size_t i = 0; i < count; i++) {
+        const snarkvm_b200_lincomb_segment_t& s = segs[i];
+        if (s.nterms > LINCOMB_MAX || (s.n && !s.d_out)) return (int)cudaErrorInvalidValue;
+        LincombSeg a{};
+        a.out = (uint32_t*)s.d_out;
+        a.n = s.n;
+        a.first = total;
+        for (uint32_t j = 0; j < s.nterms; j++) {
+            if (s.lens[j] > s.n || (s.lens[j] && !s.d_polys[j])) return (int)cudaErrorInvalidValue;
+            FrArg c;
+            memcpy(c.v, s.coeffs_mont[j], 32);
+            bool zero = true;
+            for (int k = 0; k < 8; k++) zero &= c.v[k] == 0;
+            if (s.lens[j] == 0 || zero) continue;                                  // zero coefficients and empty terms are dropped
+            a.p[a.nterms] = (const uint32_t*)s.d_polys[j];
+            a.len[a.nterms] = s.lens[j];
+            a.c[a.nterms] = c;
+            a.nterms++;
+        }
+        if (s.n == 0) continue;
+        table.push_back(a);
+        total += s.n;
+    }
+    if (total == 0) return 0;
+    LincombSeg* d_table = nullptr;
+    cudaError_t e = pool_alloc(&d_table, table.size() * sizeof(LincombSeg), stream);
+    if (e != cudaSuccess) return (int)e;
+    int rc = (int)cudaMemcpyAsync(d_table, table.data(), table.size() * sizeof(LincombSeg), cudaMemcpyHostToDevice, stream);
+    if (rc == 0) {
+        k_fr_lincomb<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(d_table, (uint32_t)table.size(), total);
+        count_launch();
+        rc = (int)cudaGetLastError();
+    }
+    cudaFreeAsync(d_table, stream);
+    return rc;
 }
 
 int fr_lincomb_device(void* d_out, size_t n, const void* const* d_polys, const size_t* lens, const void* coeffs_mont_host, uint32_t nterms,
                       cudaStream_t stream) {
     if (nterms > LINCOMB_MAX || (nterms && (!d_polys || !lens || !coeffs_mont_host))) return (int)cudaErrorInvalidValue;
-    if (n && !d_out) return (int)cudaErrorInvalidValue;
-    LincombArgs a{};
+    snarkvm_b200_lincomb_segment_t s{};
+    s.d_out = d_out;
+    s.n = n;
+    s.nterms = nterms;
     for (uint32_t j = 0; j < nterms; j++) {
-        if (lens[j] > n || (lens[j] && !d_polys[j])) return (int)cudaErrorInvalidValue;
-        FrArg c;
-        memcpy(c.v, (const uint8_t*)coeffs_mont_host + 32 * (size_t)j, 32);
-        bool zero = true;
-        for (int k = 0; k < 8; k++) zero &= c.v[k] == 0;
-        if (lens[j] == 0 || zero) continue;
-        a.p[a.nterms] = (const uint32_t*)d_polys[j];
-        a.len[a.nterms] = lens[j];
-        a.c[a.nterms] = c;
-        a.nterms++;
+        s.d_polys[j] = d_polys[j];
+        s.lens[j] = lens[j];
+        memcpy(s.coeffs_mont[j], (const uint8_t*)coeffs_mont_host + 32 * (size_t)j, 32);
     }
-    if (n == 0) return 0;
-    k_fr_lincomb<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>((uint32_t*)d_out, n, a);
-    count_launch();
-    return (int)cudaGetLastError();
+    return fr_lincomb_batch_device(&s, 1, stream);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -768,14 +909,58 @@ int fr_lincomb_device(void* d_out, size_t n, const void* const* d_polys, const s
 // on the fly (the device index keeps no row_col vector).  Stage 1: one launch over the whole matrix, grid-stride, every CTA
 // reduces its four partials in shared memory; stage 2: one CTA per product adds the per-CTA partials.
 // ---------------------------------------------------------------------------------------------------------------------
+//
+// Segmented over many matrices (each with its own K and point): segment j owns CTAs [cta0, cta0 + nctas) of the first launch and
+// the four finishing CTAs 4j … 4j + 3 of the second.  Its Lagrange coefficients are either given (`lag`, `computed` = 0) or formed
+// on the fly from the inverted denominators 1/(ω^i − τ) that one batch inversion left in `lag` (fft/domain.rs:277-291):
+// L_i = c·ω^i/(ω^i − τ) with c = (1 − τ^n)/n.  When τ lies in K, c = 0 and the one zero denominator (left zero by the inversion)
+// marks the indicator position (domain.rs:264-275).
 static constexpr unsigned DOT_MAX_CTAS = 1024;
-__global__ void __launch_bounds__(EVAL_THREADS) k_matrix_evals_dot(const uint32_t* __restrict__ row, const uint32_t* __restrict__ col,
-                                                                    const uint32_t* __restrict__ rcv, const uint32_t* __restrict__ lag,
-                                                                    size_t n, uint32_t* __restrict__ partial /* [4][gridDim.x] */) {
+struct DotSeg {
+    const uint32_t *row, *col, *rcv, *lag;
+    uint64_t n, first;                                  // first: the segment's offset in the concatenated denominators
+    FrArg tau;
+    uint32_t lg, cta0, nctas, computed;
+};
+FF_DEV uint32_t dot_seg_of_cta(const DotSeg* __restrict__ segs, uint32_t nsegs, uint32_t b) {
+    uint32_t lo = 0, hi = nsegs;
+    while (hi - lo > 1) {
+        const uint32_t mid = lo + (hi - lo) / 2;
+        if (segs[mid].cta0 <= b) lo = mid; else hi = mid;
+    }
+    return lo;
+}
+// den[first + i] = ω_K^i − τ for every segment, and scale[j] = (1 − τ^n)/n
+__global__ void k_lagrange_denominators(const DotSeg* __restrict__ segs, uint32_t nsegs, uint64_t total, const uint32_t* __restrict__ tw, int lgN,
+                                        uint32_t* __restrict__ den, uint32_t* __restrict__ scale) {
+    const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= total) return;
+    const uint32_t j = seg_of(segs, nsegs, g);
+    const DotSeg& s = segs[j];
+    const size_t i = g - s.first;
+    const Fr tau = fr_from_arg(s.tau);
+    (domain_element(i, (int)s.lg, tw, lgN) - tau).store(den + g * 8);
+    if (i == 0) {
+        Fr c = Fr::one() - fr_pow_u64(tau, s.n);
+        for (uint32_t k = 0; k < s.lg; k++) c = c.half();
+        c.store(scale + (size_t)j * 8);
+    }
+}
+__global__ void __launch_bounds__(EVAL_THREADS) k_matrix_evals_dot(const DotSeg* __restrict__ segs, uint32_t nsegs, uint32_t total_ctas,
+                                                                    const uint32_t* __restrict__ tw, int lgN, const uint32_t* __restrict__ scale,
+                                                                    uint32_t* __restrict__ partial /* [4][total_ctas] */) {
     __shared__ uint4 sh4[EVAL_THREADS * 2];
+    const uint32_t j = dot_seg_of_cta(segs, nsegs, blockIdx.x);
+    const DotSeg& sg = segs[j];
+    const uint32_t *row = sg.row, *col = sg.col, *rcv = sg.rcv, *lag = sg.lag;
+    const size_t n = sg.n, stride = (size_t)sg.nctas * blockDim.x;
+    const bool computed = sg.computed != 0;
+    const Fr c_j = computed ? Fr::load(scale + (size_t)j * 8) : Fr::zero();
     Fr s[4] = {Fr::zero(), Fr::zero(), Fr::zero(), Fr::zero()};
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-        const Fr l = Fr::load_ldg(lag + i * 8), lr = l * Fr::load_ldg(row + i * 8), c = Fr::load_ldg(col + i * 8);
+    for (size_t i = (size_t)(blockIdx.x - sg.cta0) * blockDim.x + threadIdx.x; i < n; i += stride) {
+        Fr l = Fr::load_ldg(lag + i * 8);
+        if (computed) l = l.is_zero() ? Fr::one() : c_j * l * domain_element(i, (int)sg.lg, tw, lgN);
+        const Fr lr = l * Fr::load_ldg(row + i * 8), c = Fr::load_ldg(col + i * 8);
         s[0] = s[0] + lr;
         s[1] = s[1] + l * c;
         s[2] = s[2] + lr * c;
@@ -784,9 +969,72 @@ __global__ void __launch_bounds__(EVAL_THREADS) k_matrix_evals_dot(const uint32_
 #pragma unroll
     for (int k = 0; k < 4; k++) {
         const Fr t = cta_sum(s[k], reinterpret_cast<uint32_t*>(sh4));
-        if (threadIdx.x == 0) t.store(partial + ((size_t)k * gridDim.x + blockIdx.x) * 8);
+        if (threadIdx.x == 0) t.store(partial + ((size_t)k * total_ctas + blockIdx.x) * 8);
         __syncthreads();
     }
+}
+// CTA 4j + k adds segment j's partials of product k
+__global__ void __launch_bounds__(EVAL_THREADS) k_fr_sum_segments(const DotSeg* __restrict__ segs, const uint32_t* __restrict__ partial,
+                                                                   uint32_t total_ctas, uint32_t* __restrict__ out) {
+    __shared__ uint4 sh4[EVAL_THREADS * 2];
+    const uint32_t j = blockIdx.x / 4, k = blockIdx.x % 4;
+    const uint32_t* in = partial + ((size_t)k * total_ctas + segs[j].cta0) * 8;
+    Fr acc = Fr::zero();
+    for (uint32_t i = threadIdx.x; i < segs[j].nctas; i += EVAL_THREADS) acc = acc + Fr::load_ldg(in + (size_t)i * 8);
+    const Fr s = cta_sum(acc, reinterpret_cast<uint32_t*>(sh4));
+    if (threadIdx.x == 0) s.store(out + (size_t)blockIdx.x * 8);
+}
+
+// table: the segments with row / col / rcv (and lag unless computed) set; runs the Lagrange denominators and their one batch
+// inversion when any segment is `computed`, then the dot and finishing launches, one D2H and one synchronisation
+static int evals_dot_impl(void* out_mont_host, std::vector<DotSeg>& table, cudaStream_t stream) {
+    const size_t count = table.size();
+    uint64_t total_den = 0;
+    uint32_t total_ctas = 0, lg_max = 0;
+    bool any_computed = false;
+    for (DotSeg& s : table) {
+        const size_t blocks = std::min<size_t>((s.n + EVAL_THREADS - 1) / EVAL_THREADS, DOT_MAX_CTAS);
+        s.cta0 = total_ctas;
+        s.nctas = (uint32_t)blocks;
+        total_ctas += (uint32_t)blocks;
+        s.first = total_den;
+        if (s.computed) { total_den += s.n; any_computed = true; lg_max = std::max(lg_max, s.lg); }
+    }
+    if (total_ctas == 0) { memset(out_mont_host, 0, count * 4 * 32); return 0; }
+    const void* tw = nullptr;
+    int lgN = 0, rc = 0;
+    if (any_computed && (rc = ntt_get_twiddles((int)lg_max, &tw, &lgN)) != 0) return rc;
+    // scratch: table | scale[count] | den[total_den] | partial[4][total_ctas] | out[count][4]
+    const size_t off_scale = (count * sizeof(DotSeg) + 255) & ~(size_t)255, off_den = off_scale + count * 32,
+                 off_partial = off_den + total_den * 32, off_out = off_partial + (size_t)4 * total_ctas * 32, bytes = off_out + count * 4 * 32;
+    uint8_t* scratch = nullptr;
+    cudaError_t e = pool_alloc(&scratch, bytes, stream);
+    if (e != cudaSuccess) return (int)e;
+    uint32_t *scale = (uint32_t*)(scratch + off_scale), *den = (uint32_t*)(scratch + off_den), *partial = (uint32_t*)(scratch + off_partial),
+             *out = (uint32_t*)(scratch + off_out);
+    for (DotSeg& s : table) if (s.computed) s.lag = den + s.first * 8;
+    DotSeg* d_table = (DotSeg*)scratch;
+    rc = (int)cudaMemcpyAsync(d_table, table.data(), count * sizeof(DotSeg), cudaMemcpyHostToDevice, stream);
+    if (rc == 0 && total_den) {
+        // a table is either all computed (matrix_evals_at_points) or none (matrix_evals_dot), so `first` orders every segment
+        k_lagrange_denominators<<<(unsigned)((total_den + 255) / 256), 256, 0, stream>>>(d_table, (uint32_t)count, total_den, (const uint32_t*)tw,
+                                                                                         lgN, den, scale);
+        const size_t threads = (total_den + BINV_K - 1) / BINV_K;
+        FrArg one{};
+        for (int k = 0; k < 8; k++) one.v[k] = FrParams::r1(k);                     // Montgomery one
+        k_fr_batch_inverse<<<(unsigned)((threads + 127) / 128), 128, 0, stream>>>(den, total_den, one);
+        count_launch(2);
+    }
+    if (rc == 0) {
+        k_matrix_evals_dot<<<total_ctas, EVAL_THREADS, 0, stream>>>(d_table, (uint32_t)count, total_ctas, (const uint32_t*)tw, lgN, scale, partial);
+        k_fr_sum_segments<<<(unsigned)(4 * count), EVAL_THREADS, 0, stream>>>(d_table, partial, total_ctas, out);
+        count_launch(2);
+        rc = (int)cudaGetLastError();
+    }
+    if (rc == 0) rc = (int)cudaMemcpyAsync(out_mont_host, out, count * 4 * 32, cudaMemcpyDeviceToHost, stream);
+    cudaFreeAsync(scratch, stream);
+    if (rc == 0) rc = (int)cudaStreamSynchronize(stream);
+    return rc;
 }
 
 int matrix_evals_dot_device(void* out_mont_host, const void* d_row, const void* d_col, const void* d_row_col_val, const void* d_lagrange,
@@ -794,20 +1042,25 @@ int matrix_evals_dot_device(void* out_mont_host, const void* d_row, const void* 
     if (!out_mont_host) return (int)cudaErrorInvalidValue;
     if (n == 0) { memset(out_mont_host, 0, 4 * 32); return 0; }
     if (!d_row || !d_col || !d_row_col_val || !d_lagrange) return (int)cudaErrorInvalidValue;
-    size_t blocks = (n + EVAL_THREADS - 1) / EVAL_THREADS;
-    if (blocks > DOT_MAX_CTAS) blocks = DOT_MAX_CTAS;
-    uint32_t* scratch = nullptr;                             // partials [4][blocks], then the four sums
-    cudaError_t e = pool_alloc(&scratch, (4 * blocks + 4) * 32, stream);
-    if (e != cudaSuccess) return (int)e;
-    k_matrix_evals_dot<<<(unsigned)blocks, EVAL_THREADS, 0, stream>>>((const uint32_t*)d_row, (const uint32_t*)d_col,
-                                                                      (const uint32_t*)d_row_col_val, (const uint32_t*)d_lagrange, n, scratch);
-    k_fr_sum<<<4, EVAL_THREADS, 0, stream>>>(scratch, blocks, scratch + 4 * blocks * 8);
-    count_launch(2);
-    int rc = (int)cudaGetLastError();
-    if (rc == 0) rc = (int)cudaMemcpyAsync(out_mont_host, scratch + 4 * blocks * 8, 4 * 32, cudaMemcpyDeviceToHost, stream);
-    cudaFreeAsync(scratch, stream);
-    if (rc == 0) rc = (int)cudaStreamSynchronize(stream);
-    return rc;
+    std::vector<DotSeg> table(1);
+    table[0] = DotSeg{(const uint32_t*)d_row, (const uint32_t*)d_col, (const uint32_t*)d_row_col_val, (const uint32_t*)d_lagrange, n, 0, FrArg{}, 0, 0, 0, 0};
+    return evals_dot_impl(out_mont_host, table, stream);
+}
+
+int matrix_evals_at_points_device(void* out_mont_host, const snarkvm_b200_evals_segment_t* segs, size_t count, cudaStream_t stream) {
+    if (count == 0) return 0;
+    if (!out_mont_host || !segs || count >= ((size_t)1 << 24)) return (int)cudaErrorInvalidValue;
+    std::vector<DotSeg> table(count);
+    for (size_t i = 0; i < count; i++) {
+        const snarkvm_b200_evals_segment_t& s = segs[i];
+        if (s.n == 0 || (s.n & (s.n - 1)) || s.n > ((uint64_t)1 << NTT_MAX_LG) || !s.d_row || !s.d_col || !s.d_row_col_val)
+            return (int)cudaErrorInvalidValue;
+        DotSeg& t = table[i];
+        t = DotSeg{(const uint32_t*)s.d_row, (const uint32_t*)s.d_col, (const uint32_t*)s.d_row_col_val, nullptr, s.n, 0, FrArg{}, 0, 0, 0, 1};
+        memcpy(t.tau.v, s.point_mont, 32);
+        while (((uint64_t)1 << t.lg) < s.n) t.lg++;
+    }
+    return evals_dot_impl(out_mont_host, table, stream);
 }
 
 }  // namespace b200

@@ -4,6 +4,8 @@
 #include <cstdint>
 #include <cuda_runtime.h>
 
+#include "../../include/snarkvm_b200.h"   // the segment tables of the batched entry points
+
 namespace b200 {
 
 // v_i ← coeff · v_i^{-1} in place on n Montgomery Fr elements in HBM; zeros stay zero.  coeff: 32 B Montgomery, HOST memory.
@@ -54,6 +56,13 @@ int fr_lincomb_device(void* d_out, size_t n, const void* const* d_polys, const s
 // over n elements; synchronises the stream
 int matrix_evals_dot_device(void* out_mont_host, const void* d_row, const void* d_col, const void* d_row_col_val, const void* d_lagrange,
                             size_t n, cudaStream_t stream);
+
+// The segmented forms (one launch per job for many matrices; see include/snarkvm_b200.h).  The one-matrix entry points above are
+// one-segment calls of these.
+int varuna_matrix_evals_batch_device(const snarkvm_b200_csr_segment_t* segs, size_t count, int64_t* bad_segment, cudaStream_t stream);
+int csr_serialize_batch_device(const snarkvm_b200_csr_segment_t* segs, size_t count, int64_t* bad_segment, cudaStream_t stream);
+int fr_lincomb_batch_device(const snarkvm_b200_lincomb_segment_t* segs, size_t count, cudaStream_t stream);
+int matrix_evals_at_points_device(void* out_mont_host, const snarkvm_b200_evals_segment_t* segs, size_t count, cudaStream_t stream);
 
 // Group FFT over G1 (DomainCoeff = G1Projective, fft/domain.rs:169-221 generic path): n = 2^lg affine points in, affine points
 // out (natural order both sides).  direction 1 = inverse (includes n^{-1}): UniversalParams::lagrange_basis

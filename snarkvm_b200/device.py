@@ -482,6 +482,131 @@ def matrix_evals_dot(row: torch.Tensor, col: torch.Tensor, row_col_val: torch.Te
     return out
 
 
+def ntt_batch_(xs: list, direction: NTTDirection = NTTDirection.Forward, ntt_type: NTTType = NTTType.Standard) -> list:
+    """ntt_ of every tensor in `xs` (2^lg_i Fr each, sizes may differ, all on one device) in place, transforms of equal size sharing
+    their launches → xs"""
+    if not xs:
+        return xs
+    lgs = []
+    for x in xs:
+        n = _nbytes(x) // 32
+        if n <= 0 or n & (n - 1) or n * 32 != _nbytes(x):
+            raise ValueError("domain_size is not power of 2")
+        lgs.append(n.bit_length() - 1)
+    dev = xs[0].device
+    ptrs = (ctypes.c_void_p * len(xs))(*[_check(x, "x") for x in xs])
+    lg_arr = (ctypes.c_uint32 * len(xs))(*lgs)
+    with torch.cuda.device(dev):
+        _lib.check(_lib.lib().snarkvm_b200_ntt_batch_device(ptrs, lg_arr, len(xs), int(direction), int(ntt_type), _stream()))
+    return xs
+
+
+def _check_segments(code: int, bad: ctypes.c_int64) -> None:
+    if code != 0:
+        err = _lib.CudaError(code, f"segment {bad.value}" if bad.value >= 0 else "see cudaError_t")
+        err.segment = bad.value if bad.value >= 0 else None
+        raise err
+
+
+def _csr_segment(row_ptr: torch.Tensor, cols: torch.Tensor, vals: torch.Tensor, outs) -> "_lib.CsrSegment":
+    rp, nrows, cp, vp, nnz = _csr_args(row_ptr, cols, vals)
+    s = _lib.CsrSegment()
+    s.d_row_ptr, s.d_cols, s.d_vals, s.nrows, s.nnz = rp, cp, vp, nrows, nnz
+    for k, o in enumerate(outs):
+        s.d_out[k] = o
+    return s
+
+
+def varuna_matrix_evals_batch(specs: list) -> list:
+    """varuna_matrix_evals of every (row_ptr, cols, vals, nvars, input_size, lg_constraint, lg_variable, lg_non_zero) in `specs` in one
+    launch and one synchronisation → [(row, col, row_col_val)], views of one buffer.  A bad matrix raises CudaError whose `segment`
+    is the index of the first bad spec."""
+    if not specs:
+        return []
+    dev = specs[0][0].device
+    sizes = [1 << s[7] for s in specs]
+    buf = torch.empty((3 * sum(sizes), 4), dtype=torch.int64, device=dev)
+    segs = (_lib.CsrSegment * len(specs))()
+    outs, off = [], 0
+    for k, (spec, K) in enumerate(zip(specs, sizes)):
+        row_ptr, cols, vals, nvars, input_size, lg_r, lg_c, lg_k = spec
+        trio = (buf[off: off + K], buf[off + K: off + 2 * K], buf[off + 2 * K: off + 3 * K])
+        off += 3 * K
+        s = _csr_segment(row_ptr, cols, vals, [t.data_ptr() for t in trio])
+        s.nvars, s.input_size, s.lg_constraint, s.lg_variable, s.lg_non_zero = nvars, input_size, lg_r, lg_c, lg_k
+        segs[k] = s
+        outs.append(trio)
+    bad = ctypes.c_int64(-1)
+    with torch.cuda.device(dev):
+        _check_segments(_lib.lib().snarkvm_b200_varuna_matrix_evals_batch_device(segs, len(specs), ctypes.byref(bad), _stream()), bad)
+    return outs
+
+
+def csr_serialize_batch(mats: list) -> tuple:
+    """csr_serialize of every (row_ptr, cols, vals) in `mats` in one launch and one synchronisation → (CUDA uint8 buffer, byte offsets
+    [len(mats) + 1]): stream k is buffer[offsets[k]:offsets[k + 1]].  Errors as varuna_matrix_evals_batch."""
+    if not mats:
+        return torch.empty(0, dtype=torch.uint8), [0]
+    dev = mats[0][0].device
+    offsets = [0]
+    for row_ptr, cols, _vals in mats:
+        offsets.append(offsets[-1] + 8 + 8 * (row_ptr.numel() - 1) + 40 * cols.numel())
+    buf = torch.empty(offsets[-1] // 8, dtype=torch.int64, device=dev)          # int64 storage: every stream 8-byte aligned
+    segs = (_lib.CsrSegment * len(mats))()
+    for k, m in enumerate(mats):
+        segs[k] = _csr_segment(*m, [buf.data_ptr() + offsets[k]])
+    bad = ctypes.c_int64(-1)
+    with torch.cuda.device(dev):
+        _check_segments(_lib.lib().snarkvm_b200_csr_serialize_batch_device(segs, len(mats), ctypes.byref(bad), _stream()), bad)
+    return buf.view(torch.uint8), offsets
+
+
+def fr_lincomb_batch(jobs: list) -> list:
+    """fr_lincomb of every (polys, coeffs_mont) in `jobs` in one launch → one CUDA tensor per job, bit-identical to fr_lincomb"""
+    if not jobs:
+        return []
+    dev = jobs[0][0][0].device
+    segs = (_lib.LincombSegment * len(jobs))()
+    outs = []
+    for k, (polys, coeffs_mont) in enumerate(jobs):
+        if len(polys) != len(coeffs_mont) or not polys:
+            raise ValueError("one coefficient per polynomial, at least one polynomial")
+        if len(polys) > LINCOMB_MAX_TERMS:
+            raise ValueError(f"at most {LINCOMB_MAX_TERMS} polynomials")
+        lens = [_nbytes(p) // 32 for p in polys]
+        out = torch.empty((max(lens), 4), dtype=torch.int64, device=dev)
+        s = segs[k]
+        s.d_out, s.n, s.nterms = out.data_ptr() if out.numel() else None, out.shape[0], len(polys)
+        for j, (p, m, c) in enumerate(zip(polys, lens, coeffs_mont)):
+            s.d_polys[j] = _check(p, "poly") if m else None
+            s.lens[j] = m
+            ctypes.memmove(s.coeffs_mont[j], _fr_host(c).ctypes.data, 32)
+        outs.append(out)
+    with torch.cuda.device(dev):
+        _lib.check(_lib.lib().snarkvm_b200_fr_lincomb_batch_device(segs, len(jobs), _stream()))
+    return outs
+
+
+def matrix_evals_at_points(jobs: list) -> np.ndarray:
+    """For every (row, col, row_col_val, point_mont) in `jobs` (evaluations on a K of 2^k elements, the point a Montgomery Fr): the
+    Lagrange coefficients of K at the point and matrix_evals_dot's four inner products with them, all in one pass → uint64[count, 4, 4]
+    Montgomery on the host"""
+    out = np.zeros((len(jobs), 4, 4), dtype=np.uint64)
+    if not jobs:
+        return out
+    segs = (_lib.EvalsSegment * len(jobs))()
+    for k, (row, col, rcv, point) in enumerate(jobs):
+        n = _nbytes(row) // 32
+        if _nbytes(col) != n * 32 or _nbytes(rcv) != n * 32:
+            raise ValueError("length mismatch")
+        s = segs[k]
+        s.d_row, s.d_col, s.d_row_col_val, s.n = _check(row, "row"), _check(col, "col"), _check(rcv, "row_col_val"), n
+        ctypes.memmove(s.point_mont, _fr_host(point).ctypes.data, 32)
+    with torch.cuda.device(jobs[0][0].device):
+        _lib.check(_lib.lib().snarkvm_b200_matrix_evals_at_points_device(out.ctypes.data, segs, len(jobs), _stream()))
+    return out
+
+
 def poly_divide_by_linear(p: torch.Tensor, point_mont) -> torch.Tensor:
     """Quotient of p / (x − point), the KZG witness polynomial (kzg10/mod.rs:220-241) → CUDA tensor [m − 1, 4] i64, not trimmed."""
     z = _fr_host(point_mont)

@@ -30,13 +30,16 @@ from __future__ import annotations
 
 import hashlib
 import struct
+from concurrent.futures import ThreadPoolExecutor
 from dataclasses import dataclass
 
 import numpy as np
 import torch
 
 from . import device
+from ._lib import CudaError
 from .algorithms import EvaluationDomain, _fr_int_to_mont, _fr_mont_to_int
+from .cuda import NTTDirection, NTTType
 
 R_MOD = 8444461749428370424248824938781546531375899335154063827935233455917409239041   # curves/src/bls12_377/fr.rs:138-145
 
@@ -198,10 +201,16 @@ INDEX_POLYNOMIAL_NAMES = tuple(f"{p}_{m}" for p in ("col", "row", "row_col", "ro
 
 class Circuit:
     """AHPForR1CS::index_helper (ahp/indexer/indexer.rs:121-200) for the non-hiding mode: the caller has already padded the public
-    variables to a power of two (pad_input_for_indexer_and_prover, ahp/matrices.rs:85-100).  The evaluations on K and the
-    transposes are built on the device from the CSR arrays (device.varuna_matrix_evals, device.csr_transpose)."""
+    variables to a power of two (pad_input_for_indexer_and_prover, ahp/matrices.rs:85-100).  The evaluations on K are built on the
+    device from the CSR arrays (index_circuits, which indexes many circuits in one pass; this constructor is its batch of one).  The
+    transposes are prover data: they are built on first use (device.csr_transpose), so setup and certificates never pay for them."""
 
     def __init__(self, a: Matrix, b: Matrix, c: Matrix, num_public: int, num_variables: int):
+        self._shape(a, b, c, num_public, num_variables)
+        _matrix_evals([self])
+
+    def _shape(self, a: Matrix, b: Matrix, c: Matrix, num_public: int, num_variables: int):
+        """the domains and counts; no launch"""
         self.a, self.b, self.c = a, b, c
         self.num_public, self.num_variables, self.num_constraints = num_public, num_variables, a.nrows
         if num_public & (num_public - 1):
@@ -214,37 +223,26 @@ class Circuit:
         self.non_zero_domains = [EvaluationDomain.new(m.nnz) for m in (a, b, c)]
         self.max_non_zero_domain = max(self.non_zero_domains, key=lambda d: d.size)
         self.info = CircuitInfo(num_public, num_variables, self.num_constraints, a.nnz, b.nnz, c.nnz)
-        lg_r, lg_c = self.constraint_domain.log_size_of_group, self.variable_domain.log_size_of_group
-        self.ariths, self.transposes = [], []
-        for m, K in zip((a, b, c), self.non_zero_domains):
-            row, col, rcv = device.varuna_matrix_evals(m.row_ptr, m.cols, m.vals, num_variables, self.input_domain.size, lg_r, lg_c,
-                                                       K.log_size_of_group)
-            self.ariths.append(MatrixEvals(row, col, rcv, K))
-            self.transposes.append(Matrix.from_device(*device.csr_transpose(m.row_ptr, m.cols, m.vals, num_variables,
-                                                                            self.input_domain.size, lg_c)))
+        self.ariths, self._transposes = [], None
+
+    @property
+    def transposes(self) -> list:
+        """transpose (ahp/matrices.rs:249-270) of A, B, C over the variable domain, built on the first call"""
+        if self._transposes is None:
+            lg_c = self.variable_domain.log_size_of_group
+            self._transposes = [Matrix.from_device(*device.csr_transpose(m.row_ptr, m.cols, m.vals, self.num_variables,
+                                                                         self.input_domain.size, lg_c)) for m in (self.a, self.b, self.c)]
+        return self._transposes
 
     def index_polynomials(self) -> dict:
         """MatrixArithmetization::new (ahp/matrices.rs:211-240) for A, B, C: the iFFT over each matrix's K of row, col, row_col
         (= row∘col, padding 1·1 = 1) and row_col_val → {name: [|K|, 4] i64 Montgomery coefficients} in INDEX_POLYNOMIAL_NAMES order"""
-        out = {}
-        for m, arith in zip("abc", self.ariths):
-            K = arith.domain
-            out[f"row_{m}"] = K.ifft(arith.row)
-            out[f"col_{m}"] = K.ifft(arith.col)
-            out[f"row_col_{m}"] = K.ifft_in_place(device.fr_vec_op(arith.row, arith.col, device.FR_MUL))
-            out[f"row_col_val_{m}"] = K.ifft(arith.row_col_val)
-        return {name: out[name] for name in INDEX_POLYNOMIAL_NAMES}
+        return index_polynomials([self])[0]
 
     def id(self) -> bytes:
-        """Circuit::hash (ahp/indexer/circuit.rs:109-121): Blake2s-256 of CircuitInfo and of A, B, C serialized uncompressed.  Each
-        matrix's stream is built on the device and fed to the hash on its own (no single host blob).  Computed once, then cached."""
-        if self._id is None:
-            h = hashlib.blake2s(digest_size=32)
-            h.update(self.info.to_bytes_le())
-            for m in (self.a, self.b, self.c):
-                h.update(m.serialize().cpu().numpy().data)
-            self._id = h.digest()
-        return self._id
+        """Circuit::hash (ahp/indexer/circuit.rs:109-121): Blake2s-256 of CircuitInfo and of A, B, C serialized uncompressed
+        (circuit_ids for one circuit).  Computed once, then cached."""
+        return circuit_ids([self])[0]
 
     _id = None
 
@@ -252,17 +250,124 @@ class Circuit:
         """AHPForR1CS::evaluate_index_polynomials (ahp/indexer/indexer.rs:232-260): Σ_i combiners_i·p_i(point) over the twelve index
         polynomials in INDEX_POLYNOMIAL_NAMES (= label) order, from their evaluations on K through the Lagrange coefficients of each
         matrix's K at the point (a point inside K included, fft/domain.rs:258-292); no polynomial is interpolated."""
-        combiners = [int(c) % R_MOD for c in combiners]
-        if len(combiners) != len(INDEX_POLYNOMIAL_NAMES):
-            raise ValueError(f"{len(combiners)} combiners for {len(INDEX_POLYNOMIAL_NAMES)} index polynomials")
+        return evaluate_index_polynomials([self], [point], [combiners])[0]
+
+
+def _device_of(circuits: list):
+    """the one device every circuit lives on"""
+    devs = {c.a.row_ptr.device for c in circuits}
+    if len(devs) != 1:
+        raise ValueError(f"the circuits live on {len(devs)} devices; a batch runs on one")
+    return devs.pop()
+
+
+def _bad_circuit(err: "CudaError", per_circuit: int, positions=None):
+    """a segmented call's CudaError, re-raised naming the circuit (and matrix) of the first bad segment"""
+    seg = getattr(err, "segment", None)
+    if seg is None:
+        return err
+    k = seg // per_circuit if positions is None else positions[seg // per_circuit]
+    return CudaError(err.code, f"circuit {k}: matrix {'abc'[seg % per_circuit]} has a column ≥ num_variables or a row_ptr "
+                                           "that does not run from 0 to nnz")
+
+
+def _matrix_evals(circuits: list) -> None:
+    """matrix_evals (ahp/matrices.rs:138-195) of every matrix of every circuit: one launch, one synchronisation"""
+    specs = []
+    for c in circuits:
+        lg_r, lg_c = c.constraint_domain.log_size_of_group, c.variable_domain.log_size_of_group
+        for m, K in zip((c.a, c.b, c.c), c.non_zero_domains):
+            specs.append((m.row_ptr, m.cols, m.vals, c.num_variables, c.input_domain.size, lg_r, lg_c, K.log_size_of_group))
+    try:
+        outs = device.varuna_matrix_evals_batch(specs)
+    except CudaError as e:
+        raise _bad_circuit(e, 3) from None
+    for k, c in enumerate(circuits):
+        c.ariths = [MatrixEvals(*outs[3 * k + j], K) for j, K in enumerate(c.non_zero_domains)]
+
+
+def index_circuits(specs: list) -> list:
+    """AHPForR1CS::index_helper for many circuits at once: `specs` holds (a, b, c, num_public, num_variables) per circuit → [Circuit]
+    in input order, each equal to Circuit(*spec).  The evaluations of every matrix come from one launch and one synchronisation.  A
+    malformed matrix raises CudaError naming its circuit; circuits on different devices raise ValueError."""
+    if not specs:
+        raise ValueError("no circuits to index")
+    circuits = []
+    for spec in specs:
+        c = Circuit.__new__(Circuit)
+        c._shape(*spec)
+        circuits.append(c)
+    _device_of(circuits)
+    _matrix_evals(circuits)
+    return circuits
+
+
+def index_polynomials(circuits: list) -> list:
+    """Circuit.index_polynomials of every circuit → [dict], with all 12·K interpolations in one batched iNTT (transforms of equal |K|
+    share launches)"""
+    polys = []
+    for c in circuits:
+        out = {}
+        for m, arith in zip("abc", c.ariths):
+            out[f"row_{m}"] = arith.row.clone()
+            out[f"col_{m}"] = arith.col.clone()
+            out[f"row_col_{m}"] = device.fr_vec_op(arith.row, arith.col, device.FR_MUL)
+            out[f"row_col_val_{m}"] = arith.row_col_val.clone()
+        polys.append({name: out[name] for name in INDEX_POLYNOMIAL_NAMES})
+    device.ntt_batch_([t for p in polys for t in p.values()], NTTDirection.Inverse, NTTType.Standard)
+    return polys
+
+
+# Blake2s of the circuit ids runs on this many host threads: hashlib releases the GIL while it hashes a large buffer
+ID_HASH_THREADS = 8
+
+
+def circuit_ids(circuits: list) -> list:
+    """Circuit::hash of every circuit → [32-byte id], cached on each circuit.  The byte streams of all matrices not yet hashed come
+    from one launch and one synchronisation; one copy brings them to the host, where one Blake2s per circuit runs on a small thread
+    pool.  A malformed row_ptr raises CudaError naming its circuit."""
+    todo = [k for k, c in enumerate(circuits) if c._id is None]
+    todo = [k for i, k in enumerate(todo) if all(circuits[k] is not circuits[j] for j in todo[:i])]
+    if todo:
+        try:
+            buf, offs = device.csr_serialize_batch([(m.row_ptr, m.cols, m.vals) for k in todo for m in (circuits[k].a, circuits[k].b,
+                                                                                                         circuits[k].c)])
+        except CudaError as e:
+            raise _bad_circuit(e, 3, todo) from None
+        host = buf.cpu().numpy()
+
+        def digest(i: int) -> bytes:
+            h = hashlib.blake2s(digest_size=32)
+            h.update(circuits[todo[i]].info.to_bytes_le())
+            for j in range(3 * i, 3 * i + 3):
+                h.update(host[offs[j]: offs[j + 1]].data)
+            return h.digest()
+        if len(todo) == 1:
+            digests = [digest(0)]
+        else:
+            with ThreadPoolExecutor(min(ID_HASH_THREADS, len(todo))) as pool:
+                digests = list(pool.map(digest, range(len(todo))))
+        for k, d in zip(todo, digests):
+            circuits[k]._id = d
+    return [c._id for c in circuits]
+
+
+def evaluate_index_polynomials(circuits: list, points: list, combiners: list) -> list:
+    """Circuit.evaluate_index_polynomials of circuit k at points[k] with combiners[k], for every k → [int].  The Lagrange coefficients
+    of all 3·K domains share one batch inversion, and the 4·3·K inner products one pass and one synchronisation."""
+    combiners = [[int(c) % R_MOD for c in cs] for cs in combiners]
+    for cs in combiners:
+        if len(cs) != len(INDEX_POLYNOMIAL_NAMES):
+            raise ValueError(f"{len(cs)} combiners for {len(INDEX_POLYNOMIAL_NAMES)} index polynomials")
+    dots = device.matrix_evals_at_points([(a.row, a.col, a.row_col_val, _mont(int(p))) for c, p in zip(circuits, points) for a in c.ariths])
+    out = []
+    for k, cs in enumerate(combiners):
         evals = {}
-        dev = self.a.row_ptr.device
-        for m, arith in zip("abc", self.ariths):
-            lag = arith.domain.evaluate_all_lagrange_coefficients(point, dev)
-            dots = device.matrix_evals_dot(arith.row, arith.col, arith.row_col_val, lag)
-            for name, v in zip(("row", "col", "row_col", "row_col_val"), dots):
+        for j, m in enumerate("abc"):
+            for name, v in zip(("row", "col", "row_col", "row_col_val"), dots[3 * k + j]):
                 evals[f"{name}_{m}"] = _fr_mont_to_int(v)
-        return sum(c * evals[name] for c, name in zip(combiners, INDEX_POLYNOMIAL_NAMES)) % R_MOD
+        out.append(sum(c * evals[name] for c, name in zip(cs, INDEX_POLYNOMIAL_NAMES)) % R_MOD)
+    return out
 
 
 @dataclass
@@ -282,22 +387,38 @@ class CircuitProvingKey:
     committer_key: object
 
 
+def batch_circuit_setup(circuits: list, pp_powers_of_beta_g: torch.Tensor, pp_powers_of_beta_times_gamma_g: torch.Tensor, zk: bool = False,
+                        with_id: bool = False) -> list:
+    """VarunaSNARK::batch_circuit_setup (varuna.rs:72-134): for every circuit, trim the universal parameters to its max_degree and
+    degree bounds and commit its twelve index polynomials (no degree bound, no hiding) → [(CircuitProvingKey, CircuitVerifyingKey)] in
+    input order, each equal to circuit_setup's.  All 12·K interpolations share one batched iNTT, and all 12·K commitments one MSM pass:
+    every trimmed key is a prefix of the same powers, so their bases merge into one array.  The SRS is (β^i·G, γβ^i·G) as
+    sonic_pc.CommitterKey.trim takes it; an SRS too short for the largest circuit raises ValueError before any launch.  `with_id`
+    also fills each verifying key's circuit id (circuit_ids)."""
+    from .sonic_pc import CommitterKey
+    if not circuits:
+        raise ValueError("no circuits to set up")
+    _device_of(circuits)
+    need = max(c.info.max_degree(zk) for c in circuits) + 1
+    if pp_powers_of_beta_g.shape[0] < need:                             # download_powers_for(0..max_degree), varuna.rs:85-87
+        raise ValueError(f"the SRS holds {pp_powers_of_beta_g.shape[0]} powers; the largest circuit needs {need}")
+    cks = [CommitterKey.trim(pp_powers_of_beta_g, pp_powers_of_beta_times_gamma_g, c.info.max_degree(zk), (), 1, c.info.degree_bounds())
+           for c in circuits]
+    polys = index_polynomials(circuits)
+    comms = device.sonic_commit_batch([ck.powers_of_beta_g for ck in cks for _ in INDEX_POLYNOMIAL_NAMES],
+                                      [t for p in polys for t in p.values()])
+    ids = circuit_ids(circuits) if with_id else [None] * len(circuits)
+    out = []
+    for k, (c, ck) in enumerate(zip(circuits, cks)):
+        vk = CircuitVerifyingKey(c.info, comms[12 * k: 12 * k + 12].copy(), ids[k])
+        out.append((CircuitProvingKey(vk, c, ck), vk))
+    return out
+
+
 def circuit_setup(circuit: Circuit, pp_powers_of_beta_g: torch.Tensor, pp_powers_of_beta_times_gamma_g: torch.Tensor, zk: bool = False,
                   with_id: bool = False):
-    """VarunaSNARK::circuit_setup → batch_circuit_setup for one circuit (varuna.rs:72-134, 226-233): trim the universal parameters to
-    the circuit's max_degree and degree bounds, commit the twelve index polynomials in ONE pass (no degree bound, no hiding) and return
-    (CircuitProvingKey, CircuitVerifyingKey).  The SRS is (β^i·G, γβ^i·G) as sonic_pc.CommitterKey.trim takes it.  `with_id` also
-    fills the verifying key's circuit id (Circuit.id(): a host Blake2s pass over the matrices' byte streams)."""
-    from .sonic_pc import CommitterKey, LabeledPolynomial, SonicKZG10
-    info = circuit.info
-    max_degree = info.max_degree(zk)
-    if pp_powers_of_beta_g.shape[0] < max_degree + 1:                  # download_powers_for(0..max_degree), varuna.rs:85-87
-        raise ValueError(f"the SRS holds {pp_powers_of_beta_g.shape[0]} powers; the circuit needs {max_degree + 1}")
-    ck = CommitterKey.trim(pp_powers_of_beta_g, pp_powers_of_beta_times_gamma_g, max_degree, (), 1, info.degree_bounds())
-    polys = circuit.index_polynomials()
-    comms, _rands = SonicKZG10.commit(ck, [LabeledPolynomial(name, p) for name, p in polys.items()])
-    vk = CircuitVerifyingKey(info, comms, circuit.id() if with_id else None)
-    return CircuitProvingKey(vk, circuit, ck), vk
+    """VarunaSNARK::circuit_setup (varuna.rs:226-233): batch_circuit_setup of one circuit → (CircuitProvingKey, CircuitVerifyingKey)"""
+    return batch_circuit_setup([circuit], pp_powers_of_beta_g, pp_powers_of_beta_times_gamma_g, zk, with_id)[0]
 
 
 @dataclass
@@ -316,18 +437,40 @@ def _certificate_point(challenges) -> tuple:
     return challenges[-1], [1] + challenges[:-1]
 
 
+def prove_vk_batch(pks: list, challenges: list, opening_challenges: list) -> list:
+    """VarunaSNARK::prove_vk (varuna.rs:236-276) after the sponge, for every proving key: open Σ c_i·p_i over its twelve index
+    polynomials (c = [1] + challenges[k][:11] in label order) at z = challenges[k][11] → [Certificate] in input order.  The opening is
+    SonicKZG10.batch_open of `circuit_check` with empty randomness: it consumes opening_challenges[k] (its combination challenge ξ,
+    then the discarded randomizer) as open_combinations would, and scales the combination by ξ, which is folded into the
+    coefficients.  All interpolations share one batched iNTT, all K combinations one fr_lincomb launch, and all K witness
+    commitments one MSM pass."""
+    if not pks:
+        raise ValueError("no proving keys")
+    if len(challenges) != len(pks) or len(opening_challenges) != len(pks):
+        raise ValueError("one set of challenges and opening challenges per proving key")
+    points = [_certificate_point(ch) for ch in challenges]
+    circuits = [pk.circuit for pk in pks]
+    dev = _device_of(circuits)
+    xis = []
+    for oc in opening_challenges:
+        it = iter(oc)
+        xis.append(int(next(it)) % R_MOD)
+        next(it)                                                        # `_randomizer`
+    for pk, c in zip(pks, circuits):
+        if c.max_non_zero_domain.size > pk.committer_key.powers_of_beta_g.shape[0]:
+            raise ValueError("check_degree_is_too_large")
+    polys = index_polynomials(circuits)
+    combined = device.fr_lincomb_batch([(list(p.values()), [_mont(xi * c) for c in combiners])
+                                        for p, xi, (_z, combiners) in zip(polys, xis, points)])
+    # kzg10::open (kzg10/mod.rs:220-241): a zero ξ leaves the empty polynomial, whose witness is empty
+    witnesses = [device.poly_divide_by_linear(comb, _mont(z)) if xi else _zeros(0, dev) for comb, xi, (z, _c) in zip(combined, xis, points)]
+    ws = device.sonic_commit_batch([pk.committer_key.powers_of_beta_g for pk in pks], witnesses)
+    return [Certificate(w.copy()) for w in ws]
+
+
 def prove_vk(pk: CircuitProvingKey, challenges, opening_challenges) -> Certificate:
-    """VarunaSNARK::prove_vk (varuna.rs:236-276) after the sponge: open Σ c_i·p_i over the twelve index polynomials (c = [1] +
-    challenges[:11] in label order) at z = challenges[11].  The combination is one fr_lincomb pass; the opening is
-    SonicKZG10.batch_open of `circuit_check` with empty randomness, which consumes `opening_challenges` (its combination challenge,
-    then the discarded randomizer) as open_combinations would."""
-    from .sonic_pc import LabeledPolynomial, Randomness, SonicKZG10
-    point, combiners = _certificate_point(challenges)
-    polys = list(pk.circuit.index_polynomials().values())
-    combined = device.fr_lincomb(polys, [_mont(c) for c in combiners])
-    (w, _random_v), = SonicKZG10.batch_open(pk.committer_key, [LabeledPolynomial("circuit_check", combined)],
-                                            [("circuit_check", ("challenge", point))], [Randomness()], iter(opening_challenges))
-    return Certificate(w)
+    """VarunaSNARK::prove_vk (varuna.rs:236-276) after the sponge: prove_vk_batch of one proving key"""
+    return prove_vk_batch([pk], [challenges], [opening_challenges])[0]
 
 
 @dataclass
@@ -350,24 +493,40 @@ def _affine(projective: np.ndarray) -> np.ndarray:
     return out
 
 
+def verify_vk_batch(circuits: list, vks: list, certificates: list, challenges: list, opening_challenges: list) -> list:
+    """VarunaSNARK::verify_vk (varuna.rs:280-331) up to the pairing, for every (circuit, verifying key, certificate) → [VerifyingKeyCheck]
+    in input order.  The circuits are already indexed (Circuit).  The evaluation v comes from evaluate_index_polynomials;
+    check_combinations → batch_check → accumulate_elems for one point with randomizer one (sonic_pc/mod.rs:344-411, 477-544, 582-635)
+    reduces to lhs = ξ·C_lc − ξ·v·G + z·W with C_lc = Σ c_i·C_i, ξ = opening_challenges[k]: a 14-point sum over the twelve commitments,
+    G and W.  check_elems' pairing equation is then e(lhs, H) = e(W, β·H).  G is the universal verifier's g, the SRS's first power,
+    which is the G1 generator in the mainnet setup and in synthetic_srs.  The ids not yet cached come from one circuit_ids call, the
+    K evaluations from one evaluate_index_polynomials pass, and the K sums are K jobs of one MSM pass."""
+    K = len(circuits)
+    if K == 0:
+        raise ValueError("no circuits to verify")
+    if not (len(vks) == len(certificates) == len(challenges) == len(opening_challenges) == K):
+        raise ValueError("one verifying key, certificate, set of challenges and opening challenge per circuit")
+    points = [_certificate_point(ch) for ch in challenges]
+    xis = [int(x) % R_MOD for x in opening_challenges]
+    dev = _device_of(circuits)
+    compare = [c.info == vk.circuit_info and vk.id is not None for c, vk in zip(circuits, vks)]
+    circuit_ids([c for c, k in zip(circuits, compare) if k])
+    matches = [k and c.id() == vk.id for c, vk, k in zip(circuits, vks, compare)]
+    evaluations = evaluate_index_polynomials(circuits, [z for z, _c in points], [c for _z, c in points])
+    g = device.generator_mul(torch.from_numpy(np.array([[1, 0, 0, 0]], dtype=np.uint64).view(np.int64)).to(dev)).cpu().numpy()[0]
+    bases, scalars = [], []
+    for vk, cert, (z, combiners), xi, v in zip(vks, certificates, points, xis, evaluations):
+        bases += [_affine(c) for c in vk.circuit_commitments] + [g, _affine(cert.w)]           # C_0 … C_11, G, W
+        scalars += [_mont(xi * c) for c in combiners] + [_mont(-xi * v), _mont(z)]
+    bases_d = torch.from_numpy(np.stack(bases)).to(dev)
+    scalars_d = torch.from_numpy(np.stack(scalars).view(np.int64)).to(dev)
+    lhs = device.sonic_commit_batch([bases_d[14 * k: 14 * k + 14] for k in range(K)], [scalars_d[14 * k: 14 * k + 14] for k in range(K)])
+    return [VerifyingKeyCheck(m, v, lhs[k].copy(), cert.w) for k, (m, v, cert) in enumerate(zip(matches, evaluations, certificates))]
+
+
 def verify_vk(circuit: Circuit, vk: CircuitVerifyingKey, certificate: Certificate, challenges, opening_challenge: int) -> VerifyingKeyCheck:
-    """VarunaSNARK::verify_vk (varuna.rs:280-331) up to the pairing.  The circuit is already indexed (Circuit).  The evaluation v
-    comes from evaluate_index_polynomials; check_combinations → batch_check → accumulate_elems for one point with randomizer one
-    (sonic_pc/mod.rs:344-411, 477-544, 582-635) reduces to lhs = ξ·C_lc − ξ·v·G + z·W with C_lc = Σ c_i·C_i, ξ = opening_challenge:
-    ONE 14-point MSM over the twelve commitments, G and W.  check_elems' pairing equation is then e(lhs, H) = e(W, β·H).  G is the
-    universal verifier's g, the SRS's first power, which is the G1 generator in the mainnet setup and in synthetic_srs."""
-    point, combiners = _certificate_point(challenges)
-    xi = int(opening_challenge) % R_MOD
-    matches = circuit.info == vk.circuit_info and vk.id is not None and circuit.id() == vk.id
-    evaluation = circuit.evaluate_index_polynomials(point, combiners)
-    dev = circuit.a.row_ptr.device
-    g = device.generator_mul(torch.from_numpy(np.array([[1, 0, 0, 0]], dtype=np.uint64).view(np.int64)).to(dev))
-    comms = torch.from_numpy(np.stack([_affine(c) for c in vk.circuit_commitments])).to(dev)
-    bases = torch.cat([comms, g, torch.from_numpy(_affine(certificate.w)[None]).to(dev)])           # C_0 … C_11, G, W
-    scalars = [xi * c % R_MOD for c in combiners] + [(-xi * evaluation) % R_MOD, point]
-    sc = np.array([[(s >> (64 * i)) & (2**64 - 1) for i in range(4)] for s in scalars], dtype=np.uint64)
-    lhs = device.msm(bases, torch.from_numpy(sc.view(np.int64)).to(dev))
-    return VerifyingKeyCheck(matches, evaluation, lhs, certificate.w)
+    """VarunaSNARK::verify_vk (varuna.rs:280-331) up to the pairing: verify_vk_batch of one circuit"""
+    return verify_vk_batch([circuit], [vk], [certificate], [challenges], [opening_challenge])[0]
 
 
 class Prover:
