@@ -296,6 +296,76 @@ typedef struct {
 SNARKVM_API int snarkvm_b200_matrix_evals_at_points_device(void* out_mont_host, const snarkvm_b200_evals_segment_t* segs, size_t count,
                                                            void* stream);
 
+/* The batched Varuna prover (VarunaSNARK::prove_batch, varuna.rs:336-620, over many circuits and instances).  Segment tables are
+ * HOST arrays, as above.  Argument errors return cudaErrorInvalidValue before any launch. */
+
+/* One term of an uncapped linear combination: a view of len Fr at d_poly, added times coeff_mont at output positions offset +
+ * k * period + u (u < len) for k < reps.  reps = 1 is one plain term (period is then ignored); reps > 1 needs period >= len.  The
+ * last copy must end inside its output. */
+typedef struct {
+    const void* d_poly;
+    uint64_t len, offset, period, reps;
+    uint8_t coeff_mont[32];
+} snarkvm_b200_lincomb_term_t;
+/* One output: d_out (n Fr) = the sum of terms [first_term, first_term + nterms) of the term table; positions no term covers are 0. */
+typedef struct {
+    void* d_out;
+    uint64_t n, first_term, nterms;
+} snarkvm_b200_lincomb_output_t;
+/* every output in one launch, bit-identical to the sequence of scaled, shifted additions it stands for; no cap on the number of
+ * terms.  snarkvm_b200_fr_lincomb_batch_device and snarkvm_b200_fr_lincomb_device are calls of this kernel. */
+SNARKVM_API int snarkvm_b200_fr_lincomb_terms_device(const snarkvm_b200_lincomb_output_t* outs, size_t nouts,
+                                                     const snarkvm_b200_lincomb_term_t* terms, size_t nterms, void* stream);
+
+/* One CSR sparse mat-vec of a segmented call: d_out (nrows Fr) = M * d_x (nvars Fr), with nnz = row_ptr[nrows]. */
+typedef struct {
+    const void* d_row_ptr;
+    const void* d_cols;
+    const void* d_vals;
+    uint64_t nrows, nnz;
+    const void* d_x;
+    uint64_t nvars;
+    void* d_out;
+} snarkvm_b200_spmv_segment_t;
+/* every segment's product in one pass of three launches (rows over 256 entries of any segment share one work list) and one
+ * synchronisation.  A column >= nvars, or a row_ptr that is not non-decreasing up to nnz, returns cudaErrorInvalidValue after the
+ * pass with *bad_segment (HOST, may be NULL) = the first such segment (-1 otherwise).  snarkvm_b200_sparse_matvec_device is a
+ * one-segment call. */
+SNARKVM_API int snarkvm_b200_sparse_matvec_batch_device(const snarkvm_b200_spmv_segment_t* segs, size_t count, int64_t* bad_segment,
+                                                        void* stream);
+
+/* One product of a batched PolyMultiplier: d_out (2^lg Fr) = d_a (len_a Fr) * d_b (len_b Fr) with len_a + len_b - 1 <= 2^lg. */
+typedef struct {
+    void* d_out;
+    const void* d_a;
+    const void* d_b;
+    uint64_t len_a, len_b;
+    uint32_t lg, reserved;
+} snarkvm_b200_polymul_job_t;
+/* every product in one pass: one load launch, the forward transforms of both operands through snarkvm_b200_ntt_batch_device
+ * (equal sizes share launches), one pointwise launch, the inverse transforms the same way.  Each result equals
+ * snarkvm_b200_polymul_device of the two operands at the same lg. */
+SNARKVM_API int snarkvm_b200_polymul_batch_device(const snarkvm_b200_polymul_job_t* jobs, size_t count, void* stream);
+
+/* One matrix of Varuna's fourth round (fourth.rs:151-245): its row, col, row_col_val on K (n = |K| Fr) and its circuit's constants,
+ * all 32 B Montgomery: v_rc = v_R(alpha) * v_C(beta), rc = |R| * |C|, f_scale = v_rc / (|R| * |C|).  Writes, on K:
+ * d_a = v_rc * row_col_val, d_b = rc * (row - alpha)(col - beta) and d_f = f_scale * row_col_val / ((row - alpha)(col - beta))
+ * (0 where the denominator is 0, as batch_inversion_and_mul leaves it). */
+typedef struct {
+    const void* d_row;
+    const void* d_col;
+    const void* d_row_col_val;
+    uint64_t n;
+    uint8_t v_rc_mont[32], rc_mont[32], f_scale_mont[32];
+    void* d_a;
+    void* d_b;
+    void* d_f;
+} snarkvm_b200_round4_segment_t;
+/* every segment in one launch, one batch inversion over the concatenation of all denominators and one launch for f; alpha / beta:
+ * 32 B Montgomery HOST.  No synchronisation. */
+SNARKVM_API int snarkvm_b200_varuna_round4_evals_device(const snarkvm_b200_round4_segment_t* segs, size_t count, const void* alpha_mont,
+                                                        const void* beta_mont, void* stream);
+
 /* Fr Montgomery <-> canonical, n elements in HBM (to_bigint / from_bigint, fields/src/fp_256.rs:362-413). */
 SNARKVM_API int snarkvm_b200_fr_from_mont_device(void* d_out, const void* d_in, size_t n, void* stream);
 SNARKVM_API int snarkvm_b200_fr_to_mont_device(void* d_out, const void* d_in, size_t n, void* stream);

@@ -36,6 +36,8 @@ SYMBOLS = (
     "snarkvm_b200_csr_serialize_device", "snarkvm_b200_fr_lincomb_device", "snarkvm_b200_matrix_evals_dot_device",
     "snarkvm_b200_ntt_batch_device", "snarkvm_b200_varuna_matrix_evals_batch_device", "snarkvm_b200_csr_serialize_batch_device",
     "snarkvm_b200_fr_lincomb_batch_device", "snarkvm_b200_matrix_evals_at_points_device",
+    "snarkvm_b200_fr_lincomb_terms_device", "snarkvm_b200_sparse_matvec_batch_device", "snarkvm_b200_polymul_batch_device",
+    "snarkvm_b200_varuna_round4_evals_device",
 )
 
 
@@ -57,6 +59,36 @@ class EvalsSegment(ctypes.Structure):
     """snarkvm_b200_evals_segment_t"""
     _fields_ = [("d_row", ctypes.c_void_p), ("d_col", ctypes.c_void_p), ("d_row_col_val", ctypes.c_void_p), ("n", ctypes.c_uint64),
                 ("point_mont", ctypes.c_uint8 * 32)]
+
+
+class LincombTerm(ctypes.Structure):
+    """snarkvm_b200_lincomb_term_t"""
+    _fields_ = [("d_poly", ctypes.c_void_p), ("len", ctypes.c_uint64), ("offset", ctypes.c_uint64), ("period", ctypes.c_uint64),
+                ("reps", ctypes.c_uint64), ("coeff_mont", ctypes.c_uint8 * 32)]
+
+
+class LincombOutput(ctypes.Structure):
+    """snarkvm_b200_lincomb_output_t"""
+    _fields_ = [("d_out", ctypes.c_void_p), ("n", ctypes.c_uint64), ("first_term", ctypes.c_uint64), ("nterms", ctypes.c_uint64)]
+
+
+class SpmvSegment(ctypes.Structure):
+    """snarkvm_b200_spmv_segment_t"""
+    _fields_ = [("d_row_ptr", ctypes.c_void_p), ("d_cols", ctypes.c_void_p), ("d_vals", ctypes.c_void_p), ("nrows", ctypes.c_uint64),
+                ("nnz", ctypes.c_uint64), ("d_x", ctypes.c_void_p), ("nvars", ctypes.c_uint64), ("d_out", ctypes.c_void_p)]
+
+
+class PolymulJob(ctypes.Structure):
+    """snarkvm_b200_polymul_job_t"""
+    _fields_ = [("d_out", ctypes.c_void_p), ("d_a", ctypes.c_void_p), ("d_b", ctypes.c_void_p), ("len_a", ctypes.c_uint64),
+                ("len_b", ctypes.c_uint64), ("lg", ctypes.c_uint32), ("reserved", ctypes.c_uint32)]
+
+
+class Round4Segment(ctypes.Structure):
+    """snarkvm_b200_round4_segment_t"""
+    _fields_ = [("d_row", ctypes.c_void_p), ("d_col", ctypes.c_void_p), ("d_row_col_val", ctypes.c_void_p), ("n", ctypes.c_uint64),
+                ("v_rc_mont", ctypes.c_uint8 * 32), ("rc_mont", ctypes.c_uint8 * 32), ("f_scale_mont", ctypes.c_uint8 * 32),
+                ("d_a", ctypes.c_void_p), ("d_b", ctypes.c_void_p), ("d_f", ctypes.c_void_p)]
 
 
 class CudaError(RuntimeError):
@@ -144,6 +176,10 @@ def lib():
     L.snarkvm_b200_csr_serialize_batch_device.argtypes = [ctypes.POINTER(CsrSegment), sz, ctypes.POINTER(ctypes.c_int64), vp]
     L.snarkvm_b200_fr_lincomb_batch_device.argtypes = [ctypes.POINTER(LincombSegment), sz, vp]
     L.snarkvm_b200_matrix_evals_at_points_device.argtypes = [vp, ctypes.POINTER(EvalsSegment), sz, vp]
+    L.snarkvm_b200_fr_lincomb_terms_device.argtypes = [ctypes.POINTER(LincombOutput), sz, ctypes.POINTER(LincombTerm), sz, vp]
+    L.snarkvm_b200_sparse_matvec_batch_device.argtypes = [ctypes.POINTER(SpmvSegment), sz, ctypes.POINTER(ctypes.c_int64), vp]
+    L.snarkvm_b200_polymul_batch_device.argtypes = [ctypes.POINTER(PolymulJob), sz, vp]
+    L.snarkvm_b200_varuna_round4_evals_device.argtypes = [ctypes.POINTER(Round4Segment), sz, vp, vp, vp]
     L.snarkvm_b200_msm_batch_device.argtypes = [vp, vp, sz, vp, vp, sz, vp]
     L.snarkvm_b200_msm_window_sums_plan_device.argtypes = [vp, vp, sz, vp, sz, vp, sz, vp]
     L.snarkvm_b200_kzg_commit_batch_hiding_device.argtypes = [vp, vp, sz, vp, vp, vp, vp, vp, sz, vp]

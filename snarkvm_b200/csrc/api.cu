@@ -1194,6 +1194,20 @@ int snarkvm_b200_fr_lincomb_batch_device(const snarkvm_b200_lincomb_segment_t* s
 int snarkvm_b200_matrix_evals_at_points_device(void* out_mont_host, const snarkvm_b200_evals_segment_t* segs, size_t count, void* stream) {
     return matrix_evals_at_points_device(out_mont_host, segs, count, (cudaStream_t)stream);
 }
+int snarkvm_b200_fr_lincomb_terms_device(const snarkvm_b200_lincomb_output_t* outs, size_t nouts, const snarkvm_b200_lincomb_term_t* terms,
+                                         size_t nterms, void* stream) {
+    return fr_lincomb_terms_device(outs, nouts, terms, nterms, (cudaStream_t)stream);
+}
+int snarkvm_b200_sparse_matvec_batch_device(const snarkvm_b200_spmv_segment_t* segs, size_t count, int64_t* bad_segment, void* stream) {
+    return sparse_matvec_batch_device(segs, count, bad_segment, (cudaStream_t)stream);
+}
+int snarkvm_b200_polymul_batch_device(const snarkvm_b200_polymul_job_t* jobs, size_t count, void* stream) {
+    return polymul_batch_device(jobs, count, (cudaStream_t)stream);
+}
+int snarkvm_b200_varuna_round4_evals_device(const snarkvm_b200_round4_segment_t* segs, size_t count, const void* alpha_mont,
+                                            const void* beta_mont, void* stream) {
+    return varuna_round4_evals_device(segs, count, alpha_mont, beta_mont, (cudaStream_t)stream);
+}
 
 int snarkvm_b200_fr_from_mont_device(void* d_out, const void* d_in, size_t n, void* stream) {
     return fr_from_mont_device(d_out, d_in, n, (cudaStream_t)stream);

@@ -299,28 +299,49 @@ int poly_divide_by_linear_device(void* d_q, const void* d_p, size_t m, const voi
 // 2^20-constraint circuit.  They leave the thread-per-row kernel through a device-side work list — no host round trip —
 // and are cut into segments of SPMV_SEG entries, one CTA per segment, then one CTA per long row adds its segments.
 static constexpr uint32_t SPMV_LONG = 256, SPMV_SEG = 2048;
-struct SpmvLong { uint32_t row, base, nseg; };
-__global__ void k_sparse_matvec(const uint32_t* __restrict__ row_ptr, const uint32_t* __restrict__ cols, const uint32_t* __restrict__ vals,
-                                size_t nrows, const uint32_t* __restrict__ x, size_t nvars, uint32_t* __restrict__ out, int* __restrict__ bad,
+// Segmented launches: thread g of the grid belongs to the last segment whose `first` is ≤ g (segments hold consecutive ranges of
+// the grid; empty ones are skipped by the search).
+template <class Seg> FF_DEV uint32_t seg_of(const Seg* __restrict__ segs, uint32_t nsegs, uint64_t g) {
+    uint32_t lo = 0, hi = nsegs;
+    while (hi - lo > 1) {
+        const uint32_t mid = lo + (hi - lo) / 2;
+        if (segs[mid].first <= g) lo = mid; else hi = mid;
+    }
+    return lo;
+}
+// Many mat-vecs in one pass (every instance of every circuit, or the three transposes of every circuit): thread g takes row
+// g − first of its segment; the long rows of all segments share one work list, each entry naming its segment.
+struct SpmvSeg {
+    const uint32_t *row_ptr, *cols, *vals, *x;
+    uint32_t* out;
+    uint64_t first, nrows, nnz, nvars;
+};
+struct SpmvLong { uint32_t seg, row, base, nseg; };
+struct SpmvItem { uint32_t seg, row, j; };
+__global__ void k_sparse_matvec(const SpmvSeg* __restrict__ segs, uint32_t nsegs, uint64_t total, int* __restrict__ bad_flags,
                                 uint32_t* __restrict__ ctr /* [0] long rows, [1] work items */, SpmvLong* __restrict__ long_rows,
-                                uint2* __restrict__ items) {
-    const size_t r = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (r >= nrows) return;
-    const uint32_t e0 = row_ptr[r], e1 = row_ptr[r + 1];
+                                SpmvItem* __restrict__ items) {
+    const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= total) return;
+    const uint32_t s = seg_of(segs, nsegs, g);
+    const SpmvSeg& m = segs[s];
+    const size_t r = g - m.first;
+    const uint32_t e0 = m.row_ptr[r], e1 = m.row_ptr[r + 1];
+    if (e1 < e0 || e1 > m.nnz || (r + 1 == m.nrows && e1 != m.nnz)) { bad_flags[s] = 1; return; }   // the work lists are sized by nnz
     if (e1 - e0 > SPMV_LONG) {
         const uint32_t nseg = (e1 - e0 + SPMV_SEG - 1) / SPMV_SEG;
         const uint32_t base = atomicAdd(&ctr[1], nseg), slot = atomicAdd(&ctr[0], 1u);
-        long_rows[slot] = SpmvLong{(uint32_t)r, base, nseg};
-        for (uint32_t j = 0; j < nseg; j++) items[base + j] = make_uint2((uint32_t)r, j);
+        long_rows[slot] = SpmvLong{s, (uint32_t)r, base, nseg};
+        for (uint32_t j = 0; j < nseg; j++) items[base + j] = SpmvItem{s, (uint32_t)r, j};
         return;
     }
     Fr acc = Fr::zero();
     for (uint32_t e = e0; e < e1; e++) {
-        const uint32_t c = cols[e];
-        if (c >= nvars) { *bad = 1; continue; }              // out-of-range column: reported, never read
-        acc = acc + Fr::load_ldg(x + (size_t)c * 8) * Fr::load_ldg(vals + (size_t)e * 8);
+        const uint32_t c = m.cols[e];
+        if (c >= m.nvars) { bad_flags[s] = 1; continue; }   // out-of-range column: reported, never read
+        acc = acc + Fr::load_ldg(m.x + (size_t)c * 8) * Fr::load_ldg(m.vals + (size_t)e * 8);
     }
-    acc.store(out + r * 8);
+    acc.store(m.out + r * 8);
 }
 // Σ over the 256 threads of a CTA (shared memory tree); the result is valid in thread 0
 FF_DEV Fr cta_sum_fr(Fr v, uint4* sh) {
@@ -337,28 +358,31 @@ FF_DEV Fr cta_sum_fr(Fr v, uint4* sh) {
     }
     return Fr::load(sh);
 }
-__global__ void __launch_bounds__(256) k_spmv_segments(const uint32_t* __restrict__ row_ptr, const uint32_t* __restrict__ cols,
-                                                       const uint32_t* __restrict__ vals, const uint32_t* __restrict__ x, size_t nvars,
-                                                       const uint32_t* __restrict__ ctr, const uint2* __restrict__ items,
-                                                       uint32_t* __restrict__ partial, int* __restrict__ bad) {
+__global__ void __launch_bounds__(256) k_spmv_segments(const SpmvSeg* __restrict__ segs, const uint32_t* __restrict__ ctr,
+                                                       const SpmvItem* __restrict__ items, uint32_t* __restrict__ partial,
+                                                       int* __restrict__ bad_flags) {
     __shared__ uint4 sh[512];
     const uint32_t nitems = ctr[1];
     for (uint32_t it = blockIdx.x; it < nitems; it += gridDim.x) {
-        const uint2 w = items[it];
-        const uint32_t e0 = row_ptr[w.x] + w.y * SPMV_SEG, rend = row_ptr[w.x + 1], e1 = e0 + SPMV_SEG < rend ? e0 + SPMV_SEG : rend;
+        const SpmvItem w = items[it];
+        const uint32_t *cols = segs[w.seg].cols, *vals = segs[w.seg].vals, *x = segs[w.seg].x, *row_ptr = segs[w.seg].row_ptr;
+        const uint32_t nvars = (uint32_t)segs[w.seg].nvars;
+        const uint32_t e0 = row_ptr[w.row] + w.j * SPMV_SEG, rend = row_ptr[w.row + 1], e1 = e0 + SPMV_SEG < rend ? e0 + SPMV_SEG : rend;
+        bool bad = false;
         Fr acc = Fr::zero();
         for (uint32_t e = e0 + threadIdx.x; e < e1; e += 256) {
             const uint32_t c = cols[e];
-            if (c >= nvars) { *bad = 1; continue; }
+            if (c >= nvars) { bad = true; continue; }
             acc = acc + Fr::load_ldg(x + (size_t)c * 8) * Fr::load_ldg(vals + (size_t)e * 8);
         }
+        if (bad) bad_flags[w.seg] = 1;
         const Fr tot = cta_sum_fr(acc, sh);
         if (threadIdx.x == 0) tot.store(partial + (size_t)it * 8);
         __syncthreads();
     }
 }
-__global__ void __launch_bounds__(256) k_spmv_long_rows(const uint32_t* __restrict__ ctr, const SpmvLong* __restrict__ long_rows,
-                                                        const uint32_t* __restrict__ partial, uint32_t* __restrict__ out) {
+__global__ void __launch_bounds__(256) k_spmv_long_rows(const SpmvSeg* __restrict__ segs, const uint32_t* __restrict__ ctr,
+                                                        const SpmvLong* __restrict__ long_rows, const uint32_t* __restrict__ partial) {
     __shared__ uint4 sh[512];
     const uint32_t nlong = ctr[0];
     for (uint32_t k = blockIdx.x; k < nlong; k += gridDim.x) {
@@ -366,48 +390,78 @@ __global__ void __launch_bounds__(256) k_spmv_long_rows(const uint32_t* __restri
         Fr acc = Fr::zero();
         for (uint32_t j = threadIdx.x; j < L.nseg; j += 256) acc = acc + Fr::load(partial + (size_t)(L.base + j) * 8);
         const Fr tot = cta_sum_fr(acc, sh);
-        if (threadIdx.x == 0) tot.store(out + (size_t)L.row * 8);
+        if (threadIdx.x == 0) tot.store(segs[L.seg].out + (size_t)L.row * 8);
         __syncthreads();
     }
+}
+
+static int seg_finish(int rc, uint8_t* scratch, const int* bad, size_t count, int64_t* bad_segment, cudaStream_t stream);
+
+int sparse_matvec_batch_device(const snarkvm_b200_spmv_segment_t* segs, size_t count, int64_t* bad_segment, cudaStream_t stream) {
+    if (bad_segment) *bad_segment = -1;
+    if (count == 0) return 0;
+    if (!segs || count >= ((size_t)1 << 31)) return (int)cudaErrorInvalidValue;
+    std::vector<SpmvSeg> table;
+    std::vector<size_t> index;                                    // table entry → segment (segments without rows are left out)
+    uint64_t total = 0;
+    size_t max_long = 0, max_items = 0;
+    for (size_t i = 0; i < count; i++) {
+        const snarkvm_b200_spmv_segment_t& s = segs[i];
+        if (s.nrows == 0) continue;
+        if (!s.d_out || !s.d_row_ptr || !s.d_x || (s.nnz && (!s.d_cols || !s.d_vals))) return (int)cudaErrorInvalidValue;
+        if (s.nrows >= ((uint64_t)1 << 32) || s.nnz >= ((uint64_t)1 << 32) || s.nvars >= ((uint64_t)1 << 32)) return (int)cudaErrorInvalidValue;
+        table.push_back(SpmvSeg{(const uint32_t*)s.d_row_ptr, (const uint32_t*)s.d_cols, (const uint32_t*)s.d_vals, (const uint32_t*)s.d_x,
+                                (uint32_t*)s.d_out, total, s.nrows, s.nnz, s.nvars});
+        index.push_back(i);
+        total += s.nrows;
+        const size_t ml = (size_t)s.nnz / SPMV_LONG + 1;
+        max_long += ml;
+        max_items += (size_t)s.nnz / SPMV_SEG + ml + 1;
+    }
+    if (table.empty()) return 0;
+    // the segment and long-row kernels walk their work lists grid-stride: four CTAs per SM and one CTA per SM
+    int dev = 0, sms = 0;
+    int rc = (int)cudaGetDevice(&dev);
+    if (rc == 0) rc = (int)cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    if (rc != 0) return rc;
+    const size_t n = table.size(), nflags = (n * sizeof(int) + 255) & ~(size_t)255;
+    // scratch: bad flags | counters | segment table | long rows | work items | partial sums
+    const size_t off_ctr = nflags, off_table = off_ctr + 256, off_long = off_table + ((n * sizeof(SpmvSeg) + 255) & ~(size_t)255),
+                 off_items = off_long + ((max_long * sizeof(SpmvLong) + 255) & ~(size_t)255),
+                 off_partial = off_items + ((max_items * sizeof(SpmvItem) + 255) & ~(size_t)255), bytes = off_partial + max_items * 32;
+    uint8_t* scratch = nullptr;
+    cudaError_t e = pool_alloc(&scratch, bytes, stream);
+    if (e != cudaSuccess) return (int)e;
+    int* bad = (int*)scratch;
+    uint32_t* ctr = (uint32_t*)(scratch + off_ctr);
+    SpmvSeg* d_table = (SpmvSeg*)(scratch + off_table);
+    rc = (int)cudaMemsetAsync(scratch, 0, off_table, stream);     // bad flags and counters
+    if (rc == 0) rc = (int)cudaMemcpyAsync(d_table, table.data(), n * sizeof(SpmvSeg), cudaMemcpyHostToDevice, stream);
+    if (rc == 0) {
+        k_sparse_matvec<<<(unsigned)((total + 127) / 128), 128, 0, stream>>>(d_table, (uint32_t)n, total, bad, ctr, (SpmvLong*)(scratch + off_long),
+                                                                           (SpmvItem*)(scratch + off_items));
+        k_spmv_segments<<<4 * sms, 256, 0, stream>>>(d_table, ctr, (const SpmvItem*)(scratch + off_items), (uint32_t*)(scratch + off_partial), bad);
+        k_spmv_long_rows<<<sms, 256, 0, stream>>>(d_table, ctr, (const SpmvLong*)(scratch + off_long), (const uint32_t*)(scratch + off_partial));
+        count_launch(3);
+        rc = (int)cudaGetLastError();
+    }
+    int64_t bad_entry = -1;
+    rc = seg_finish(rc, scratch, bad, n, &bad_entry, stream);
+    if (bad_segment && bad_entry >= 0) *bad_segment = (int64_t)index[(size_t)bad_entry];
+    return rc;
 }
 
 int sparse_matvec_device(void* d_out, const void* d_row_ptr, const void* d_cols, const void* d_vals, size_t nrows, const void* d_x,
                          size_t nvars, cudaStream_t stream) {
     if (nrows == 0) return 0;
     if (!d_out || !d_row_ptr || !d_x) return (int)cudaErrorInvalidValue;
-    // the segment and long-row kernels walk their work lists grid-stride: four CTAs per SM and one CTA per SM
-    int dev = 0, sms = 0;
-    int rc = (int)cudaGetDevice(&dev);
-    if (rc == 0) rc = (int)cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (rc != 0) return rc;
     // the number of entries sizes the work lists of the long rows
     uint32_t nnz = 0;
-    rc = (int)cudaMemcpyAsync(&nnz, (const uint32_t*)d_row_ptr + nrows, 4, cudaMemcpyDeviceToHost, stream);
+    int rc = (int)cudaMemcpyAsync(&nnz, (const uint32_t*)d_row_ptr + nrows, 4, cudaMemcpyDeviceToHost, stream);
     if (rc == 0) rc = (int)cudaStreamSynchronize(stream);
     if (rc != 0) return rc;
-    const size_t max_long = (size_t)nnz / SPMV_LONG + 1, max_items = (size_t)nnz / SPMV_SEG + max_long + 1;
-    uint8_t* scratch = nullptr;
-    const size_t off_long = 256, off_items = off_long + ((max_long * sizeof(SpmvLong) + 255) & ~(size_t)255),
-                 off_partial = off_items + ((max_items * sizeof(uint2) + 255) & ~(size_t)255), total = off_partial + max_items * 32;
-    cudaError_t e = pool_alloc(&scratch, total, stream);
-    if (e != cudaSuccess) return (int)e;
-    int* bad = (int*)scratch;                                     // [0] bad flag, [1..2] counters
-    uint32_t* ctr = (uint32_t*)scratch + 1;
-    rc = (int)cudaMemsetAsync(scratch, 0, 256, stream);
-    k_sparse_matvec<<<(unsigned)((nrows + 127) / 128), 128, 0, stream>>>((const uint32_t*)d_row_ptr, (const uint32_t*)d_cols, (const uint32_t*)d_vals,
-                                                                         nrows, (const uint32_t*)d_x, nvars, (uint32_t*)d_out, bad, ctr,
-                                                                         (SpmvLong*)(scratch + off_long), (uint2*)(scratch + off_items));
-    k_spmv_segments<<<4 * sms, 256, 0, stream>>>((const uint32_t*)d_row_ptr, (const uint32_t*)d_cols, (const uint32_t*)d_vals, (const uint32_t*)d_x, nvars,
-                                                 ctr, (const uint2*)(scratch + off_items), (uint32_t*)(scratch + off_partial), bad);
-    k_spmv_long_rows<<<sms, 256, 0, stream>>>(ctr, (const SpmvLong*)(scratch + off_long), (const uint32_t*)(scratch + off_partial), (uint32_t*)d_out);
-    count_launch(3);
-    if (rc == 0) rc = (int)cudaGetLastError();
-    int h_bad = 0;
-    if (rc == 0) rc = (int)cudaMemcpyAsync(&h_bad, bad, sizeof(int), cudaMemcpyDeviceToHost, stream);
-    cudaFreeAsync(scratch, stream);
-    if (rc == 0) rc = (int)cudaStreamSynchronize(stream);
-    if (rc == 0 && h_bad) rc = (int)cudaErrorInvalidValue;
-    return rc;
+    const snarkvm_b200_spmv_segment_t s{d_row_ptr, d_cols, d_vals, nrows, nnz, d_x, nvars, d_out};
+    return sparse_matvec_batch_device(&s, 1, nullptr, stream);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -493,17 +547,6 @@ FF_DEV uint32_t reindex_by_subdomain(uint32_t index, uint32_t input_size, uint32
 }
 FF_DEV void csr_check_bounds(const CsrArgs& m, int* bad) {
     if (blockIdx.x == 0 && threadIdx.x == 0 && (m.row_ptr[0] != 0 || m.row_ptr[m.nrows] != m.nnz)) *bad = 1;
-}
-
-// Segmented launches: thread g of the grid belongs to the last segment whose `first` is ≤ g (segments hold consecutive ranges of
-// the grid; empty ones are skipped by the search).
-template <class Seg> FF_DEV uint32_t seg_of(const Seg* __restrict__ segs, uint32_t nsegs, uint64_t g) {
-    uint32_t lo = 0, hi = nsegs;
-    while (hi - lo > 1) {
-        const uint32_t mid = lo + (hi - lo) / 2;
-        if (segs[mid].first <= g) lo = mid; else hi = mid;
-    }
-    return lo;
 }
 
 struct EvalsSeg {
@@ -818,74 +861,110 @@ int csr_serialize_device(void* d_out, size_t out_bytes, const void* d_row_ptr, s
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// out = Σ_j c_j·p_j over up to LINCOMB_MAX polynomials of different lengths in one pass: each output coefficient is read-modified
-// once instead of once per term (the poly_axpy loop).  A term whose coefficient is one adds p_j without the product; zero
-// coefficients and empty terms are dropped on the host.  Field sums are exact, so the result is the axpy sequence's bit for bit.
-// ---------------------------------------------------------------------------------------------------------------------
-// Segmented: every output of a batch (one per circuit) in one launch; thread g writes coefficient g − first of its segment.
-static constexpr int LINCOMB_MAX = 12;
-struct LincombSeg {
-    uint32_t* out;
-    uint64_t n, first;
-    const uint32_t* p[LINCOMB_MAX];
-    uint64_t len[LINCOMB_MAX];
-    FrArg c[LINCOMB_MAX];
-    uint32_t nterms;
+// out = Σ_j c_j·p_j over polynomials of different lengths in one pass: each output coefficient is read-modified once instead of
+// once per term (the poly_axpy loop).  A term is a view (pointer, length) placed at an offset of its output, optionally repeated
+// `reps` times `period` apart: the selector sums of the batched Varuna prover (a quotient by v_n of a degree < 2n product is its
+// upper half; a remainder times v_t / v_s is t/s copies of it, s apart) are such terms.  A term whose coefficient is one adds
+// p_j without the product; zero coefficients and empty terms are dropped on the host.  Field sums are exact, so the result is the
+// sequence of additions' bit for bit.
+// Segmented: every output of a call in one launch; thread g writes coefficient g − first of its output, looping over that output's
+// terms in the term table.
+struct LincombTerm {
+    const uint32_t* p;
+    uint64_t len, offset, period, reps;
+    FrArg c;
 };
-__global__ void k_fr_lincomb(const LincombSeg* __restrict__ segs, uint32_t nsegs, uint64_t total) {
+struct LincombOut {
+    uint32_t* out;
+    uint64_t n, first, t0, nterms;
+};
+__global__ void k_fr_lincomb(const LincombOut* __restrict__ outs, uint32_t nouts, uint64_t total, const LincombTerm* __restrict__ terms) {
     const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (g >= total) return;
-    const LincombSeg& a = segs[seg_of(segs, nsegs, g)];
-    const size_t i = g - a.first;
+    const LincombOut& a = outs[seg_of(outs, nouts, g)];
+    const uint64_t i = g - a.first;
     Fr acc = Fr::zero();
-    for (uint32_t j = 0; j < a.nterms; j++) {
-        if (i >= a.len[j]) continue;
-        const Fr x = Fr::load_ldg(a.p[j] + i * 8), c = fr_from_arg(a.c[j]);
+    for (uint64_t j = a.t0; j < a.t0 + a.nterms; j++) {
+        const LincombTerm& t = terms[j];
+        if (i < t.offset) continue;
+        uint64_t u = i - t.offset;
+        if (t.reps > 1) {
+            if (u >= t.period * t.reps) continue;
+            u %= t.period;
+        }
+        if (u >= t.len) continue;
+        const Fr x = Fr::load_ldg(t.p + u * 8), c = fr_from_arg(t.c);
         acc = acc + (c == Fr::one() ? x : c * x);
     }
     acc.store(a.out + i * 8);
 }
 
-int fr_lincomb_batch_device(const snarkvm_b200_lincomb_segment_t* segs, size_t count, cudaStream_t stream) {
-    if (count == 0) return 0;
-    if (!segs || count >= ((size_t)1 << 31)) return (int)cudaErrorInvalidValue;
-    std::vector<LincombSeg> table;
+int fr_lincomb_terms_device(const snarkvm_b200_lincomb_output_t* outs, size_t nouts, const snarkvm_b200_lincomb_term_t* terms, size_t nterms,
+                            cudaStream_t stream) {
+    if (nouts == 0) return 0;
+    if (!outs || (nterms && !terms) || nouts >= ((size_t)1 << 31)) return (int)cudaErrorInvalidValue;
+    std::vector<LincombOut> table;
+    std::vector<LincombTerm> kept;
     uint64_t total = 0;
-    for (size_t i = 0; i < count; i++) {
-        const snarkvm_b200_lincomb_segment_t& s = segs[i];
-        if (s.nterms > LINCOMB_MAX || (s.n && !s.d_out)) return (int)cudaErrorInvalidValue;
-        LincombSeg a{};
-        a.out = (uint32_t*)s.d_out;
-        a.n = s.n;
-        a.first = total;
-        for (uint32_t j = 0; j < s.nterms; j++) {
-            if (s.lens[j] > s.n || (s.lens[j] && !s.d_polys[j])) return (int)cudaErrorInvalidValue;
-            FrArg c;
-            memcpy(c.v, s.coeffs_mont[j], 32);
+    for (size_t i = 0; i < nouts; i++) {
+        const snarkvm_b200_lincomb_output_t& o = outs[i];
+        if ((o.n && !o.d_out) || o.first_term > nterms || o.nterms > nterms - o.first_term) return (int)cudaErrorInvalidValue;
+        LincombOut a{(uint32_t*)o.d_out, o.n, total, kept.size(), 0};
+        for (uint64_t j = o.first_term; j < o.first_term + o.nterms; j++) {
+            const snarkvm_b200_lincomb_term_t& s = terms[j];
+            if (s.len && !s.d_poly) return (int)cudaErrorInvalidValue;
+            if (s.reps > 1 && s.period < s.len) return (int)cudaErrorInvalidValue;
+            const uint64_t reps = s.reps ? s.reps : 1, step = reps > 1 ? s.period : 0;
+            if (s.len && (s.offset > o.n || s.len > o.n || (reps - 1) > (o.n / (step ? step : 1)) ||
+                          s.offset + (reps - 1) * step + s.len > o.n)) return (int)cudaErrorInvalidValue;   // every copy ends inside the output
+            LincombTerm t{(const uint32_t*)s.d_poly, s.len, s.offset, reps > 1 ? s.period : s.len, reps, FrArg{}};
+            memcpy(t.c.v, s.coeff_mont, 32);
             bool zero = true;
-            for (int k = 0; k < 8; k++) zero &= c.v[k] == 0;
-            if (s.lens[j] == 0 || zero) continue;                                  // zero coefficients and empty terms are dropped
-            a.p[a.nterms] = (const uint32_t*)s.d_polys[j];
-            a.len[a.nterms] = s.lens[j];
-            a.c[a.nterms] = c;
+            for (int k = 0; k < 8; k++) zero &= t.c.v[k] == 0;
+            if (s.len == 0 || s.reps == 0 || zero) continue;                         // zero coefficients and empty terms are dropped
+            kept.push_back(t);
             a.nterms++;
         }
-        if (s.n == 0) continue;
+        if (o.n == 0) { kept.resize(a.t0); continue; }
         table.push_back(a);
-        total += s.n;
+        total += o.n;
     }
     if (total == 0) return 0;
-    LincombSeg* d_table = nullptr;
-    cudaError_t e = pool_alloc(&d_table, table.size() * sizeof(LincombSeg), stream);
+    const size_t off_terms = (table.size() * sizeof(LincombOut) + 255) & ~(size_t)255, bytes = off_terms + kept.size() * sizeof(LincombTerm);
+    uint8_t* scratch = nullptr;
+    cudaError_t e = pool_alloc(&scratch, bytes, stream);
     if (e != cudaSuccess) return (int)e;
-    int rc = (int)cudaMemcpyAsync(d_table, table.data(), table.size() * sizeof(LincombSeg), cudaMemcpyHostToDevice, stream);
+    int rc = (int)cudaMemcpyAsync(scratch, table.data(), table.size() * sizeof(LincombOut), cudaMemcpyHostToDevice, stream);
+    if (rc == 0 && !kept.empty())
+        rc = (int)cudaMemcpyAsync(scratch + off_terms, kept.data(), kept.size() * sizeof(LincombTerm), cudaMemcpyHostToDevice, stream);
     if (rc == 0) {
-        k_fr_lincomb<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(d_table, (uint32_t)table.size(), total);
+        k_fr_lincomb<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>((const LincombOut*)scratch, (uint32_t)table.size(), total,
+                                                                          (const LincombTerm*)(scratch + off_terms));
         count_launch();
         rc = (int)cudaGetLastError();
     }
-    cudaFreeAsync(d_table, stream);
+    cudaFreeAsync(scratch, stream);
     return rc;
+}
+
+// The capped segment form (at most 12 terms per output, all at offset 0) as a call of the same kernel.
+static constexpr int LINCOMB_MAX = 12;
+int fr_lincomb_batch_device(const snarkvm_b200_lincomb_segment_t* segs, size_t count, cudaStream_t stream) {
+    if (count == 0) return 0;
+    if (!segs || count >= ((size_t)1 << 31)) return (int)cudaErrorInvalidValue;
+    std::vector<snarkvm_b200_lincomb_output_t> outs(count);
+    std::vector<snarkvm_b200_lincomb_term_t> terms;
+    for (size_t i = 0; i < count; i++) {
+        const snarkvm_b200_lincomb_segment_t& s = segs[i];
+        if (s.nterms > LINCOMB_MAX) return (int)cudaErrorInvalidValue;
+        outs[i] = snarkvm_b200_lincomb_output_t{s.d_out, s.n, terms.size(), s.nterms};
+        for (uint32_t j = 0; j < s.nterms; j++) {
+            snarkvm_b200_lincomb_term_t t{s.d_polys[j], s.lens[j], 0, 0, 1, {}};
+            memcpy(t.coeff_mont, s.coeffs_mont[j], 32);
+            terms.push_back(t);
+        }
+    }
+    return fr_lincomb_terms_device(outs.data(), count, terms.data(), terms.size(), stream);
 }
 
 int fr_lincomb_device(void* d_out, size_t n, const void* const* d_polys, const size_t* lens, const void* coeffs_mont_host, uint32_t nterms,
@@ -901,6 +980,146 @@ int fr_lincomb_device(void* d_out, size_t n, const void* const* d_polys, const s
         memcpy(s.coeffs_mont[j], (const uint8_t*)coeffs_mont_host + 32 * (size_t)j, 32);
     }
     return fr_lincomb_batch_device(&s, 1, stream);
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Many independent PolyMultiplier products (fft/polynomial/multiplier.rs:70-134) in one pass: one launch loads every zero-padded
+// operand (a into its output, b into scratch), the forward transforms of all 2·count operands go through ntt_batch_device (equal
+// sizes share launches), one launch multiplies pointwise, and the inverse transforms of the outputs go through ntt_batch_device.
+// ---------------------------------------------------------------------------------------------------------------------
+struct PolymulSeg {
+    uint32_t* out;
+    uint32_t* tmp;
+    const uint32_t *a, *b;
+    uint64_t first, n, len_a, len_b;
+};
+__global__ void k_polymul_load(const PolymulSeg* __restrict__ segs, uint32_t nsegs, uint64_t total) {
+    const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= total) return;
+    const PolymulSeg& s = segs[seg_of(segs, nsegs, g)];
+    const uint64_t i = g - s.first;
+    (i < s.len_a ? Fr::load_ldg(s.a + i * 8) : Fr::zero()).store(s.out + i * 8);
+    (i < s.len_b ? Fr::load_ldg(s.b + i * 8) : Fr::zero()).store(s.tmp + i * 8);
+}
+__global__ void k_polymul_pointwise(const PolymulSeg* __restrict__ segs, uint32_t nsegs, uint64_t total) {
+    const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= total) return;
+    const PolymulSeg& s = segs[seg_of(segs, nsegs, g)];
+    const uint64_t i = g - s.first;
+    (Fr::load(s.out + i * 8) * Fr::load(s.tmp + i * 8)).store(s.out + i * 8);
+}
+
+int polymul_batch_device(const snarkvm_b200_polymul_job_t* jobs, size_t count, cudaStream_t stream) {
+    if (count == 0) return 0;
+    if (!jobs || count >= ((size_t)1 << 31)) return (int)cudaErrorInvalidValue;
+    std::vector<PolymulSeg> table(count);
+    std::vector<void*> fwd(2 * count), inv(count);
+    std::vector<uint32_t> fwd_lg(2 * count), inv_lg(count);
+    uint64_t total = 0;
+    for (size_t i = 0; i < count; i++) {
+        const snarkvm_b200_polymul_job_t& j = jobs[i];
+        if (j.lg > NTT_MAX_LG || !j.d_out || !j.d_a || !j.d_b || j.len_a == 0 || j.len_b == 0) return (int)cudaErrorInvalidValue;
+        const uint64_t n = (uint64_t)1 << j.lg;
+        if (j.len_a > n || j.len_b > n || j.len_a + j.len_b - 1 > n) return (int)cudaErrorInvalidValue;
+        table[i] = PolymulSeg{(uint32_t*)j.d_out, nullptr, (const uint32_t*)j.d_a, (const uint32_t*)j.d_b, total, n, j.len_a, j.len_b};
+        total += n;
+    }
+    uint8_t* scratch = nullptr;                                  // segment table | the b operands, concatenated
+    const size_t off_tmp = (count * sizeof(PolymulSeg) + 255) & ~(size_t)255;
+    cudaError_t e = pool_alloc(&scratch, off_tmp + total * 32, stream);
+    if (e != cudaSuccess) return (int)e;
+    uint32_t* tmp = (uint32_t*)(scratch + off_tmp);
+    for (size_t i = 0; i < count; i++) {
+        table[i].tmp = tmp + table[i].first * 8;
+        fwd[i] = table[i].out; fwd[count + i] = table[i].tmp; inv[i] = table[i].out;
+        fwd_lg[i] = fwd_lg[count + i] = inv_lg[i] = jobs[i].lg;
+    }
+    const PolymulSeg* d_table = (const PolymulSeg*)scratch;
+    const unsigned grid = (unsigned)((total + 255) / 256);
+    int rc = (int)cudaMemcpyAsync(scratch, table.data(), count * sizeof(PolymulSeg), cudaMemcpyHostToDevice, stream);
+    if (rc == 0) {
+        k_polymul_load<<<grid, 256, 0, stream>>>(d_table, (uint32_t)count, total);
+        count_launch();
+        rc = (int)cudaGetLastError();
+    }
+    if (rc == 0) rc = ntt_batch_device(fwd.data(), fwd_lg.data(), 2 * count, NTT_FORWARD, NTT_STANDARD, stream);
+    if (rc == 0) {
+        k_polymul_pointwise<<<grid, 256, 0, stream>>>(d_table, (uint32_t)count, total);
+        count_launch();
+        rc = (int)cudaGetLastError();
+    }
+    if (rc == 0) rc = ntt_batch_device(inv.data(), inv_lg.data(), count, NTT_INVERSE, NTT_STANDARD, stream);
+    cudaFreeAsync(scratch, stream);
+    return rc;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Varuna's fourth round (ahp/prover/round_functions/fourth.rs:151-245) on K for every matrix of every circuit: one launch writes
+// a = v_rc·row_col_val, b = |R||C|·(r − α)(c − β) and the denominators (r − α)(c − β) (= (α − r)(β − c)) into one concatenated
+// buffer; one batch inversion (fields/src/lib.rs:78-129, zeros stay zero) runs over all of them; one launch writes
+// f = (v_rc / (|R||C|))·row_col_val / ((r − α)(c − β)).
+// ---------------------------------------------------------------------------------------------------------------------
+struct Round4Seg {
+    const uint32_t *row, *col, *rcv;
+    uint32_t *a, *b, *f;
+    uint64_t first, n;
+    FrArg v_rc, rc, scale;
+};
+__global__ void k_round4_evals(const Round4Seg* __restrict__ segs, uint32_t nsegs, uint64_t total, FrArg alpha_arg, FrArg beta_arg,
+                               uint32_t* __restrict__ den) {
+    const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= total) return;
+    const Round4Seg& s = segs[seg_of(segs, nsegs, g)];
+    const uint64_t i = g - s.first;
+    const Fr d = (Fr::load_ldg(s.row + i * 8) - fr_from_arg(alpha_arg)) * (Fr::load_ldg(s.col + i * 8) - fr_from_arg(beta_arg));
+    (fr_from_arg(s.v_rc) * Fr::load_ldg(s.rcv + i * 8)).store(s.a + i * 8);
+    (fr_from_arg(s.rc) * d).store(s.b + i * 8);
+    d.store(den + g * 8);
+}
+__global__ void k_round4_f(const Round4Seg* __restrict__ segs, uint32_t nsegs, uint64_t total, const uint32_t* __restrict__ inv) {
+    const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= total) return;
+    const Round4Seg& s = segs[seg_of(segs, nsegs, g)];
+    const uint64_t i = g - s.first;
+    (fr_from_arg(s.scale) * Fr::load(inv + g * 8) * Fr::load_ldg(s.rcv + i * 8)).store(s.f + i * 8);
+}
+
+int varuna_round4_evals_device(const snarkvm_b200_round4_segment_t* segs, size_t count, const void* alpha_mont, const void* beta_mont,
+                               cudaStream_t stream) {
+    if (count == 0) return 0;
+    if (!segs || !alpha_mont || !beta_mont || count >= ((size_t)1 << 31)) return (int)cudaErrorInvalidValue;
+    std::vector<Round4Seg> table(count);
+    uint64_t total = 0;
+    for (size_t i = 0; i < count; i++) {
+        const snarkvm_b200_round4_segment_t& s = segs[i];
+        if (s.n == 0 || !s.d_row || !s.d_col || !s.d_row_col_val || !s.d_a || !s.d_b || !s.d_f) return (int)cudaErrorInvalidValue;
+        Round4Seg& t = table[i];
+        t = Round4Seg{(const uint32_t*)s.d_row, (const uint32_t*)s.d_col, (const uint32_t*)s.d_row_col_val, (uint32_t*)s.d_a, (uint32_t*)s.d_b,
+                      (uint32_t*)s.d_f, total, s.n, FrArg{}, FrArg{}, FrArg{}};
+        memcpy(t.v_rc.v, s.v_rc_mont, 32); memcpy(t.rc.v, s.rc_mont, 32); memcpy(t.scale.v, s.f_scale_mont, 32);
+        total += s.n;
+    }
+    FrArg alpha, beta, one{};
+    memcpy(alpha.v, alpha_mont, 32); memcpy(beta.v, beta_mont, 32);
+    for (int k = 0; k < 8; k++) one.v[k] = FrParams::r1(k);                   // Montgomery one
+    uint8_t* scratch = nullptr;                                                  // segment table | denominators, concatenated
+    const size_t off_den = (count * sizeof(Round4Seg) + 255) & ~(size_t)255;
+    cudaError_t e = pool_alloc(&scratch, off_den + total * 32, stream);
+    if (e != cudaSuccess) return (int)e;
+    const Round4Seg* d_table = (const Round4Seg*)scratch;
+    uint32_t* den = (uint32_t*)(scratch + off_den);
+    int rc = (int)cudaMemcpyAsync(scratch, table.data(), count * sizeof(Round4Seg), cudaMemcpyHostToDevice, stream);
+    if (rc == 0) {
+        const unsigned grid = (unsigned)((total + 255) / 256);
+        const size_t threads = (total + BINV_K - 1) / BINV_K;
+        k_round4_evals<<<grid, 256, 0, stream>>>(d_table, (uint32_t)count, total, alpha, beta, den);
+        k_fr_batch_inverse<<<(unsigned)((threads + 127) / 128), 128, 0, stream>>>(den, total, one);
+        k_round4_f<<<grid, 256, 0, stream>>>(d_table, (uint32_t)count, total, den);
+        count_launch(3);
+        rc = (int)cudaGetLastError();
+    }
+    cudaFreeAsync(scratch, stream);
+    return rc;
 }
 
 // ---------------------------------------------------------------------------------------------------------------------

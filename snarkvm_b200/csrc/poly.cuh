@@ -64,6 +64,15 @@ int csr_serialize_batch_device(const snarkvm_b200_csr_segment_t* segs, size_t co
 int fr_lincomb_batch_device(const snarkvm_b200_lincomb_segment_t* segs, size_t count, cudaStream_t stream);
 int matrix_evals_at_points_device(void* out_mont_host, const snarkvm_b200_evals_segment_t* segs, size_t count, cudaStream_t stream);
 
+// The batched Varuna prover's pieces (include/snarkvm_b200.h).  fr_lincomb_batch_device / fr_lincomb_device are calls of
+// fr_lincomb_terms_device, sparse_matvec_device a one-segment call of sparse_matvec_batch_device.
+int fr_lincomb_terms_device(const snarkvm_b200_lincomb_output_t* outs, size_t nouts, const snarkvm_b200_lincomb_term_t* terms, size_t nterms,
+                            cudaStream_t stream);
+int sparse_matvec_batch_device(const snarkvm_b200_spmv_segment_t* segs, size_t count, int64_t* bad_segment, cudaStream_t stream);
+int polymul_batch_device(const snarkvm_b200_polymul_job_t* jobs, size_t count, cudaStream_t stream);
+int varuna_round4_evals_device(const snarkvm_b200_round4_segment_t* segs, size_t count, const void* alpha_mont, const void* beta_mont,
+                               cudaStream_t stream);
+
 // Group FFT over G1 (DomainCoeff = G1Projective, fft/domain.rs:169-221 generic path): n = 2^lg affine points in, affine points
 // out (natural order both sides).  direction 1 = inverse (includes n^{-1}): UniversalParams::lagrange_basis
 // (polycommit/kzg10/data_structures.rs:68-72).

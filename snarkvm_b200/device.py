@@ -607,6 +607,116 @@ def matrix_evals_at_points(jobs: list) -> np.ndarray:
     return out
 
 
+def fr_lincomb_terms(jobs: list, outs: list | None = None) -> list:
+    """Uncapped linear combinations in one launch: job k is (n, terms) with every term (poly, coeff_mont, offset, period, reps) or
+    (poly, coeff_mont, offset) or (poly, coeff_mont): out_k (n Fr) = Σ coeff·poly placed at offset + i·period for i < reps (reps = 1
+    by default).  Terms are contiguous CUDA views (a row slice of a polynomial is one).  `outs[k]`, when given, is the CUDA tensor that
+    receives job k (n rows); otherwise each output is allocated → [out_k], bit-identical to the sequence of additions"""
+    if not jobs:
+        return []
+    if outs is not None and len(outs) != len(jobs):
+        raise ValueError("one output per job")
+    nterms = sum(len(t) for _n, t in jobs)
+    outputs = (_lib.LincombOutput * len(jobs))()
+    terms = (_lib.LincombTerm * max(1, nterms))()
+    dev, result, k = None, [], 0
+    for j, (n, tlist) in enumerate(jobs):
+        for t in tlist:
+            poly, coeff = t[0], t[1]
+            offset, period, reps = (tuple(t[2:]) + (0, 0, 1)[len(t) - 2:])[:3]
+            m = _nbytes(poly) // 32
+            dev = dev or poly.device
+            s = terms[k]
+            s.d_poly, s.len, s.offset, s.period, s.reps = _check(poly, "poly") if m else None, m, offset, period, reps
+            ctypes.memmove(s.coeff_mont, _fr_host(coeff).ctypes.data, 32)
+            k += 1
+        out = outs[j] if outs is not None else None
+        if out is None:
+            out = torch.empty((n, 4), dtype=torch.int64, device=dev or "cuda")
+        elif _nbytes(out) != n * 32:
+            raise ValueError("an output must hold n Fr")
+        outputs[j].d_out, outputs[j].n = _check(out, "out") if n else None, n
+        outputs[j].first_term, outputs[j].nterms = k - len(tlist), len(tlist)
+        result.append(out)
+    with torch.cuda.device(result[0].device):
+        _lib.check(_lib.lib().snarkvm_b200_fr_lincomb_terms_device(outputs, len(jobs), terms, nterms, _stream()))
+    return result
+
+
+def sparse_matvec_batch(jobs: list, outs: list | None = None) -> list:
+    """sparse_matvec of every (row_ptr, cols, vals, x) in one pass (three launches, one synchronisation) → one CUDA tensor [nrows, 4]
+    per job (or into `outs[k]`).  A bad column or row_ptr raises CudaError whose `segment` is the first bad job."""
+    if not jobs:
+        return []
+    segs = (_lib.SpmvSegment * len(jobs))()
+    result = []
+    for k, (row_ptr, cols, vals, x) in enumerate(jobs):
+        rp, nrows, cp, vp, nnz = _csr_args(row_ptr, cols, vals)
+        out = outs[k] if outs is not None else torch.empty((max(nrows, 0), 4), dtype=torch.int64, device=x.device)
+        if _nbytes(out) != nrows * 32:
+            raise ValueError("an output must hold nrows Fr")
+        s = segs[k]
+        s.d_row_ptr, s.d_cols, s.d_vals, s.nrows, s.nnz = rp, cp, vp, nrows, nnz
+        s.d_x, s.nvars, s.d_out = _check(x, "x"), _nbytes(x) // 32, _check(out, "out") if nrows else None
+        result.append(out)
+    bad = ctypes.c_int64(-1)
+    with torch.cuda.device(jobs[0][3].device):
+        _check_segments(_lib.lib().snarkvm_b200_sparse_matvec_batch_device(segs, len(jobs), ctypes.byref(bad), _stream()), bad)
+    return result
+
+
+def polymul_batch(pairs: list) -> list:
+    """PolyMultiplier::multiply of every (a, b) in one pass (one load launch, the forward transforms through ntt_batch_, one pointwise
+    launch, the inverse transforms) → one CUDA tensor [2^lg, 4] per pair, lg = log2 of next_pow2(len a + len b − 1), each equal to
+    polymul(a, b); an empty operand gives an empty product"""
+    outs = []
+    jobs = (_lib.PolymulJob * max(1, len(pairs)))()
+    count = 0
+    for a, b in pairs:
+        la, lb = _nbytes(a) // 32, _nbytes(b) // 32
+        if la == 0 or lb == 0:
+            outs.append(torch.zeros((0, 4), dtype=torch.int64, device=a.device))
+            continue
+        lg = (la + lb - 2).bit_length()
+        out = torch.empty((1 << lg, 4), dtype=torch.int64, device=a.device)
+        j = jobs[count]
+        j.d_out, j.d_a, j.d_b, j.len_a, j.len_b, j.lg = out.data_ptr(), _check(a, "a"), _check(b, "b"), la, lb, lg
+        outs.append(out)
+        count += 1
+    if count:
+        with torch.cuda.device(pairs[0][0].device):
+            _lib.check(_lib.lib().snarkvm_b200_polymul_batch_device(jobs, count, _stream()))
+    return outs
+
+
+def varuna_round4_evals(jobs: list, alpha_mont, beta_mont) -> list:
+    """Varuna's fourth-round evaluations on K for every (row, col, row_col_val, v_rc_mont, rc_mont, f_scale_mont): three launches for all
+    of them → [(a, b, f)], views of one buffer: a = v_rc·row_col_val, b = rc·(row − α)(col − β), f = f_scale·row_col_val /
+    ((row − α)(col − β)), zero where the denominator is zero"""
+    if not jobs:
+        return []
+    dev = jobs[0][0].device
+    sizes = [_nbytes(j[0]) // 32 for j in jobs]
+    buf = torch.empty((3 * sum(sizes), 4), dtype=torch.int64, device=dev)
+    segs = (_lib.Round4Segment * len(jobs))()
+    outs, off = [], 0
+    for k, ((row, col, rcv, v_rc, rc, scale), n) in enumerate(zip(jobs, sizes)):
+        if _nbytes(col) != n * 32 or _nbytes(rcv) != n * 32:
+            raise ValueError("length mismatch")
+        trio = (buf[off: off + n], buf[off + n: off + 2 * n], buf[off + 2 * n: off + 3 * n])
+        off += 3 * n
+        s = segs[k]
+        s.d_row, s.d_col, s.d_row_col_val, s.n = _check(row, "row"), _check(col, "col"), _check(rcv, "row_col_val"), n
+        for name, v in (("v_rc_mont", v_rc), ("rc_mont", rc), ("f_scale_mont", scale)):
+            ctypes.memmove(getattr(s, name), _fr_host(v).ctypes.data, 32)
+        s.d_a, s.d_b, s.d_f = (t.data_ptr() for t in trio)
+        outs.append(trio)
+    a, b = _fr_host(alpha_mont), _fr_host(beta_mont)
+    with torch.cuda.device(dev):
+        _lib.check(_lib.lib().snarkvm_b200_varuna_round4_evals_device(segs, len(jobs), a.ctypes.data, b.ctypes.data, _stream()))
+    return outs
+
+
 def poly_divide_by_linear(p: torch.Tensor, point_mont) -> torch.Tensor:
     """Quotient of p / (x − point), the KZG witness polynomial (kzg10/mod.rs:220-241) → CUDA tensor [m − 1, 4] i64, not trimmed."""
     z = _fr_host(point_mont)

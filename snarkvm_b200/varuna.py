@@ -529,168 +529,146 @@ def verify_vk(circuit: Circuit, vk: CircuitVerifyingKey, certificate: Certificat
     return verify_vk_batch([circuit], [vk], [certificate], [challenges], [opening_challenge])[0]
 
 
-class Prover:
-    """init_prover + State::initialize (round_functions/mod.rs:43-170, state.rs:107-178) and the five rounds.
-    `assignments`: one CUDA tensor [num_variables, 4] per instance — padded public variables (first one is One) then private."""
+def witness_label(circuit_id: bytes, poly: str, i: int) -> str:
+    """ahp/ahp.rs:46-50: circuit_{id as hex}_{poly}_{i:08}"""
+    return f"circuit_{circuit_id.hex()}_{poly}_{i:08}"
 
-    def __init__(self, circuit: Circuit, assignments: list):
-        self.circuit = c = circuit
-        self.batch = len(assignments)
-        self.z = [z.contiguous() for z in assignments]
-        for z in self.z:
-            if z.shape[0] != c.num_variables:
-                raise ValueError("instance does not match the index")                       # AHPError::InstanceDoesNotMatchIndex
-        self.z_a = [device.sparse_matvec(c.a.row_ptr, c.a.cols, c.a.vals, z) for z in self.z]
-        self.z_b = [device.sparse_matvec(c.b.row_ptr, c.b.cols, c.b.vals, z) for z in self.z]
-        self.z_c = [device.sparse_matvec(c.c.row_ptr, c.c.cols, c.c.vals, z) for z in self.z]
-        self.x_polys = [c.input_domain.ifft(z[: c.num_public]) for z in self.z]                 # state.rs:137-139
 
-    # ---- round 1: calculate_w (first.rs:129-160) ----
-    def first_round(self):
-        c = self.circuit
-        V, I = c.variable_domain, c.input_domain
-        dev = self.z[0].device
-        # the index plumbing of calculate_w depends only on the two domain sizes: built once per circuit and device, on the device
-        # (building it with numpy and uploading it every proof was most of the round's time at 2^20 constraints)
-        cache = c.__dict__.setdefault("_w_index", {})
-        if dev not in cache:
-            ratio = V.size // I.size
-            k = torch.arange(V.size, dtype=torch.int64, device=dev)
-            mask = (k % ratio) != 0
-            cache[dev] = (k[mask].contiguous(), (k - torch.div(k, ratio, rounding_mode="floor") - 1)[mask].contiguous())
-        keep, src = cache[dev]
-        self.w_polys = []
-        for z, x_poly in zip(self.z, self.x_polys):
-            w_ext = _zeros(V.size - I.size, dev)
-            prv = z[c.num_public:]
-            w_ext[: prv.shape[0]] = prv
-            x_evals = V.fft_in_place(_pad(x_poly, V.size).clone())
-            evals = _zeros(V.size, dev)
-            evals[keep] = device.fr_vec_op(w_ext[src].contiguous(), x_evals[keep].contiguous(), device.FR_SUB)
-            w_poly, _rem = divide_by_vanishing(V.ifft_in_place(evals), I)
-            self.w_polys.append(w_poly)
-        return self.w_polys
+def _vanish(d: EvaluationDomain, x: int) -> int:
+    return (pow(x, d.size, R_MOD) - 1) % R_MOD
 
-    # ---- calculate_assignments (third.rs:207-234): z = w·v_I + x ----
-    def assignments(self):
-        I = self.circuit.input_domain
-        self.z_polys = [_add(mul_by_vanishing(w, I), x) for w, x in zip(self.w_polys, self.x_polys)]
-        return self.z_polys
 
-    # ---- round 2: calculate_rowcheck_witness (second.rs:77-146) ----
-    def second_round(self, circuit_combiner: int = 1, instance_combiners=None):
-        c = self.circuit
-        Rd = c.constraint_domain
-        instance_combiners = instance_combiners or [1] * self.batch
-        h_0 = _zeros(0, self.z[0].device)
-        for comb, za, zb, zc in zip(instance_combiners, self.z_a, self.z_b, self.z_c):
-            pa, pb, pc = (Rd.ifft_in_place(_pad(e, Rd.size).clone()) for e in (za, zb, zc))
-            rowcheck = _sub(polymul(pa, pb), pc)
-            h_i, _ = apply_randomized_selector(_scale(rowcheck, comb), circuit_combiner, Rd, Rd, False)
-            h_0 = _add(h_0, h_i)
-        self.h_0 = h_0
-        return h_0
+def _selector(target: EvaluationDomain, src: EvaluationDomain, x: int) -> int:
+    """the selector of src inside target at x (selectors.rs): v_target(x)·|src| / (v_src(x)·|target|); one when they are equal"""
+    if target.size == src.size:
+        return 1
+    return _vanish(target, x) * src.size % R_MOD * pow(_vanish(src, x) * target.size % R_MOD, -1, R_MOD) % R_MOD
 
-    # ---- evaluate_all_lagrange_coefficients (fft/domain.rs:258-292) on the device ----
-    @staticmethod
-    def lagrange_coefficients(domain: EvaluationDomain, tau: int, dev) -> torch.Tensor:
-        return domain.evaluate_all_lagrange_coefficients(tau, dev)
 
-    # ---- round 3: lineval sumcheck (third.rs:126-205, 266-326) ----
-    def third_round(self, alpha: int, eta_b: int, eta_c: int, circuit_combiner: int = 1, instance_combiners=None):
-        c = self.circuit
-        Rd, V = c.constraint_domain, c.variable_domain
-        dev = self.z[0].device
-        instance_combiners = instance_combiners or [1] * self.batch
-        l_at_alpha = self.lagrange_coefficients(Rd, alpha, dev)
-        h_1, xg_1, sums = _zeros(0, dev), _zeros(0, dev), []
-        m_polys = []
-        for tm in c.transposes:
-            m_evals = device.sparse_matvec(tm.row_ptr, tm.cols, tm.vals, l_at_alpha)            # M(α, c) for every c ∈ C
-            m_polys.append(V.ifft_in_place(m_evals))
-        for inst_comb, z_poly in zip(instance_combiners, self.z_polys):
-            inst_sums = []
-            for m_at_alpha, m_comb in zip(m_polys, (1, eta_b % R_MOD, eta_c % R_MOD)):
-                z_m = polymul(m_at_alpha, z_poly)
-                # Σ_{c ∈ C} z_m(c) = |C| · Σ_j coefficient_{j·|C|}
-                picks = device.fr_from_mont(z_m[:: V.size].contiguous()).cpu().numpy().view(np.uint64)
-                inst_sums.append(V.size * sum(sum(int(v) << (64 * i) for i, v in enumerate(row)) for row in picks) % R_MOD)
-                combiner = circuit_combiner * inst_comb % R_MOD * m_comb % R_MOD
-                h_i, xg_i = apply_randomized_selector(z_m, combiner, V, V, True)
-                h_1, xg_1 = _add(h_1, h_i), _add(xg_1, xg_i)
-            sums.append(inst_sums)
-        if self.mask_poly is not None:                                  # third.rs:207-213 (hiding mode)
-            h_mask, xg_mask = divide_by_vanishing(self.mask_poly, V)
-            h_1, xg_1 = _add(h_1, h_mask), _add(xg_1, xg_mask)
-        self.h_1, self.g_1, self.third_sums = h_1, xg_1[1:].contiguous(), sums
-        return self.g_1, self.h_1
+def _largest(domains) -> EvaluationDomain:
+    return max(domains, key=lambda d: d.size)
 
-    # ---- AHPForR1CS::construct_linear_combinations (ahp/ahp.rs:172-389) + verifier_query_set, one circuit ----
-    def polynomials(self) -> dict:
-        """label → device polynomial, everything prove_batch hands to open_combinations (varuna.rs:509-517)"""
-        out = {f"w_{j}": w for j, w in enumerate(self.w_polys)}
-        if self.mask_poly is not None:
-            out["mask_poly"] = self.mask_poly
-        out.update({"h_0": self.h_0, "g_1": self.g_1, "h_1": self.h_1, "h_2": self.h_2})
-        for m, g, a, b in zip("abc", self.gs, self.a_polys, self.b_polys):
-            out[f"g_{m}"], out[f"a_poly_{m}"], out[f"b_poly_{m}"] = g, a, b
+
+class BatchProver:
+    """init_prover + State::initialize and the five AHP rounds of VarunaSNARK::prove_batch (varuna.rs:336-620) for K circuits, each with
+    its own batch of instances.  `program`: [(Circuit, [assignment, …])], an assignment being one CUDA tensor [num_variables, 4] per
+    instance (padded public variables, the first one One, then private).  The circuits are taken in Circuit.id() order, as the
+    reference keys its prover state by circuit and orders circuits by id (ahp/indexer/circuit.rs:96-100); `circuits`, and every
+    per-circuit argument and attribute, follow that order, so the order of `program` changes no result.  A one-circuit batch never
+    computes the id.  Challenges are arguments (the Poseidon sponge stays with the caller):
+        batch_combiners: per circuit (circuit combiner, [one combiner per instance]),
+        deltas:          per circuit (δ_a, δ_b, δ_c).
+    Per-circuit O(n) work runs as segmented kernels: one pass for a round's mat-vecs, products, fourth-round evaluations and selector
+    sums, whatever the number of circuits and instances (launches grow only with the number of distinct domain sizes)."""
+
+    def __init__(self, program: list):
+        if not program:
+            raise ValueError("no circuits to prove")
+        for k, (c, zs) in enumerate(program):
+            if not zs:
+                raise ValueError(f"circuit {k}: no instances")
+            for z in zs:
+                if z.shape[0] != c.num_variables:                       # AHPError::InstanceDoesNotMatchIndex
+                    raise ValueError(f"circuit {k}: instance does not match the index ({z.shape[0]} variables, the index has "
+                                     f"{c.num_variables})")
+        self.dev = _device_of([c for c, _ in program])
+        if any(z.device != self.dev for _, zs in program for z in zs):
+            raise ValueError("an assignment lives on another device than its circuit")
+        order = [0]
+        if len(program) > 1:
+            ids = circuit_ids([c for c, _ in program])
+            if len(set(ids)) != len(ids):
+                raise ValueError("two entries of the program have equal circuit ids")
+            order = sorted(range(len(program)), key=lambda k: ids[k])
+        self.positions = order                                            # circuit i of the batch is program[positions[i]]
+        self.circuits = [program[k][0] for k in order]
+        self.z = [[z.contiguous() for z in program[k][1]] for k in order]
+        self.batch = [len(zs) for zs in self.z]
+        cs = self.circuits
+        self.max_constraint_domain = _largest(c.constraint_domain for c in cs)
+        self.max_variable_domain = _largest(c.variable_domain for c in cs)
+        self.max_non_zero_domain = _largest(c.max_non_zero_domain for c in cs)
+        # z_A, z_B, z_C of every instance (round_functions/mod.rs:128-152): one pass, each written into a zeroed |R|-row slot so that
+        # round 2 interpolates them without a per-instance copy
+        slots = [(i, j, m) for i, c in enumerate(cs) for j in range(self.batch[i]) for m in range(3)]
+        sizes = [cs[i].constraint_domain.size for i, _j, _m in slots]
+        self._zbuf = _zeros(sum(sizes), self.dev)
+        offs = np.concatenate([[0], np.cumsum(sizes)]).tolist()
+        outs = [self._zbuf[o: o + cs[i].num_constraints] for o, (i, _j, _m) in zip(offs, slots)]
+        self._zslots = list(zip(offs, sizes))
+        jobs = [(mat.row_ptr, mat.cols, mat.vals, self.z[i][j]) for i, j, m in slots for mat in ((cs[i].a, cs[i].b, cs[i].c)[m],)]
+        try:
+            device.sparse_matvec_batch(jobs, outs)
+        except CudaError as e:
+            seg = getattr(e, "segment", None)
+            if seg is None:
+                raise
+            i, _j, m = slots[seg]
+            raise CudaError(e.code, f"circuit {self.positions[i]}: matrix {'abc'[m]} has a column ≥ num_variables or a row_ptr that does not "
+                                    "run from 0 to nnz") from None
+        it = iter(outs)
+        self.z_a, self.z_b, self.z_c = ([[None] * b for b in self.batch] for _ in range(3))
+        for i, j, m in slots:
+            (self.z_a, self.z_b, self.z_c)[m][i][j] = next(it)
+        # x_poly (state.rs:137-139): the interpolations of every instance's public part in one batched iNTT
+        pubs = [self.z[i][j][: c.num_public] for i, c in enumerate(cs) for j in range(self.batch[i])]
+        xbuf = torch.cat(pubs) if len(pubs) > 1 else pubs[0].clone()
+        offs = np.concatenate([[0], np.cumsum([p.shape[0] for p in pubs])]).tolist()
+        flat = [xbuf[a: b] for a, b in zip(offs, offs[1:])]
+        device.ntt_batch_(flat, NTTDirection.Inverse, NTTType.Standard)
+        self.x_polys = self._per_circuit(flat)
+        self.mask_poly = None
+
+    def _per_circuit(self, flat: list) -> list:
+        out, it = [], iter(flat)
+        for b in self.batch:
+            out.append([next(it) for _ in range(b)])
         return out
 
-    @staticmethod
-    def _eval(poly: torch.Tensor, point: int) -> int:
-        return _fr_mont_to_int(device.poly_evaluate(poly.contiguous(), _mont(point))) if poly.shape[0] else 0
+    def _combiners(self, batch_combiners) -> list:
+        if batch_combiners is None:
+            return [(1, [1] * b) for b in self.batch]
+        if len(batch_combiners) != len(self.circuits):
+            raise ValueError(f"{len(batch_combiners)} sets of batch combiners for {len(self.circuits)} circuits")
+        out = []
+        for (cc, inst), b in zip(batch_combiners, self.batch):
+            if len(inst) != b:
+                raise ValueError(f"{len(inst)} instance combiners for {b} instances")
+            out.append((int(cc) % R_MOD, [int(x) % R_MOD for x in inst]))
+        return out
 
-    def linear_combinations(self, alpha, eta_b, eta_c, beta, deltas, gamma, circuit_combiner: int = 1, instance_combiners=None):
-        """→ (lcs, query_set) exactly as oracle/varuna.py Prover.linear_combinations: the coefficients are host integers (a few dozen
-        field operations), the three evaluations they need — g_1(β), g_M(γ), x_j(β) — are device Horner passes."""
-        c = self.circuit
-        Rd, V, I, K = c.constraint_domain, c.variable_domain, c.input_domain, c.max_non_zero_domain
-        vanish = lambda d, x: (pow(x, d.size, R_MOD) - 1) % R_MOD       # noqa: E731
-        instance_combiners = instance_combiners or [1] * self.batch
-        lcs = {}
-        const = 0
-        for comb, sums in zip(instance_combiners, self.third_sums):
-            const = (const + comb * (sums[0] * sums[1] - sums[2])) % R_MOD
-        lcs["rowcheck_zerocheck"] = [(circuit_combiner * const % R_MOD, None), ((-vanish(Rd, alpha)) % R_MOD, "h_0")]
-        lcs["g_1"] = [(1, "g_1")]
-        v_c_beta, v_x_beta = vanish(V, beta), vanish(I, beta)
-        g_1_at_beta = self._eval(self.g_1, beta)
-        doms = [a.domain for a in c.ariths]
-        sums4 = [s * d.size % R_MOD for s, d in zip(self.fourth_sums, doms)]
-        weight = (sums4[0] + sums4[1] * eta_b + sums4[2] * eta_c) % R_MOD
-        lineval = [(1, "mask_poly")] if self.mask_poly is not None else []
-        for j, comb in enumerate(instance_combiners):
-            x_at_beta = self._eval(self.x_polys[j], beta)
-            k = circuit_combiner * comb % R_MOD
-            lineval.append((k * weight % R_MOD * x_at_beta % R_MOD, None))
-            lineval.append((k * weight % R_MOD * v_x_beta % R_MOD, f"w_{j}"))
-        batch_lineval_sum = circuit_combiner * sum(comb * (s[0] + eta_b * s[1] + eta_c * s[2]) for comb, s in zip(instance_combiners, self.third_sums)) % R_MOD \
-            * pow(V.size, -1, R_MOD) % R_MOD
-        lineval += [((-v_c_beta) % R_MOD, "h_1"), ((-beta * g_1_at_beta) % R_MOD, None), ((-batch_lineval_sum) % R_MOD, None)]
-        lcs["lineval_sumcheck"] = lineval
-        v_k_gamma = vanish(K, gamma)
-        matrix = []
-        for m, g, s, delta, dom in zip("abc", self.gs, self.fourth_sums, deltas, doms):
-            lcs[f"g_{m}"] = [(1, f"g_{m}")]
-            selector = v_k_gamma * dom.size % R_MOD * pow(vanish(dom, gamma) * K.size % R_MOD, -1, R_MOD) % R_MOD
-            b_term = (gamma * self._eval(g, gamma) + s) % R_MOD
-            matrix.append((delta * selector % R_MOD, f"a_poly_{m}"))
-            matrix.append(((-delta * selector % R_MOD * b_term) % R_MOD, f"b_poly_{m}"))
-        matrix.append(((-v_k_gamma) % R_MOD, "h_2"))
-        lcs["matrix_sumcheck"] = matrix
-        points = {"rowcheck_zerocheck": ("alpha", alpha), "g_1": ("beta", beta), "lineval_sumcheck": ("beta", beta),
-                  "g_a": ("gamma", gamma), "g_b": ("gamma", gamma), "g_c": ("gamma", gamma), "matrix_sumcheck": ("gamma", gamma)}
-        order = sorted(lcs)
-        return [(k, lcs[k]) for k in order], [(k, points[k]) for k in order]
-
-    mask_poly = None
+    # ---- round 1: calculate_w (first.rs:129-160), per instance ----
+    def first_round(self):
+        self.w_polys = []
+        for c, zs, xs in zip(self.circuits, self.z, self.x_polys):
+            V, I = c.variable_domain, c.input_domain
+            # the index plumbing of calculate_w depends only on the two domain sizes: built once per circuit and device
+            cache = c.__dict__.setdefault("_w_index", {})
+            if self.dev not in cache:
+                ratio = V.size // I.size
+                k = torch.arange(V.size, dtype=torch.int64, device=self.dev)
+                mask = (k % ratio) != 0
+                cache[self.dev] = (k[mask].contiguous(), (k - torch.div(k, ratio, rounding_mode="floor") - 1)[mask].contiguous())
+            keep, src = cache[self.dev]
+            ws = []
+            for z, x_poly in zip(zs, xs):
+                w_ext = _zeros(V.size - I.size, self.dev)
+                prv = z[c.num_public:]
+                w_ext[: prv.shape[0]] = prv
+                x_evals = V.fft_in_place(_pad(x_poly, V.size).clone())
+                evals = _zeros(V.size, self.dev)
+                evals[keep] = device.fr_vec_op(w_ext[src].contiguous(), x_evals[keep].contiguous(), device.FR_SUB)
+                w_poly, _rem = divide_by_vanishing(V.ifft_in_place(evals), I)
+                ws.append(w_poly)
+            self.w_polys.append(ws)
+        return self.w_polys
 
     def set_mask_poly(self, h_1_mask_rand, g_1_mask_rand):
-        """calculate_mask_poly (first.rs:102-127) for the hiding mode: rand(degree 3)·v_H on the variable domain plus rand(degree 5)
-        with a zero constant term; the random coefficients (ints) are arguments.  The mask is a first-round oracle (committed without a
-        degree or hiding bound, first.rs:54-56) and enters h_1 / g_1 in the third round."""
+        """calculate_mask_poly (first.rs:102-127) for the hiding mode, over the LARGEST variable domain: rand(degree 3)·v_H plus
+        rand(degree 5) with a zero constant term; the random coefficients (ints) are arguments.  A first-round oracle (no degree or
+        hiding bound, first.rs:54-56) that enters h_1 / g_1 in the third round."""
         assert len(h_1_mask_rand) == 4 and len(g_1_mask_rand) == 6
-        n = self.circuit.variable_domain.size
+        n = self.max_variable_domain.size
         mask = [0] * (n + 4)
         for i, c in enumerate(h_1_mask_rand):
             mask[n + i] = (mask[n + i] + c) % R_MOD
@@ -698,50 +676,333 @@ class Prover:
         for i, c in enumerate(g_1_mask_rand):
             if i:
                 mask[i] = (mask[i] + c) % R_MOD
-        dev = self.z[0].device
         idx = sorted(set(range(6)) | set(range(n, n + 4)))              # the (at most ten) non-zero coefficients
         vals = np.array([_mont(mask[i]) for i in idx], dtype=np.uint64).reshape(-1, 4)
-        self.mask_poly = _zeros(n + 4, dev)
-        self.mask_poly[torch.tensor(idx, dtype=torch.int64, device=dev)] = torch.from_numpy(vals.view(np.int64)).to(dev)
+        self.mask_poly = _zeros(n + 4, self.dev)
+        self.mask_poly[torch.tensor(idx, dtype=torch.int64, device=self.dev)] = torch.from_numpy(vals.view(np.int64)).to(self.dev)
         return self.mask_poly
 
-    # ---- round 4: matrix sumchecks (fourth.rs:151-245) ----
+    # ---- calculate_assignments (third.rs:207-234): z = w·v_I + x, one launch for every instance ----
+    def assignments(self):
+        jobs = []
+        for c, ws, xs in zip(self.circuits, self.w_polys, self.x_polys):
+            I = c.input_domain.size
+            for w, x in zip(ws, xs):
+                jobs.append((I + w.shape[0], [(x, _mont(1)), (w, _mont(-1)), (w, _mont(1), I)]))
+        self.z_polys = self._per_circuit(device.fr_lincomb_terms(jobs))
+        return self.z_polys
+
+    # ---- round 2: h_0 (second.rs:76-142) ----
+    def second_round(self, batch_combiners=None):
+        """h_0 = Σ over circuits and instances of apply_randomized_selector(comb_inst·rowcheck, comb_circuit, R_max, R_i, false).  The
+        rowcheck z_A·z_B − z_C has degree < 2|R_i| and z_C degree < |R_i|, so its quotient by v_{R_i} is the upper half of z_A·z_B:
+        one batched iNTT, one batched product and one selector sum for the whole batch."""
+        combs = self._combiners(batch_combiners)
+        R = self.max_constraint_domain
+        evals = self._zbuf.clone()                                        # z_A, z_B of every instance, interpolated in place
+        ab = [evals[o: o + n] for k, (o, n) in enumerate(self._zslots) if k % 3 != 2]
+        device.ntt_batch_(ab, NTTDirection.Inverse, NTTType.Standard)
+        prods = device.polymul_batch(list(zip(ab[0::2], ab[1::2])))
+        terms, k = [], 0
+        for c, (cc, inst) in zip(self.circuits, combs):
+            n = c.constraint_domain.size
+            scale = cc * n % R_MOD * pow(R.size, -1, R_MOD) % R_MOD
+            for comb in inst:
+                p = prods[k]
+                k += 1
+                terms.append((p[n:], _mont(comb * scale)))
+        n_out = max(t[0].shape[0] for t in terms)
+        self.h_0 = device.fr_lincomb_terms([(n_out, terms)])[0]
+        return self.h_0
+
+    # ---- evaluate_all_lagrange_coefficients (fft/domain.rs:258-292) on the device ----
+    @staticmethod
+    def lagrange_coefficients(domain: EvaluationDomain, tau: int, dev) -> torch.Tensor:
+        return domain.evaluate_all_lagrange_coefficients(tau, dev)
+
+    # ---- round 3: lineval sumcheck (third.rs:126-218, 280-326) ----
+    def third_round(self, alpha: int, eta_b: int, eta_c: int, batch_combiners=None):
+        """h_1 and g_1 over C_max (remainder witness, target C_max, source C_i) and the per-instance sums |C_i|·Σ_j coeff_{j·|C_i|}.
+        M(α, ·) of every transpose is one segmented mat-vec (α is shared: one Lagrange vector per distinct |R|), their interpolation
+        one batched iNTT, the 3·Σ instances products M(α)·z one batched product; the sums and both selector sums are one launch and
+        the sums reach the host in one copy."""
+        combs = self._combiners(batch_combiners)
+        cs, C = self.circuits, self.max_variable_domain
+        lag = {}
+        for c in cs:
+            if c.constraint_domain.size not in lag:
+                lag[c.constraint_domain.size] = self.lagrange_coefficients(c.constraint_domain, alpha, self.dev)
+        m_evals = device.sparse_matvec_batch([(t.row_ptr, t.cols, t.vals, lag[c.constraint_domain.size]) for c in cs for t in c.transposes])
+        device.ntt_batch_(m_evals, NTTDirection.Inverse, NTTType.Standard)
+        pairs, owners = [], []
+        for i, c in enumerate(cs):
+            for j, z_poly in enumerate(self.z_polys[i]):
+                for m in range(3):
+                    pairs.append((m_evals[3 * i + m], z_poly))
+                    owners.append((i, j, m))
+        prods = device.polymul_batch(pairs)
+        sums_buf = _zeros(len(prods), self.dev)
+        sum_jobs, h_terms, xg_terms = [], [], []
+        etas = (1, eta_b % R_MOD, eta_c % R_MOD)
+        for (i, j, m), z_m in zip(owners, prods):
+            n = cs[i].variable_domain.size
+            # Σ_{c ∈ C_i} z_m(c) = |C_i| · Σ_j coefficient_{j·|C_i|}
+            sum_jobs.append((1, [(z_m[k: k + 1], _mont(1)) for k in range(0, z_m.shape[0], n)]))
+            cc, inst = combs[i]
+            mult = cc * inst[j] % R_MOD * etas[m] % R_MOD * n % R_MOD * pow(C.size, -1, R_MOD) % R_MOD
+            assert z_m.shape[0] <= 2 * n
+            lo, hi = z_m[:n], z_m[n:]
+            h_terms.append((hi, _mont(mult)))
+            # the remainder lo + hi times v_{C_max} / v_{C_i}: |C_max| / |C_i| copies of it, |C_i| apart
+            xg_terms += [(lo, _mont(mult), 0, n, C.size // n), (hi, _mont(mult), 0, n, C.size // n)]
+        if self.mask_poly is not None:                                  # third.rs:207-213 (hiding mode)
+            h_mask, xg_mask = divide_by_vanishing(self.mask_poly, C)
+            h_terms.append((h_mask, _mont(1)))
+            xg_terms.append((xg_mask, _mont(1)))
+        n_h = max(t[0].shape[0] for t in h_terms)
+        n_xg = C.size
+        *_sums, self.h_1, xg_1 = device.fr_lincomb_terms(sum_jobs + [(n_h, h_terms), (n_xg, xg_terms)],
+                                                         [sums_buf[k: k + 1] for k in range(len(prods))] + [None, None])
+        self.g_1 = xg_1[1:]
+        host = device.fr_from_mont(sums_buf).cpu().numpy().view(np.uint64)
+        self.third_sums = [[[0, 0, 0] for _ in range(b)] for b in self.batch]
+        for (i, j, m), row in zip(owners, host):
+            n = cs[i].variable_domain.size
+            self.third_sums[i][j][m] = n * sum(int(v) << (64 * t) for t, v in enumerate(row)) % R_MOD
+        return self.g_1, self.h_1
+
+    # ---- round 4: matrix sumchecks (fourth.rs:79-245) ----
     def fourth_round(self, alpha: int, beta: int):
-        c = self.circuit
-        Rd, V = c.constraint_domain, c.variable_domain
-        v_rc = (pow(alpha, Rd.size, R_MOD) - 1) * (pow(beta, V.size, R_MOD) - 1) % R_MOD
-        rc_size = Rd.size * V.size % R_MOD
-        consts = v_rc * pow(Rd.size, -1, R_MOD) % R_MOD * pow(V.size, -1, R_MOD) % R_MOD
+        """per matrix of every circuit, with that circuit's v_{R_i}(α)·v_{C_i}(β) and |R_i|·|C_i|; the selector goes from K_matrix to the
+        global K_max.  The evaluations of all 3K matrices are three launches, their 9K interpolations one batched iNTT, the products
+        b·f one batched product, the 3K quotients one launch; the 3K sums f[0] reach the host in one copy."""
+        cs, Kmax = self.circuits, self.max_non_zero_domain
+        jobs = []
+        for c in cs:
+            Rd, V = c.constraint_domain, c.variable_domain
+            v_rc = _vanish(Rd, alpha) * _vanish(V, beta) % R_MOD
+            rc = Rd.size * V.size % R_MOD
+            scale = v_rc * pow(Rd.size, -1, R_MOD) % R_MOD * pow(V.size, -1, R_MOD) % R_MOD
+            for arith in c.ariths:
+                jobs.append((arith.row, arith.col, arith.row_col_val, _mont(v_rc), _mont(rc), _mont(scale)))
+        evals = device.varuna_round4_evals(jobs, _mont(alpha), _mont(beta))
+        device.ntt_batch_([t for trio in evals for t in trio], NTTDirection.Inverse, NTTType.Standard)
+        bf = device.polymul_batch([(b, f) for _a, b, f in evals])
+        doms = [a.domain for c in cs for a in c.ariths]
+        lhs = device.fr_lincomb_terms([(d.size, [(p[d.size:], _mont(-d.size * pow(Kmax.size, -1, R_MOD)))]) for p, d in zip(bf, doms)])
+        f0 = torch.stack([f[0] for _a, _b, f in evals]).cpu().numpy().view(np.uint64)
         self.gs, self.lhs, self.fourth_sums, self.a_polys, self.b_polys = [], [], [], [], []
-        for arith in c.ariths:
-            K = arith.domain
-            a_poly = K.ifft_in_place(_scale(arith.row_col_val, v_rc).clone())
-            # (α − r)(β − c) = (r − α)(c − β): the common factor of b's evaluations and of the denominators
-            ra = device.fr_vec_op(arith.row, _mont(alpha), device.FR_SUB)
-            cb = device.fr_vec_op(arith.col, _mont(beta), device.FR_SUB)
-            prod = device.fr_vec_op(ra, cb, device.FR_MUL)
-            b_poly = K.ifft_in_place(_scale(prod, rc_size).clone())                          # |R||C|(αβ − βr − αc + rc)
-            device.fr_batch_inversion_and_mul(prod, _mont(consts))                            # fields/src/lib.rs:78-129
-            f = K.ifft_in_place(device.fr_vec_op(prod, arith.row_col_val, device.FR_MUL))
-            h = _sub(a_poly, polymul(b_poly, f))
-            lhs, _ = apply_randomized_selector(h, 1, c.max_non_zero_domain, K, False)
-            self.gs.append(f[1:].contiguous()); self.lhs.append(lhs)
-            self.fourth_sums.append(_fr_mont_to_int(f[0].cpu().numpy().view(np.uint64)))
-            self.a_polys.append(a_poly); self.b_polys.append(b_poly)
+        for i in range(len(cs)):
+            trio = evals[3 * i: 3 * i + 3]
+            self.gs.append([f[1:] for _a, _b, f in trio])
+            self.lhs.append(lhs[3 * i: 3 * i + 3])
+            self.fourth_sums.append([_fr_mont_to_int(f0[3 * i + m]) for m in range(3)])
+            self.a_polys.append([a for a, _b, _f in trio])
+            self.b_polys.append([b for _a, b, _f in trio])
         return self.gs
 
-    # ---- round 5 (fifth.rs:41-67) ----
+    # ---- round 5 (fifth.rs:43-67): h_2 = Σ δ·lhs over all 3K matrices, one launch ----
     def fifth_round(self, deltas):
-        h_2 = _zeros(0, self.z[0].device)
-        for d, lhs in zip(deltas, self.lhs):
-            h_2 = _add(h_2, _scale(lhs, d % R_MOD))
-        self.h_2 = h_2
-        return h_2
+        if len(deltas) != len(self.circuits) or any(len(d) != 3 for d in deltas):
+            raise ValueError(f"one (δ_a, δ_b, δ_c) per circuit: {len(self.circuits)} circuits")
+        terms = [(lhs, _mont(int(d) % R_MOD)) for ds, ls in zip(deltas, self.lhs) for d, lhs in zip(ds, ls)]
+        self.h_2 = device.fr_lincomb_terms([(max(t[0].shape[0] for t in terms), terms)])[0]
+        return self.h_2
+
+    # ---- labels, oracles, linear combinations ----
+    def _labels(self):
+        """label(i, name, j) of circuit i's polynomial: the reference's witness_label names (ahp.rs:46-50; a_poly / b_poly as
+        construct_matrix_linear_combinations names them, ahp.rs:408-409)"""
+        ids = circuit_ids(self.circuits)
+
+        def label(i, name, j=0):
+            if name in ("a_poly", "b_poly"):
+                return f"circuit_{ids[i].hex()}_{name}_{'abc'[j]}"
+            return witness_label(ids[i], name, j)
+        return label
+
+    def polynomials(self, label=None) -> dict:
+        """label → device polynomial, everything prove_batch hands to open_combinations, in its order (varuna.rs:509-517): the a and b
+        polynomials of every circuit, the first-round oracles (w of every instance, then mask_poly), h_0, g_1, h_1, every g_M, h_2"""
+        label = label or self._labels()
+        out = {}
+        for i, ps in enumerate(self.a_polys):
+            out.update({label(i, "a_poly", m): p for m, p in enumerate(ps)})
+        for i, ps in enumerate(self.b_polys):
+            out.update({label(i, "b_poly", m): p for m, p in enumerate(ps)})
+        for i, ws in enumerate(self.w_polys):
+            out.update({label(i, "w", j): w for j, w in enumerate(ws)})
+        if self.mask_poly is not None:
+            out["mask_poly"] = self.mask_poly
+        out.update({"h_0": self.h_0, "g_1": self.g_1, "h_1": self.h_1})
+        for i, gs in enumerate(self.gs):
+            out.update({label(i, f"g_{m}", 0): g for m, g in zip("abc", gs)})
+        out["h_2"] = self.h_2
+        return out
 
     def oracles(self) -> dict:
         """every polynomial the prover commits to, by round (varuna.rs:387-506)"""
-        first = list(self.w_polys) + ([self.mask_poly] if self.mask_poly is not None else [])
-        return {1: first, 2: [self.h_0], 3: [self.g_1, self.h_1], 4: list(self.gs), 5: [self.h_2]}
+        first = [w for ws in self.w_polys for w in ws] + ([self.mask_poly] if self.mask_poly is not None else [])
+        return {1: first, 2: [self.h_0], 3: [self.g_1, self.h_1], 4: [g for gs in self.gs for g in gs], 5: [self.h_2]}
+
+    def labeled_oracles(self, zk: bool = False, label=None, rounds=(1, 2, 3, 4, 5)) -> dict:
+        """round → [sonic_pc.LabeledPolynomial] for each of `rounds` (all computed already) with the reference's bounds (first.rs,
+        third.rs, fourth.rs polynomial infos): g_1 bounded by |C_max| − 2, each circuit's g_M by its own |K_M| − 2; in the hiding mode
+        (zk) w, g_1 and g_M carry hiding bound 1.  Each round's list commits in ONE SonicKZG10.commit pass, whose passes take mixed
+        degree bounds as they are."""
+        from .sonic_pc import LabeledPolynomial
+        label = label or self._labels()
+        hb = 1 if zk else None
+
+        def fit(p, bound):                                               # device polynomials may carry trailing zeros
+            return p[: bound + 1] if p.shape[0] > bound + 1 else p
+
+        def first():
+            out = [LabeledPolynomial(label(i, "w", j), w, None, hb) for i, ws in enumerate(self.w_polys) for j, w in enumerate(ws)]
+            if self.mask_poly is not None:
+                out.append(LabeledPolynomial("mask_poly", self.mask_poly, None, None))
+            return out
+
+        def third():
+            bg1 = self.max_variable_domain.size - 2
+            return [LabeledPolynomial("g_1", fit(self.g_1, bg1), bg1, hb), LabeledPolynomial("h_1", self.h_1, None, None)]
+
+        def fourth():
+            return [LabeledPolynomial(label(i, f"g_{m}", 0), fit(g, d.size - 2), d.size - 2, hb)
+                    for i, (c, gs) in enumerate(zip(self.circuits, self.gs)) for m, g, d in zip("abc", gs, c.non_zero_domains)]
+        build = {1: first, 2: lambda: [LabeledPolynomial("h_0", self.h_0, None, None)], 3: third, 4: fourth,
+                 5: lambda: [LabeledPolynomial("h_2", self.h_2, None, None)]}
+        return {r: build[r]() for r in rounds}
+
+    @staticmethod
+    def _eval(poly: torch.Tensor, point: int) -> int:
+        return _fr_mont_to_int(device.poly_evaluate(poly.contiguous(), _mont(point))) if poly.shape[0] else 0
+
+    def linear_combinations(self, alpha, eta_b, eta_c, beta, deltas, gamma, batch_combiners=None, label=None):
+        """AHPForR1CS::construct_linear_combinations (ahp/ahp.rs:172-389) and the verifier's query set for K circuits → (lcs, query_set):
+        lcs = [(label, [(coefficient, polynomial label or None for LCTerm::One)])] in the reference's BTreeMap order, query_set =
+        [(lc label, (point name, point))].  Each circuit's terms are scaled by the selector of its domain inside the max domain at α, β
+        and γ.  The coefficients are host integers; the evaluations they need (g_1(β), g_M(γ), x(β)) are device Horner passes."""
+        combs = self._combiners(batch_combiners)
+        label = label or self._labels()
+        cs = self.circuits
+        R, C, K = self.max_constraint_domain, self.max_variable_domain, self.max_non_zero_domain
+        lcs = {}
+        const = 0
+        for c, (cc, inst), sums in zip(cs, combs, self.third_sums):
+            term = sum(comb * (s[0] * s[1] - s[2]) for comb, s in zip(inst, sums)) % R_MOD
+            const = (const + cc * _selector(R, c.constraint_domain, alpha) % R_MOD * term) % R_MOD
+        lcs["rowcheck_zerocheck"] = [(const, None), ((-_vanish(R, alpha)) % R_MOD, "h_0")]
+        lcs["g_1"] = [(1, "g_1")]
+        g_1_at_beta = self._eval(self.g_1, beta)
+        lineval = [(1, "mask_poly")] if self.mask_poly is not None else []
+        batch_lineval_sum = 0
+        for i, (c, (cc, inst)) in enumerate(zip(cs, combs)):
+            sums4 = [s * a.domain.size % R_MOD for s, a in zip(self.fourth_sums[i], c.ariths)]
+            weight = (sums4[0] + sums4[1] * eta_b + sums4[2] * eta_c) % R_MOD
+            v_x_beta, sel = _vanish(c.input_domain, beta), _selector(C, c.variable_domain, beta)
+            for j, comb in enumerate(inst):
+                k = cc * comb % R_MOD * sel % R_MOD
+                lineval.append((k * weight % R_MOD * self._eval(self.x_polys[i][j], beta) % R_MOD, None))
+                lineval.append((k * weight % R_MOD * v_x_beta % R_MOD, label(i, "w", j)))
+            batch_lineval_sum += cc * sum(comb * (s[0] + eta_b * s[1] + eta_c * s[2]) for comb, s in zip(inst, self.third_sums[i]))
+        batch_lineval_sum = batch_lineval_sum % R_MOD * pow(C.size, -1, R_MOD) % R_MOD
+        lineval += [((-_vanish(C, beta)) % R_MOD, "h_1"), ((-beta * g_1_at_beta) % R_MOD, None), ((-batch_lineval_sum) % R_MOD, None)]
+        lcs["lineval_sumcheck"] = lineval
+        if len(deltas) != len(cs) or any(len(d) != 3 for d in deltas):
+            raise ValueError(f"one (δ_a, δ_b, δ_c) per circuit: {len(cs)} circuits")
+        points = {"rowcheck_zerocheck": ("alpha", alpha), "g_1": ("beta", beta), "lineval_sumcheck": ("beta", beta),
+                  "matrix_sumcheck": ("gamma", gamma)}
+        matrix = []
+        for i, c in enumerate(cs):
+            for m, (g, s, delta, a) in enumerate(zip(self.gs[i], self.fourth_sums[i], deltas[i], c.ariths)):
+                g_label = label(i, f"g_{'abc'[m]}", 0)
+                lcs[g_label] = [(1, g_label)]
+                points[g_label] = ("gamma", gamma)
+                selector = _selector(K, a.domain, gamma)
+                b_term = (gamma * self._eval(g, gamma) + s) % R_MOD
+                matrix.append((delta * selector % R_MOD, label(i, "a_poly", m)))
+                matrix.append(((-delta * selector % R_MOD * b_term) % R_MOD, label(i, "b_poly", m)))
+        matrix.append(((-_vanish(K, gamma)) % R_MOD, "h_2"))
+        lcs["matrix_sumcheck"] = matrix
+        order = sorted(lcs)
+        return [(k, lcs[k]) for k in order], [(k, points[k]) for k in order]
+
+
+def _short_label(_i, name, j=0):
+    """the one-circuit labels: w_{j}, g_{m}, a_poly_{m}, b_poly_{m}"""
+    if name in ("a_poly", "b_poly"):
+        return f"{name}_{'abc'[j]}"
+    return name if name.startswith("g_") else f"{name}_{j}"
+
+
+class Prover:
+    """BatchProver of one circuit, with the one-circuit interface: `assignments` is one CUDA tensor [num_variables, 4] per instance
+    (padded public variables, the first one One, then private); attributes are the circuit's own lists, labels are short (w_{j}, g_{m},
+    a_poly_{m}, b_poly_{m}).  The circuit id is never computed."""
+
+    def __init__(self, circuit: Circuit, assignments: list):
+        self._b = BatchProver([(circuit, assignments)])
+        self.circuit = circuit
+        self.batch = len(assignments)
+        self.z = self._b.z[0]
+
+    lagrange_coefficients = staticmethod(BatchProver.lagrange_coefficients)
+    _eval = staticmethod(BatchProver._eval)
+
+    def _combiners(self, circuit_combiner, instance_combiners):
+        return [(circuit_combiner, instance_combiners or [1] * self.batch)]
+
+    z_a = property(lambda self: self._b.z_a[0])
+    z_b = property(lambda self: self._b.z_b[0])
+    z_c = property(lambda self: self._b.z_c[0])
+    x_polys = property(lambda self: self._b.x_polys[0])
+    w_polys = property(lambda self: self._b.w_polys[0])
+    z_polys = property(lambda self: self._b.z_polys[0])
+    h_0 = property(lambda self: self._b.h_0)
+    g_1 = property(lambda self: self._b.g_1)
+    h_1 = property(lambda self: self._b.h_1)
+    h_2 = property(lambda self: self._b.h_2)
+    mask_poly = property(lambda self: self._b.mask_poly)
+    third_sums = property(lambda self: self._b.third_sums[0])
+    gs = property(lambda self: self._b.gs[0])
+    lhs = property(lambda self: self._b.lhs[0])
+    fourth_sums = property(lambda self: self._b.fourth_sums[0])
+    a_polys = property(lambda self: self._b.a_polys[0])
+    b_polys = property(lambda self: self._b.b_polys[0])
+
+    def first_round(self):
+        return self._b.first_round()[0]
+
+    def assignments(self):
+        return self._b.assignments()[0]
+
+    def second_round(self, circuit_combiner: int = 1, instance_combiners=None):
+        return self._b.second_round(self._combiners(circuit_combiner, instance_combiners))
+
+    def third_round(self, alpha: int, eta_b: int, eta_c: int, circuit_combiner: int = 1, instance_combiners=None):
+        return self._b.third_round(alpha, eta_b, eta_c, self._combiners(circuit_combiner, instance_combiners))
+
+    def set_mask_poly(self, h_1_mask_rand, g_1_mask_rand):
+        return self._b.set_mask_poly(h_1_mask_rand, g_1_mask_rand)
+
+    def fourth_round(self, alpha: int, beta: int):
+        return self._b.fourth_round(alpha, beta)[0]
+
+    def fifth_round(self, deltas):
+        return self._b.fifth_round([deltas])
+
+    def polynomials(self) -> dict:
+        """label → device polynomial, everything prove_batch hands to open_combinations (varuna.rs:509-517)"""
+        return self._b.polynomials(_short_label)
+
+    def oracles(self) -> dict:
+        return self._b.oracles()
+
+    def linear_combinations(self, alpha, eta_b, eta_c, beta, deltas, gamma, circuit_combiner: int = 1, instance_combiners=None):
+        """→ (lcs, query_set) exactly as oracle/varuna.py Prover.linear_combinations"""
+        return self._b.linear_combinations(alpha, eta_b, eta_c, beta, [deltas], gamma, self._combiners(circuit_combiner, instance_combiners),
+                                           _short_label)
 
 
 def test_circuit_csr(a: int, b: int, mul_depth: int, num_constraints: int, num_variables: int, dev):
