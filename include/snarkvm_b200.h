@@ -452,6 +452,31 @@ SNARKVM_API int snarkvm_b200_generate_bases_device(void* d_points, size_t npoint
  * powers_of_beta_g of a universal setup with a KNOWN trapdoor (kzg10/data_structures.rs UniversalParams) for tests and benches. */
 SNARKVM_API int snarkvm_b200_generator_mul_device(void* d_points, size_t stride, const void* d_scalars, size_t npoints, void* stream);
 
+/* BLS12-377 pairing (curves/src/templates/bls12/{bls12.rs, g2.rs}).
+ * A prepared G2 point (G2Prepared::from_affine) is SNARKVM_B200_G2_PREPARED_BYTES bytes: 69 coefficient triples of three Fq2
+ * (c0.c0 c0.c1 c1.c0 … c2.c1, Montgomery: 288 B per triple), then its infinity flag as a u32 and 28 zero bytes.  The point at
+ * infinity has no coefficients (zeros) and contributes nothing to a Miller loop.
+ * A GT value is the reference's Fp12 image: twelve Montgomery Fq in the order c0.c0.c0, c0.c0.c1, c0.c1.c0, … c1.c2.c1, 576 B. */
+#define SNARKVM_B200_G2_PREPARED_BYTES 19904
+#define SNARKVM_B200_GT_BYTES 576
+/* Prepares npoints G2 Affine images (x.c0 x.c1 y.c0 y.c1 infinity, stride ≥ 200, a multiple of 8, as snarkvm_b200_msm_g2_device
+ * takes them) into d_prepared (npoints × SNARKVM_B200_G2_PREPARED_BYTES, 16-byte aligned).  One launch, one synchronisation.  A
+ * coordinate whose image is not below q returns cudaErrorInvalidValue and *bad_point (HOST, may be NULL) receives the lowest such
+ * point's index (-1 otherwise); d_prepared is then unspecified. */
+SNARKVM_API int snarkvm_b200_g2_prepare_device(void* d_prepared, const void* d_points, size_t npoints, size_t stride, int64_t* bad_point,
+                                               void* stream);
+/* Products of pairings over a table of checks (PairingEngine::product_of_pairings per check).  Pair i is (G1 Affine image at
+ * d_g1 + i·g1_stride, prepared G2 number d_g2_index[i] of d_prepared); check c owns pairs [d_check_start[c], d_check_start[c + 1]),
+ * so d_check_start (device, nchecks + 1 u32) starts at 0, never decreases and ends at npairs.  Writes each check's GT value
+ * (d_gt: nchecks × 576 B, 16-byte aligned) and d_is_one[c] = 1 when it is one (device u32).  d_miller (may be NULL) receives each
+ * pair's Miller loop value (npairs × 576 B); the pairs of a check are multiplied and the final exponentiation runs once per check.
+ * A pair at infinity on either side contributes one; a check with no other pairs gives one.  One synchronisation per call.  A
+ * coordinate not below q, a G2 index ≥ nprepared or a malformed d_check_start returns cudaErrorInvalidValue, and *bad_check (HOST,
+ * may be NULL) receives the lowest check concerned (-1 otherwise); the outputs are then unspecified. */
+SNARKVM_API int snarkvm_b200_pairing_products_device(void* d_gt, uint32_t* d_is_one, void* d_miller, const void* d_g1, size_t g1_stride,
+                                                     const uint32_t* d_g2_index, size_t npairs, const void* d_prepared, size_t nprepared,
+                                                     const uint32_t* d_check_start, size_t nchecks, int64_t* bad_check, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

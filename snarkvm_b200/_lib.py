@@ -37,7 +37,7 @@ SYMBOLS = (
     "snarkvm_b200_ntt_batch_device", "snarkvm_b200_varuna_matrix_evals_batch_device", "snarkvm_b200_csr_serialize_batch_device",
     "snarkvm_b200_fr_lincomb_batch_device", "snarkvm_b200_matrix_evals_at_points_device",
     "snarkvm_b200_fr_lincomb_terms_device", "snarkvm_b200_sparse_matvec_batch_device", "snarkvm_b200_polymul_batch_device",
-    "snarkvm_b200_varuna_round4_evals_device",
+    "snarkvm_b200_varuna_round4_evals_device", "snarkvm_b200_g2_prepare_device", "snarkvm_b200_pairing_products_device",
 )
 
 
@@ -180,6 +180,8 @@ def lib():
     L.snarkvm_b200_sparse_matvec_batch_device.argtypes = [ctypes.POINTER(SpmvSegment), sz, ctypes.POINTER(ctypes.c_int64), vp]
     L.snarkvm_b200_polymul_batch_device.argtypes = [ctypes.POINTER(PolymulJob), sz, vp]
     L.snarkvm_b200_varuna_round4_evals_device.argtypes = [ctypes.POINTER(Round4Segment), sz, vp, vp, vp]
+    L.snarkvm_b200_g2_prepare_device.argtypes = [vp, vp, sz, sz, ctypes.POINTER(ctypes.c_int64), vp]
+    L.snarkvm_b200_pairing_products_device.argtypes = [vp, vp, vp, vp, sz, vp, sz, vp, sz, vp, sz, ctypes.POINTER(ctypes.c_int64), vp]
     L.snarkvm_b200_msm_batch_device.argtypes = [vp, vp, sz, vp, vp, sz, vp]
     L.snarkvm_b200_msm_window_sums_plan_device.argtypes = [vp, vp, sz, vp, sz, vp, sz, vp]
     L.snarkvm_b200_kzg_commit_batch_hiding_device.argtypes = [vp, vp, sz, vp, vp, vp, vp, vp, sz, vp]

@@ -25,6 +25,7 @@
 #include "host_ec.hpp"
 #include "msm.cuh"
 #include "ntt.cuh"
+#include "pairing.cuh"
 #include "poly.cuh"
 
 namespace b200 { void host_stream_copy(void* dst, const void* src, size_t n); }      // hostcopy.cpp: memcpy with non-temporal stores
@@ -1219,6 +1220,16 @@ int snarkvm_b200_fr_to_mont_device(void* d_out, const void* d_in, size_t n, void
 int snarkvm_b200_srs_decode_device(void* d_out, size_t stride, const void* d_in96, size_t npoints, uint32_t* d_invalid, void* stream) {
     if (!d_out || !d_in96 || !d_invalid) return (int)cudaErrorInvalidValue;
     return srs_decode_device(d_out, stride, d_in96, npoints, d_invalid, (cudaStream_t)stream);
+}
+
+int snarkvm_b200_g2_prepare_device(void* d_prepared, const void* d_points, size_t npoints, size_t stride, int64_t* bad_point, void* stream) {
+    return g2_prepare_device(d_prepared, d_points, npoints, stride, bad_point, (cudaStream_t)stream);
+}
+int snarkvm_b200_pairing_products_device(void* d_gt, uint32_t* d_is_one, void* d_miller, const void* d_g1, size_t g1_stride,
+                                         const uint32_t* d_g2_index, size_t npairs, const void* d_prepared, size_t nprepared,
+                                         const uint32_t* d_check_start, size_t nchecks, int64_t* bad_check, void* stream) {
+    return pairing_products_device(d_gt, d_is_one, d_miller, d_g1, g1_stride, d_g2_index, npairs, d_prepared, nprepared, d_check_start,
+                                   nchecks, bad_check, (cudaStream_t)stream);
 }
 
 int snarkvm_b200_register_bases(const void* host_points, size_t npoints, size_t stride) {

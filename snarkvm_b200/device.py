@@ -114,6 +114,57 @@ def generate_bases_g2(npoints: int, seed: int, device="cuda", stride: int = G2_A
     return t
 
 
+G2_PREPARED_BYTES = 19904    # 69 coefficient triples of three Fq2, infinity flag (u32), padding
+GT_BYTES = 576               # Fp12: twelve Montgomery Fq
+
+
+def g2_prepare(points: torch.Tensor, stride: int = G2_AFFINE_STRIDE) -> torch.Tensor:
+    """G2Prepared::from_affine of every Affine<G2> image in HBM → prepared points [n, G2_PREPARED_BYTES] (uint8, HBM).  A
+    coordinate image ≥ q raises CudaError naming the lowest such point (.point)."""
+    n = _nbytes(points) // stride
+    out = torch.empty((n, G2_PREPARED_BYTES), dtype=torch.uint8, device=points.device)
+    bad = ctypes.c_int64(-1)
+    with torch.cuda.device(points.device):
+        code = _lib.lib().snarkvm_b200_g2_prepare_device(out.data_ptr(), _check(points, "points") if n else None, n, stride,
+                                                         ctypes.byref(bad), _stream())
+    if code != 0:
+        err = _lib.CudaError(code, f"G2 point {bad.value}" if bad.value >= 0 else "see cudaError_t")
+        err.point = bad.value if bad.value >= 0 else None
+        raise err
+    return out
+
+
+def pairing_products(g1: torch.Tensor, g2_index: torch.Tensor, prepared: torch.Tensor, check_start: torch.Tensor,
+                     g1_stride: int = AFFINE_STRIDE, miller: bool = False):
+    """PairingEngine::product_of_pairings for every check in one call.  Pair i is (G1 Affine image g1[i], prepared point
+    prepared[g2_index[i]]); check c owns pairs check_start[c] .. check_start[c + 1] − 1 (check_start: int32, nchecks + 1 entries,
+    from 0 to the number of pairs).  → (GT values [nchecks, GT_BYTES] uint8 in HBM, is_one: bool tensor [nchecks] in HBM), and with
+    `miller` the pairs' Miller values [npairs, GT_BYTES] as a third item.  A coordinate image ≥ q, a G2 index out of range or a
+    malformed check_start raises CudaError naming the lowest check concerned (.check)."""
+    dev = check_start.device
+    nchecks = check_start.numel() - 1
+    if nchecks < 0 or check_start.dtype != torch.int32:
+        raise ValueError("check_start: int32, one entry more than there are checks")
+    npairs = _nbytes(g1) // g1_stride
+    if g2_index.numel() != npairs or (npairs and g2_index.dtype != torch.int32):
+        raise ValueError("one int32 G2 index per G1 point")
+    gt = torch.empty((max(nchecks, 0), GT_BYTES), dtype=torch.uint8, device=dev)
+    is_one = torch.zeros(max(nchecks, 0), dtype=torch.int32, device=dev)
+    mv = torch.empty((npairs, GT_BYTES), dtype=torch.uint8, device=dev) if miller else None
+    bad = ctypes.c_int64(-1)
+    with torch.cuda.device(dev):
+        code = _lib.lib().snarkvm_b200_pairing_products_device(
+            gt.data_ptr(), is_one.data_ptr(), mv.data_ptr() if miller and npairs else None,
+            _check(g1, "g1") if npairs else None, g1_stride, _check(g2_index, "g2_index") if npairs else None, npairs,
+            _check(prepared, "prepared") if prepared.numel() else None, _nbytes(prepared) // G2_PREPARED_BYTES,
+            _check(check_start, "check_start"), nchecks, ctypes.byref(bad), _stream())
+    if code != 0:
+        err = _lib.CudaError(code, f"check {bad.value}" if bad.value >= 0 else "see cudaError_t")
+        err.check = bad.value if bad.value >= 0 else None
+        raise err
+    return (gt, is_one.bool(), mv) if miller else (gt, is_one.bool())
+
+
 def msm_window_sums(bases: torch.Tensor, scalars: torch.Tensor, stride: int = AFFINE_STRIDE, plan_npoints: int | None = None,
                     flags: torch.Tensor | None = None, out: torch.Tensor | None = None) -> torch.Tensor:
     """Per-window XYZZ sums [nwin, 24] (int64 view of 192-byte points), left in HBM.  `plan_npoints` (≥ the number of

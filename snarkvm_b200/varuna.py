@@ -475,13 +475,74 @@ def prove_vk(pk: CircuitProvingKey, challenges, opening_challenges) -> Certifica
 
 @dataclass
 class VerifyingKeyCheck:
-    """verify_vk up to its pairing.  `matches`: the circuit's info and id equal the verifying key's (the reference stops with
+    """verify_vk's result.  `matches`: the circuit's info and id equal the verifying key's (the reference stops with
     CircuitNotFound otherwise; the other fields are still computed here).  The certificate is valid iff `matches` and
-    e(lhs, H) = e(w, β·H)."""
+    e(lhs, H)·e(−w, β·H) = 1.  `valid` is that verdict when verify_vk ran with a UniversalVerifier, and None without one."""
     matches: bool
     evaluation: int
     lhs: np.ndarray
     w: np.ndarray
+    valid: bool | None = None
+
+
+Q_MOD = 258664426012969094010652733694893533536393512754914660539884262666720468348340822774968888139573360124440321458177  # fq.rs
+_FQ_R = (1 << 384) % Q_MOD
+# G2_GENERATOR_{X,Y}_{C0,C1} of curves/src/bls12_377/g2.rs, out of Montgomery form
+G2_GENERATOR = (
+    (170590608266080109581922461902299092015242589883741236963254737235977648828052995125541529645051927918098146183295,
+     83407003718128594709087171351153471074446327721872642659202721143408712182996929763094113874399921859453255070254),
+    (1843833842842620867708835993770650838640642469700861403869757682057607397502738488921663703124647238454792872005,
+     33145532013610981697337930729788870077912093258611421158732879580766461459275194744385880708057348608045241477209),
+)
+
+
+def _g2_affine(p) -> np.ndarray:
+    """((x0, x1), (y0, y1)) of plain integers, or None → the 200-byte Affine<G2> image (Montgomery; Affine::zero() = (0, 1, true))"""
+    coords, inf = (((0, 0), (1, 0)), 1) if p is None else (p, 0)
+    out = np.zeros(200, dtype=np.uint8)
+    out[:192] = np.frombuffer(b"".join((v * _FQ_R % Q_MOD).to_bytes(48, "little") for c in coords for v in c), dtype=np.uint8)
+    out[192] = inf
+    return out
+
+
+class UniversalVerifier:
+    """The pairing half of the universal verifier (kzg10/data_structures.rs UniversalParams: h, prepared_h, prepared_beta_h; g is
+    the first power of β·G): g as a 104-byte Affine<G1> image, h (the G2 generator) and β·h as 200-byte Affine<G2> images, and
+    `prepared`, h and β·h prepared once on the device ([2, device.G2_PREPARED_BYTES], h first)."""
+
+    def __init__(self, beta_h: np.ndarray, device_="cuda"):
+        dev = torch.device(device_)
+        self.h = _g2_affine(G2_GENERATOR)
+        self.beta_h = np.ascontiguousarray(beta_h, dtype=np.uint8).reshape(200)
+        self.g = device.generator_mul(torch.from_numpy(np.array([[1, 0, 0, 0]], dtype=np.uint64).view(np.int64)).to(dev)).cpu().numpy()[0]
+        self.prepared = device.g2_prepare(torch.from_numpy(np.stack([self.h, self.beta_h])).to(dev))
+        self.device = self.prepared.device
+
+    @classmethod
+    def from_usrs(cls, blob: bytes, device_="cuda") -> "UniversalVerifier":
+        """β·H from the mainnet `beta-h.usrs` bytes: x.c0, x.c1, y.c0, y.c1 (48 B LE each), bit 6 of the last byte = infinity and
+        bit 7 = y's sign (utilities/src/serialize/flags.rs).  A coordinate ≥ q raises ValueError."""
+        if len(blob) != 192:
+            raise ValueError(f"a G2 point is 192 bytes, not {len(blob)}")
+        b = bytearray(blob)
+        infinity = bool(b[191] & 0x40)
+        b[191] &= 0x3F
+        v = [int.from_bytes(bytes(b[48 * i: 48 * i + 48]), "little") for i in range(4)]
+        if any(x >= Q_MOD for x in v):
+            raise ValueError("a coordinate of β·H is not below q")
+        return cls(_g2_affine(None if infinity else ((v[0], v[1]), (v[2], v[3]))), device_)
+
+    @classmethod
+    def synthetic(cls, beta: int, device_="cuda") -> "UniversalVerifier":
+        """the verifier of a setup with a known β (sonic_pc.synthetic_srs): β·H by the G2 MSM of one point"""
+        dev = torch.device(device_)
+        beta %= R_MOD
+        scalar = torch.from_numpy(np.array([[(beta >> (64 * i)) & (2**64 - 1) for i in range(4)]], dtype=np.uint64).view(np.int64)).to(dev)
+        proj = device.msm_g2(torch.from_numpy(_g2_affine(G2_GENERATOR)[None]).to(dev), scalar)       # normalised: (x, y, 1) or (0, 1, 0)
+        img = np.zeros(200, dtype=np.uint8)
+        img[:192] = proj[:24].view(np.uint8)
+        img[192] = 0 if proj[24:].any() else 1
+        return cls(img, device_)
 
 
 def _affine(projective: np.ndarray) -> np.ndarray:
@@ -493,7 +554,16 @@ def _affine(projective: np.ndarray) -> np.ndarray:
     return out
 
 
-def verify_vk_batch(circuits: list, vks: list, certificates: list, challenges: list, opening_challenges: list) -> list:
+def _affine_neg(projective: np.ndarray) -> np.ndarray:
+    """the Affine image of −P (y ↦ q − y on the Montgomery image; zero stays zero)"""
+    out = _affine(projective)
+    y = int.from_bytes(out[48:96].tobytes(), "little")
+    out[48:96] = np.frombuffer(((Q_MOD - y) % Q_MOD).to_bytes(48, "little"), dtype=np.uint8)
+    return out
+
+
+def verify_vk_batch(circuits: list, vks: list, certificates: list, challenges: list, opening_challenges: list,
+                    verifier: UniversalVerifier | None = None) -> list:
     """VarunaSNARK::verify_vk (varuna.rs:280-331) up to the pairing, for every (circuit, verifying key, certificate) → [VerifyingKeyCheck]
     in input order.  The circuits are already indexed (Circuit).  The evaluation v comes from evaluate_index_polynomials;
     check_combinations → batch_check → accumulate_elems for one point with randomizer one (sonic_pc/mod.rs:344-411, 477-544, 582-635)
@@ -521,12 +591,25 @@ def verify_vk_batch(circuits: list, vks: list, certificates: list, challenges: l
     bases_d = torch.from_numpy(np.stack(bases)).to(dev)
     scalars_d = torch.from_numpy(np.stack(scalars).view(np.int64)).to(dev)
     lhs = device.sonic_commit_batch([bases_d[14 * k: 14 * k + 14] for k in range(K)], [scalars_d[14 * k: 14 * k + 14] for k in range(K)])
-    return [VerifyingKeyCheck(m, v, lhs[k].copy(), cert.w) for k, (m, v, cert) in enumerate(zip(matches, evaluations, certificates))]
+    checks = [VerifyingKeyCheck(m, v, lhs[k].copy(), cert.w) for k, (m, v, cert) in enumerate(zip(matches, evaluations, certificates))]
+    if verifier is None:
+        return checks
+    if verifier.device != dev:
+        raise ValueError("the verifier's prepared points live on another device than the circuits")
+    # check_elems (sonic_pc/mod.rs:637-677): e(lhs, H)·e(−W, β·H) = 1, every circuit one check of one pairing-products call
+    g1 = torch.from_numpy(np.stack([a for c in checks for a in (_affine(c.lhs), _affine_neg(c.w))])).to(dev)
+    g2_index = torch.tensor([0, 1] * K, dtype=torch.int32, device=dev)
+    check_start = torch.arange(0, 2 * K + 1, 2, dtype=torch.int32, device=dev)
+    _gt, is_one = device.pairing_products(g1, g2_index, verifier.prepared, check_start)
+    for c, one in zip(checks, is_one.cpu().tolist()):
+        c.valid = bool(c.matches and one)
+    return checks
 
 
-def verify_vk(circuit: Circuit, vk: CircuitVerifyingKey, certificate: Certificate, challenges, opening_challenge: int) -> VerifyingKeyCheck:
-    """VarunaSNARK::verify_vk (varuna.rs:280-331) up to the pairing: verify_vk_batch of one circuit"""
-    return verify_vk_batch([circuit], [vk], [certificate], [challenges], [opening_challenge])[0]
+def verify_vk(circuit: Circuit, vk: CircuitVerifyingKey, certificate: Certificate, challenges, opening_challenge: int,
+              verifier: UniversalVerifier | None = None) -> VerifyingKeyCheck:
+    """VarunaSNARK::verify_vk (varuna.rs:280-331): verify_vk_batch of one circuit (up to the pairing without a verifier)"""
+    return verify_vk_batch([circuit], [vk], [certificate], [challenges], [opening_challenge], verifier)[0]
 
 
 def witness_label(circuit_id: bytes, poly: str, i: int) -> str:
