@@ -404,12 +404,14 @@ SNARKVM_API int snarkvm_b200_selftest_host_copy(size_t max_bytes, uint64_t seed,
  *
  * snarkvm_b200_test_field_op_device: d_out[i] = op(d_a[i], d_b[i]) for i < n, all device pointers.  ctx picks the translation unit
  * the test kernel is compiled in: MSM = msm.cu, where MUL / SQR call the out-of-line mul_call / sqr_call that msm.cu's kernels call
- * as well; NTT = ntt.cu, where they are inlined into the test kernel (a copy of its own, not the one in the NTT butterflies).
+ * as well; NTT = ntt.cu, where they are inlined into the test kernel (a copy of its own, not the one in the NTT butterflies);
+ * PAIRING = pairing.cu, which also calls out-of-line mul_call / sqr_call, but its own copies (the library is not built with
+ * relocatable device code, so each translation unit compiles its own): the ones every Fq6 / Fq12 product of the pairing calls.
  * Fr and Fq take ops ADD … FROM_MONT and the warp-cooperative COOP_MUL / COOP_INVERSE (one warp per element; a COOP_MUL
  * whose lanes >= N do not return 0 is written as all-ones limbs); Fq2 takes ADD, SUB, NEG, DBL, MUL, SQR, INVERSE; TIMES5 is
  * Fq2::times5 on plain Fq elements (field = FQ).  TO_MONT / FROM_MONT take any value < p. */
 enum {
-    SNARKVM_B200_TEST_CTX_MSM = 0, SNARKVM_B200_TEST_CTX_NTT = 1,
+    SNARKVM_B200_TEST_CTX_MSM = 0, SNARKVM_B200_TEST_CTX_NTT = 1, SNARKVM_B200_TEST_CTX_PAIRING = 2,
     SNARKVM_B200_FIELD_FR = 0, SNARKVM_B200_FIELD_FQ = 1, SNARKVM_B200_FIELD_FQ2 = 2,
     SNARKVM_B200_GROUP_G1 = 0, SNARKVM_B200_GROUP_G2 = 1
 };
@@ -435,6 +437,31 @@ SNARKVM_API int snarkvm_b200_test_curve_op_device(int group, int op, void* d_out
 /* The host arithmetic that finishes every MSM (host_ec.hpp), on HOST buffers; needs no GPU.  field FQ: ADD, SUB, MUL, SQR, INVERSE;
  * field FQ2: ADD, SUB, MUL, SQR, INVERSE; XYZZ_ADD / XYZZ_DBL on XYZZ points over the field (G1 for FQ, G2 for FQ2). */
 SNARKVM_API int snarkvm_b200_test_field_op_host(int field, int op, void* out, const void* a, const void* b, size_t n);
+/* The extension tower and the G2 line steps of the pairing (tower.cuh, pairing.cu), element-wise and compiled in pairing.cu, where
+ * the pairing kernels call them: d_out[i] = op(d_a[i], d_b[i], d_c[i]) for i < n, all device pointers.  An Fq6 is c0 c1 c2 of Fq2
+ * (72 words), an Fq12 is c0 c1 of Fq6 (144 words, the GT image order); a line-step state is X Y Z of Fq2 (72 words).
+ *   FQ6_MUL a·b, FQ6_SQR a², FQ6_MUL_BY_NONRESIDUE a·v, FQ6_INVERSE a⁻¹ (zero ↦ zero), FQ6_FROBENIUS a^(q^k), k < 6: Fq6 in and out.
+ *   FQ6_MUL_BY_01: a·(b0 + b1·v), d_b = b0 b1 (48 words).
+ *   FQ12_MUL a·b, FQ12_SQR a², FQ12_INVERSE a⁻¹ (zero ↦ zero), FQ12_CONJUGATE, FQ12_FROBENIUS a^(q^k), k < 12: Fq12 in and out.
+ *   FQ12_CYCLOTOMIC_SQUARE (Granger–Scott) and FQ12_EXP_BY_X (a^X, X = 0x8508c00000000001): a must lie in the cyclotomic subgroup.
+ *   FQ12_FINAL_EXPONENTIATION: the pairing's final exponentiation, zero ↦ zero.  FQ12_IS_ONE: one word per element, 1 when a is
+ *   the Montgomery image of one, else 0.
+ *   FQ12_MUL_BY_034: a·((c0, 0, 0) + (c3, c4, 0)·w), d_b = c0 c3 c4 (72 words).  FQ12_ELL: the Miller loop's line evaluation
+ *   a·mul_by_034(c0·p.y, c1·p.x, c2), d_b = a prepared coefficient triple c0 c1 c2 (72 words), d_c = the G1 point p.x p.y (24 words).
+ *   G2_DOUBLING_STEP (d_a = X Y Z) and G2_ADDITION_STEP (d_a = X Y Z, d_b = the affine Q: x y, 48 words) of G2 preparation:
+ *   the new X Y Z, then the coefficient triple (144 words).  The steps are polynomial formulas: any Fq2 operands are valid.
+ * k is the Frobenius power and must be 0 for every other op; an unknown op or a k out of range returns cudaErrorInvalidValue. */
+enum {
+    SNARKVM_B200_OP_FQ6_MUL = 48, SNARKVM_B200_OP_FQ6_SQR = 49, SNARKVM_B200_OP_FQ6_MUL_BY_01 = 50,
+    SNARKVM_B200_OP_FQ6_MUL_BY_NONRESIDUE = 51, SNARKVM_B200_OP_FQ6_INVERSE = 52, SNARKVM_B200_OP_FQ6_FROBENIUS = 53,
+    SNARKVM_B200_OP_FQ12_MUL = 54, SNARKVM_B200_OP_FQ12_SQR = 55, SNARKVM_B200_OP_FQ12_MUL_BY_034 = 56,
+    SNARKVM_B200_OP_FQ12_CYCLOTOMIC_SQUARE = 57, SNARKVM_B200_OP_FQ12_INVERSE = 58, SNARKVM_B200_OP_FQ12_CONJUGATE = 59,
+    SNARKVM_B200_OP_FQ12_FROBENIUS = 60, SNARKVM_B200_OP_FQ12_IS_ONE = 61, SNARKVM_B200_OP_FQ12_EXP_BY_X = 62,
+    SNARKVM_B200_OP_FQ12_FINAL_EXPONENTIATION = 63, SNARKVM_B200_OP_FQ12_ELL = 64,
+    SNARKVM_B200_OP_G2_DOUBLING_STEP = 65, SNARKVM_B200_OP_G2_ADDITION_STEP = 66
+};
+SNARKVM_API int snarkvm_b200_test_tower_op_device(int op, int k, void* d_out, const void* d_a, const void* d_b, const void* d_c, size_t n,
+                                                  void* stream);
 
 /* Deterministic synthetic bases P_i = h(seed, i) * G written in the reference affine layout. */
 /* ---- G2 (points over Fq2) ----------------------------------------------------------------------------------------------

@@ -38,6 +38,7 @@ SYMBOLS = (
     "snarkvm_b200_fr_lincomb_batch_device", "snarkvm_b200_matrix_evals_at_points_device",
     "snarkvm_b200_fr_lincomb_terms_device", "snarkvm_b200_sparse_matvec_batch_device", "snarkvm_b200_polymul_batch_device",
     "snarkvm_b200_varuna_round4_evals_device", "snarkvm_b200_g2_prepare_device", "snarkvm_b200_pairing_products_device",
+    "snarkvm_b200_test_tower_op_device",
 )
 
 
@@ -195,6 +196,7 @@ def lib():
     L.snarkvm_b200_test_field_op_device.argtypes = [i32, i32, i32, vp, vp, vp, sz, vp]
     L.snarkvm_b200_test_curve_op_device.argtypes = [i32, i32, vp, vp, vp, vp, sz, vp]
     L.snarkvm_b200_test_field_op_host.argtypes = [i32, i32, vp, vp, vp, sz]
+    L.snarkvm_b200_test_tower_op_device.argtypes = [i32, i32, vp, vp, vp, vp, sz, vp]
     L.snarkvm_b200_msm_window_sums_host.argtypes = [vp, vp, sz, vp, sz, vp, sz, vp]
     for s in SYMBOLS[5:]:
         getattr(L, s).restype = i32

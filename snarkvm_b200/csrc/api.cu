@@ -1330,7 +1330,12 @@ int snarkvm_b200_selftest_coop(uint32_t nwarps, uint64_t seed, uint32_t* mismatc
 int snarkvm_b200_test_field_op_device(int ctx, int field, int op, void* d_out, const void* d_a, const void* d_b, size_t n, void* stream) {
     if (ctx == SNARKVM_B200_TEST_CTX_MSM) return test_field_op_msm(field, op, d_out, d_a, d_b, n, (cudaStream_t)stream);
     if (ctx == SNARKVM_B200_TEST_CTX_NTT) return test_field_op_ntt(field, op, d_out, d_a, d_b, n, (cudaStream_t)stream);
+    if (ctx == SNARKVM_B200_TEST_CTX_PAIRING) return test_field_op_pairing(field, op, d_out, d_a, d_b, n, (cudaStream_t)stream);
     return (int)cudaErrorInvalidValue;
+}
+int snarkvm_b200_test_tower_op_device(int op, int k, void* d_out, const void* d_a, const void* d_b, const void* d_c, size_t n,
+                                      void* stream) {
+    return test_tower_op_device(op, k, d_out, d_a, d_b, d_c, n, (cudaStream_t)stream);
 }
 int snarkvm_b200_test_curve_op_device(int group, int op, void* d_out, const void* d_a, const void* d_b, const uint32_t* d_k, size_t n,
                                       void* stream) {

@@ -113,6 +113,7 @@ int selftest_coop_device(uint32_t nwarps, uint64_t seed, uint32_t* d_mismatches,
 // element-wise arithmetic test kernels (testops.cuh instantiated in msm.cu and in ntt.cu; snarkvm_b200_test_*_device)
 int test_field_op_msm(int field, int op, void* d_out, const void* d_a, const void* d_b, size_t n, cudaStream_t stream);
 int test_field_op_ntt(int field, int op, void* d_out, const void* d_a, const void* d_b, size_t n, cudaStream_t stream);
+int test_field_op_pairing(int field, int op, void* d_out, const void* d_a, const void* d_b, size_t n, cudaStream_t stream);
 int test_curve_op_device(int group, int op, void* d_out, const void* d_a, const void* d_b, const uint32_t* d_k, size_t n, cudaStream_t stream);
 
 // out[i] = Σ_r in[r][i]  over `nranks` arrays of `count` XYZZ points (multi-GPU combine).

@@ -17,6 +17,7 @@
 #define FF_CALL_MUL 1
 #include "tower.cuh"
 #include "pairing.cuh"
+#include "../../include/snarkvm_b200.h"   // the test ops
 
 namespace b200 {
 
@@ -270,4 +271,97 @@ int pairing_products_device(void* d_gt, uint32_t* d_is_one, void* d_miller, cons
     return finish(rc, scratch, d_bad, bad_check, stream);
 }
 
+// ---- element-wise tests of the tower and the line steps (snarkvm_b200_test_tower_op_device) -------------------------------------
+// Compiled here so that they call the same doubling_step, addition_step, ell, exp_by_x and final_exponentiation, and the same
+// out-of-line Fq products, as the kernels above.  Operands and results: Montgomery words, one element per thread.
+namespace {
+
+FF_DEV Fq6 t6_load(const uint32_t* p) { Fq6 r; r.c0 = Fq2::load(p); r.c1 = Fq2::load(p + 24); r.c2 = Fq2::load(p + 48); return r; }
+FF_DEV void t6_store(uint32_t* p, const Fq6& x) { x.c0.store(p); x.c1.store(p + 24); x.c2.store(p + 48); }
+
+__global__ void __launch_bounds__(128) k_test_fq6_op(int op, int k, uint32_t* __restrict__ out, const uint32_t* __restrict__ a,
+                                                     const uint32_t* __restrict__ b, size_t n) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const Fq6 x = t6_load(a + i * Fq6::WORDS);
+    Fq6 r;
+    switch (op) {
+        case SNARKVM_B200_OP_FQ6_MUL: r = x * t6_load(b + i * Fq6::WORDS); break;
+        case SNARKVM_B200_OP_FQ6_SQR: r = x.sqr(); break;
+        case SNARKVM_B200_OP_FQ6_MUL_BY_01: r = x.mul_by_01(Fq2::load(b + i * 48), Fq2::load(b + i * 48 + 24)); break;
+        case SNARKVM_B200_OP_FQ6_MUL_BY_NONRESIDUE: r = x.mul_by_nonresidue(); break;
+        case SNARKVM_B200_OP_FQ6_INVERSE: r = x.inverse(); break;
+        default: r = x.frobenius_map(k); break;
+    }
+    t6_store(out + i * Fq6::WORDS, r);
+}
+
+__global__ void __launch_bounds__(128) k_test_fq12_op(int op, int k, uint32_t* __restrict__ out, const uint32_t* __restrict__ a,
+                                                      const uint32_t* __restrict__ b, const uint32_t* __restrict__ c, size_t n) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const Fq12 x = Fq12::load(a + i * Fq12::WORDS);
+    if (op == SNARKVM_B200_OP_FQ12_IS_ONE) { out[i] = x.is_one() ? 1u : 0u; return; }
+    Fq12 r;
+    switch (op) {
+        case SNARKVM_B200_OP_FQ12_MUL: r = fq12_mul(x, Fq12::load(b + i * Fq12::WORDS)); break;
+        case SNARKVM_B200_OP_FQ12_SQR: r = fq12_sqr(x); break;
+        case SNARKVM_B200_OP_FQ12_MUL_BY_034: {
+            const uint32_t* y = b + i * 72;
+            r = fq12_mul_by_034(x, Fq2::load(y), Fq2::load(y + 24), Fq2::load(y + 48));
+            break;
+        }
+        case SNARKVM_B200_OP_FQ12_CYCLOTOMIC_SQUARE: r = fq12_cyclotomic_square(x); break;
+        case SNARKVM_B200_OP_FQ12_INVERSE: r = fq12_inverse(x); break;
+        case SNARKVM_B200_OP_FQ12_CONJUGATE: r = x.conjugate(); break;
+        case SNARKVM_B200_OP_FQ12_FROBENIUS: r = fq12_frobenius_map(x, k); break;
+        case SNARKVM_B200_OP_FQ12_EXP_BY_X: r = exp_by_x(x); break;
+        case SNARKVM_B200_OP_FQ12_FINAL_EXPONENTIATION: r = final_exponentiation(x); break;
+        default: {                                                               // ELL
+            AffinePoint p;
+            p.x = Fq::load(c + i * 24); p.y = Fq::load(c + i * 24 + 12); p.inf = false;
+            r = ell(x, reinterpret_cast<const uint8_t*>(b + i * 72), p);
+        }
+    }
+    r.store(out + i * Fq12::WORDS);
+}
+
+__global__ void __launch_bounds__(128) k_test_line_step(int op, uint32_t* __restrict__ out, const uint32_t* __restrict__ a,
+                                                        const uint32_t* __restrict__ b, size_t n) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint32_t* s = a + i * 72;
+    G2Hom r{Fq2::load(s), Fq2::load(s + 24), Fq2::load(s + 48)};
+    uint32_t* o = out + i * 144;
+    if (op == SNARKVM_B200_OP_G2_DOUBLING_STEP) doubling_step(r, Fq::one().half(), reinterpret_cast<uint8_t*>(o + 72));
+    else addition_step(r, Fq2::load(b + i * 48), Fq2::load(b + i * 48 + 24), reinterpret_cast<uint8_t*>(o + 72));
+    r.x.store(o); r.y.store(o + 24); r.z.store(o + 48);
+}
+
+}  // namespace
+
+int test_tower_op_device(int op, int k, void* d_out, const void* d_a, const void* d_b, const void* d_c, size_t n, cudaStream_t stream) {
+    const bool frob6 = op == SNARKVM_B200_OP_FQ6_FROBENIUS, frob12 = op == SNARKVM_B200_OP_FQ12_FROBENIUS;
+    if (op < SNARKVM_B200_OP_FQ6_MUL || op > SNARKVM_B200_OP_G2_ADDITION_STEP) return (int)cudaErrorInvalidValue;
+    if (k < 0 || k >= (frob6 ? 6 : frob12 ? 12 : 1)) return (int)cudaErrorInvalidValue;
+    if (n == 0) return 0;
+    const bool needs_b = op == SNARKVM_B200_OP_FQ6_MUL || op == SNARKVM_B200_OP_FQ6_MUL_BY_01 || op == SNARKVM_B200_OP_FQ12_MUL ||
+                         op == SNARKVM_B200_OP_FQ12_MUL_BY_034 || op == SNARKVM_B200_OP_FQ12_ELL || op == SNARKVM_B200_OP_G2_ADDITION_STEP;
+    if (!d_out || !d_a || (needs_b && !d_b) || (op == SNARKVM_B200_OP_FQ12_ELL && !d_c) || n > ((size_t)1 << 26))
+        return (int)cudaErrorInvalidValue;
+    if (((uintptr_t)d_out | (uintptr_t)d_a | (uintptr_t)d_b | (uintptr_t)d_c) & 15) return (int)cudaErrorInvalidValue;  // 16-B loads
+    uint32_t* out = (uint32_t*)d_out;
+    const uint32_t *a = (const uint32_t*)d_a, *b = (const uint32_t*)d_b, *c = (const uint32_t*)d_c;
+    const unsigned blocks = (unsigned)((n + 127) / 128);
+    if (op <= SNARKVM_B200_OP_FQ6_FROBENIUS) k_test_fq6_op<<<blocks, 128, 0, stream>>>(op, k, out, a, b, n);
+    else if (op <= SNARKVM_B200_OP_FQ12_ELL) k_test_fq12_op<<<blocks, 128, 0, stream>>>(op, k, out, a, b, c, n);
+    else k_test_line_step<<<blocks, 128, 0, stream>>>(op, out, a, b, n);
+    count_launch();
+    return (int)cudaGetLastError();
+}
+
 }  // namespace b200
+
+// the field-arithmetic test kernels, compiled here with this translation unit's own mul_call / sqr_call
+#define FIELD_TEST_ENTRY test_field_op_pairing
+#include "testops.cuh"

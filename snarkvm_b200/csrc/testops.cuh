@@ -1,8 +1,9 @@
 // Element-wise test kernels for the field arithmetic of ff.cuh / ec.cuh (snarkvm_b200_test_field_op_device).
 //
-// The machine code of a Montgomery product depends on the translation unit it is compiled in: msm.cu defines FF_CALL_MUL,
-// so `a * b` and `a.sqr()` call the out-of-line mul_call / sqr_call there, while ntt.cu inlines them.  ptxas is free to
-// schedule the carry flag differently in each, so this header is included by both and each instance is tested on its own.
+// The machine code of a Montgomery product depends on the translation unit it is compiled in: msm.cu and pairing.cu define
+// FF_CALL_MUL, so `a * b` and `a.sqr()` call the out-of-line mul_call / sqr_call there (each its own copy: the library is not
+// built with relocatable device code), while ntt.cu inlines them.  ptxas is free to schedule the carry flag differently in each,
+// so this header is included by all three and each instance is tested on its own.
 // The includer names the entry point with FIELD_TEST_ENTRY before including it; every kernel has internal linkage.
 //
 // Operands come from the caller (tests/field_corpus.py): n elements of WORDS little-endian 32-bit limbs each, reduced
@@ -11,7 +12,8 @@
 //
 // The copy of the multiplier that runs here is the one inlined into these test kernels, not the one inside the NTT butterflies
 // or the MSM kernels: "ntt" tests ff.cuh as compiled without FF_CALL_MUL (inlined into a kernel of ntt.cu), "msm" as compiled
-// with it (the out-of-line mul_call / sqr_call of msm.cu, which msm.cu's kernels call too).
+// with it (the out-of-line mul_call / sqr_call of msm.cu, which msm.cu's kernels call too), "pairing" the out-of-line copies of
+// pairing.cu, which every Fq6 / Fq12 product of the pairing calls.
 #pragma once
 #include "ec.cuh"
 #include "msm.cuh"   // count_launch

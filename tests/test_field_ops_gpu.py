@@ -1,9 +1,10 @@
 """GPU: every field operation of ff.cuh / ec.cuh and every group operation of ec.cuh / quad.cuh, one element at a time on the operand
 corpus of tests/field_corpus.py, compared limb for limb with Python big integers (oracle/bls12_377.py, oracle/g2.py).
 
-The field operations run in test kernels compiled in two translation units: msm.cu (FF_CALL_MUL: products and squares call the
-out-of-line mul_call / sqr_call that the MSM kernels call) and ntt.cu (inlined into the test kernel — its own inline site, not
-the machine code of the NTT butterflies)."""
+The field operations run in test kernels compiled in three translation units: msm.cu (FF_CALL_MUL: products and squares call the
+out-of-line mul_call / sqr_call that the MSM kernels call), ntt.cu (inlined into the test kernel — its own inline site, not
+the machine code of the NTT butterflies) and pairing.cu (FF_CALL_MUL too, but its own out-of-line copies, which every product of
+the pairing calls)."""
 import numpy as np
 import pytest
 
@@ -11,7 +12,7 @@ import field_corpus as fc
 
 pytestmark = pytest.mark.gpu
 
-CTX = {"msm": 0, "ntt": 1}
+CTX = {"msm": 0, "ntt": 1, "pairing": 2}
 FIELD = {"fr": 0, "fq": 1, "fq2": 2}
 OP = {"add": 0, "sub": 1, "neg": 2, "dbl": 3, "half": 4, "mul": 5, "mul_inline": 6, "mul_call": 7, "mul_karatsuba": 8,
       "sqr": 9, "sqr_inline": 10, "sqr_call": 11, "inverse": 12, "to_mont": 13, "from_mont": 14, "times5": 15,
@@ -76,7 +77,7 @@ def _operands(name, op):
 
 @pytest.mark.parametrize("op", FIELD_OPS)
 @pytest.mark.parametrize("name", ["fr", "fq"])
-@pytest.mark.parametrize("ctx", ["msm", "ntt"])
+@pytest.mark.parametrize("ctx", list(CTX))
 def test_field_op_matches_big_integers(ctx, name, op):
     p, n = fc.FIELDS[name]
     A, B = _operands(name, op)
@@ -86,7 +87,7 @@ def test_field_op_matches_big_integers(ctx, name, op):
 
 
 @pytest.mark.parametrize("op", ["add", "sub", "neg", "dbl", "mul", "sqr", "inverse"])
-@pytest.mark.parametrize("ctx", ["msm", "ntt"])
+@pytest.mark.parametrize("ctx", list(CTX))
 def test_fq2_op_matches_big_integers(ctx, op):
     from oracle import g2 as og2
     q, R = fc.Q, fc.QR
@@ -116,7 +117,7 @@ def test_fq2_op_matches_big_integers(ctx, op):
         assert g == want, (ctx, op, a, b, g, want)
 
 
-@pytest.mark.parametrize("ctx", ["msm", "ntt"])
+@pytest.mark.parametrize("ctx", list(CTX))
 def test_times5_matches_big_integers(ctx):
     A = [a for a, _ in fc.field_pairs("fq")]
     got = fc.from_limbs(_run_field(ctx, "fq", "times5", fc.to_limbs(A, 12), fc.to_limbs(A, 12), 12))
@@ -172,12 +173,19 @@ def test_to_affine_matches_big_integers(group):
             assert (x[0] if w == 1 else tuple(x)) == want[0] and (y[0] if w == 1 else tuple(y)) == want[1]
 
 
-def test_entry_points_reject_unknown_ops():
+def test_entry_points_reject_unknown_contexts_and_ops():
+    """every context in CTX (msm, ntt, pairing) accepts a valid op; the values around them are no context; an op a field does not
+    take is rejected in every context"""
     import torch
     from snarkvm_b200 import _lib
     L = _lib.lib()
     buf = torch.zeros(96, dtype=torch.int32, device="cuda:0")
+    p = buf.data_ptr()
     s = torch.cuda.current_stream().cuda_stream
-    assert L.snarkvm_b200_test_field_op_device(2, 0, 0, buf.data_ptr(), buf.data_ptr(), buf.data_ptr(), 1, s) != 0
-    assert L.snarkvm_b200_test_field_op_device(0, 2, OP["half"], buf.data_ptr(), buf.data_ptr(), buf.data_ptr(), 1, s) != 0
-    assert L.snarkvm_b200_test_curve_op_device(1, OP["quad_add"], buf.data_ptr(), buf.data_ptr(), buf.data_ptr(), buf.data_ptr(), 1, s) != 0
+    for ctx in CTX.values():
+        assert L.snarkvm_b200_test_field_op_device(ctx, FIELD["fr"], OP["add"], p, p, p, 1, s) == 0, ctx
+        assert L.snarkvm_b200_test_field_op_device(ctx, FIELD["fq2"], OP["half"], p, p, p, 1, s) != 0, ctx
+    for ctx in (-1, len(CTX)):
+        assert L.snarkvm_b200_test_field_op_device(ctx, FIELD["fr"], OP["add"], p, p, p, 1, s) != 0, ctx
+    assert L.snarkvm_b200_test_curve_op_device(1, OP["quad_add"], p, p, p, p, 1, s) != 0
+    torch.cuda.synchronize()
