@@ -603,40 +603,108 @@ FF_DEV Fq ring_fq(const uint4* slot) {                       // slot = &ring[(st
     return r;
 }
 
-// Output descriptors, written once per level by k_pair_desc (one thread per output, warp-coherent binary search for the
-// bucket) so that the pair kernel never chases off_out → off_in → sorted in its instruction stream: it reads 8 bytes per
-// output, coalesced, two steps ahead.
-//   level 0:  p, q = the two sorted entries (point index | sign << 31); q = NONE when the output has a single input
-//   above:    p = index of the first input in dense_in; q = NONE / anything else
-static constexpr uint32_t PAIR_NONE = 0xffffffffu;
-template <bool GATHER>
-__global__ void __launch_bounds__(256) k_pair_desc(const uint32_t* __restrict__ sorted, const uint32_t* __restrict__ off_in,
-                                                   const uint32_t* __restrict__ off_out, uint32_t total_buckets, uint2* __restrict__ desc,
-                                                   const uint32_t* __restrict__ in_base_ptr /* dense inputs: *in_base_ptr = position of element 0, or null */) {
-    const uint32_t o = blockIdx.x * blockDim.x + threadIdx.x;
-    if (o >= __ldg(off_out + total_buckets)) return;
-    uint32_t lo = 0, hi = total_buckets;                  // off_out[lo] <= o < off_out[hi]
-    while (hi - lo > 1) { uint32_t mid = (lo + hi) >> 1; if (__ldg(off_out + mid) <= o) lo = mid; else hi = mid; }
-    const uint32_t i = o - __ldg(off_out + lo), base_in = __ldg(off_in + lo), cnt = __ldg(off_in + lo + 1) - base_in;
-    const uint32_t idx = base_in + 2u * i;
-    const bool has2 = 2u * i + 1u < cnt;
-    uint2 d;
-    if (GATHER) { d.x = __ldg(sorted + idx); d.y = has2 ? __ldg(sorted + idx + 1) : PAIR_NONE; }
-    else { d.x = idx - (in_base_ptr ? __ldg(in_base_ptr) : 0u); d.y = has2 ? 0u : PAIR_NONE; }
-    desc[o] = d;
+// Bucket search for a warp of consecutive indices.  `off` is an exclusive scan over nb buckets (off[nb] = total) and every
+// lane holds an index x < off[nb], nondecreasing across the lanes; the lane's bucket is the largest b with off[b] <= x.
+// warp_bucket_first: one binary search for a warp-uniform x (every lane walks the same path, so each step is one broadcast
+// load).  warp_bucket_walk: from a warp-uniform bucket b with off[b] <= x on every lane, lane l loads off[b + 1 + l] and
+// counts the boundaries at or below its x with a five-step shuffle search over the warp — one load per 32 buckets, so buckets
+// smaller than a warp and buckets of millions of entries cost the same.  Lanes still past the 32 loaded boundaries after two
+// rounds (long runs of empty buckets) finish with their own binary search.
+FF_DEV uint32_t warp_bucket_first(const uint32_t* __restrict__ off, uint32_t nb, uint32_t x) {
+    uint32_t lo = 0, hi = nb;                             // off[lo] <= x < off[hi]
+    while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (__ldg(off + mid) <= x) lo = mid; else hi = mid; }
+    return lo;
+}
+FF_DEV uint32_t warp_bucket_walk(const uint32_t* __restrict__ off, uint32_t nb, uint32_t b, uint32_t x) {
+    const int lane = threadIdx.x & 31;
+    uint32_t res = b;
+    bool done = false;
+    for (int round = 0;; round++) {
+        const uint32_t k = b + 1u + (uint32_t)lane;
+        const uint32_t e = k <= nb ? __ldg(off + k) : 0xffffffffu;
+        uint32_t c = 0;                                   // boundaries off[b + 1 … b + c] <= x  (c ≤ 31 here)
+#pragma unroll
+        for (uint32_t s = 16; s >= 1; s >>= 1)
+            if (__shfl_sync(0xffffffffu, e, (int)(c + s - 1u)) <= x) c += s;
+        const uint32_t e31 = __shfl_sync(0xffffffffu, e, 31);
+        if (!done && e31 > x) { res = b + c; done = true; }
+        if (__all_sync(0xffffffffu, done)) return res;
+        b += 32u;                                         // off[b] = e31 <= x on every lane not done
+        if (round == 1) break;
+    }
+    if (!done) { uint32_t lo = b, hi = nb; while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (__ldg(off + mid) <= x) lo = mid; else hi = mid; } res = lo; }
+    return res;
 }
 
-struct PairDesc {            // one lane's output of one step
-    uint32_t p, q;           // as written by k_pair_desc — possibly still in flight: only touch them when the step is issued / computed
-    bool valid;              // the output exists (known from the indices alone, never from loaded data)
-    FF_DEV bool has2() const { return valid && q != PAIR_NONE; }
+// Pair descriptors, written once per level by k_pair_desc so that the pair kernel never chases off_out → off_in → sorted in
+// its instruction stream: it reads 8 bytes per pair, coalesced, two steps ahead.  Only real pairs (both inputs present) get a
+// descriptor and a lane step: pair j of the level is the i-th pair of its bucket b, i = j − pair_off[b] (pair_off = scan of
+// ⌊cnt/2⌋), its inputs are off_in[b] + 2i and the one after, and it writes output off_out[b] + i (off_out = scan of ⌈cnt/2⌉,
+// so the output layout is that of all outputs, the pairs of a bucket first).
+//   level 0, gather:  desc = the two sorted entries (point index | sign << 31); out_pos[j] = the output position
+//   dense inputs:     desc = (index of the first input in dense_in, output position)
+// The single input of a bucket with an odd count is not a step: the same kernel copies it to the bucket's last output.
+static constexpr int DESC_CHUNKS = 8;                    // 32-pair chunks per warp: one binary search per 256 pairs
+template <bool GATHER>
+__global__ void __launch_bounds__(256) k_pair_desc(const uint32_t* __restrict__ sorted, const uint32_t* __restrict__ off_in,
+                                                   const uint32_t* __restrict__ off_out, const uint32_t* __restrict__ pair_off,
+                                                   uint32_t total_buckets, uint2* __restrict__ desc, uint32_t* __restrict__ out_pos,
+                                                   const uint32_t* __restrict__ in_base_ptr /* dense inputs: *in_base_ptr = position of element 0, or null */,
+                                                   const uint32_t* __restrict__ records, uint32_t in_words, uint32_t* __restrict__ dense_out) {
+    const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+    const uint32_t in_base = (!GATHER && in_base_ptr) ? __ldg(in_base_ptr) : 0u;
+    // ---- single inputs: one thread per bucket ----
+    if (t < total_buckets) {
+        const uint32_t end = __ldg(off_in + t + 1);
+        if ((end - __ldg(off_in + t)) & 1u) {
+            const uint32_t idx = end - 1u;
+            DensePoint P;
+            if (GATHER) {
+                const uint32_t s = __ldg(sorted + idx);
+                P = load_dense(records + (size_t)(s & 0x7fffffffu) * BASE_WORDS);
+                if ((s >> 31) && !P.inf) P.y = P.y.neg();
+            } else {
+                P = load_dense(records + (size_t)(idx - in_base) * in_words);
+            }
+            store_dense(dense_out + (size_t)(__ldg(off_out + t + 1) - 1u) * DENSE_WORDS, P);
+        }
+    }
+    // ---- pairs: 32 · DESC_CHUNKS consecutive ones per warp ----
+    const uint32_t total = __ldg(pair_off + total_buckets);
+    const uint32_t lane = threadIdx.x & 31u;
+    const uint64_t j0_64 = (uint64_t)(t >> 5) * (32u * DESC_CHUNKS);
+    if (j0_64 >= total) return;                           // warp-uniform
+    uint32_t j0 = (uint32_t)j0_64;
+    uint32_t b = warp_bucket_first(pair_off, total_buckets, j0);
+    for (int c = 0; c < DESC_CHUNKS && j0 < total; c++, j0 += 32u) {
+        const uint32_t j = j0 + lane < total ? j0 + lane : total - 1u;
+        const uint32_t bj = warp_bucket_walk(pair_off, total_buckets, b, j);
+        b = __shfl_sync(0xffffffffu, bj, 31);             // the next chunk starts at or after the last lane's bucket
+        if (j0 + lane < total) {
+            const uint32_t i = j - __ldg(pair_off + bj);
+            const uint32_t idx = __ldg(off_in + bj) + 2u * i, o = __ldg(off_out + bj) + i;
+            uint2 d;
+            if (GATHER) { d.x = __ldg(sorted + idx); d.y = __ldg(sorted + idx + 1); out_pos[j] = o; }
+            else { d.x = idx - in_base; d.y = o; }
+            desc[j] = d;
+        }
+    }
+}
+
+struct PairDesc {            // one lane's pair of one step
+    uint32_t p, q, o;        // inputs and output position as written by k_pair_desc — possibly still in flight: only touch them
+                             // when the step is issued / computed (dense inputs: the second input is p + 1)
+    bool valid;              // the pair exists (known from the indices alone, never from loaded data)
 };
-// descriptor of step j for this lane (dlane = desc + W0 + lane); steps outside [0, nv) do not exist
-FF_DEV PairDesc pair_load_desc(int64_t j, uint32_t nv, const uint2* __restrict__ dlane) {
-    PairDesc d; d.p = 0; d.q = PAIR_NONE; d.valid = false;
+// descriptor of step j for this lane (dlane = desc + W0 + lane, olane = out_pos + W0 + lane); steps outside [0, nv) do not
+// exist.  POS: load the output position too (backward pass).
+template <bool GATHER, bool POS>
+FF_DEV PairDesc pair_load_desc(int64_t j, uint32_t nv, const uint2* __restrict__ dlane, const uint32_t* __restrict__ olane) {
+    PairDesc d; d.p = 0; d.q = 0; d.o = 0; d.valid = false;
     if (j < 0 || j >= (int64_t)nv) return d;
     const uint2 v = __ldg(dlane + 32 * j);
     d.p = v.x; d.q = v.y; d.valid = true;
+    if (POS) d.o = GATHER ? __ldg(olane + 32 * j) : v.y;
     return d;
 }
 // in_words: stride of the dense inputs — the call's record stride at level 0 (BASE_WORDS or DENSE_WORDS, see
@@ -655,11 +723,9 @@ FF_DEV void pair_issue(const PairDesc& d, uint4* ring, int st, int lane, const u
         const uint32_t* p = pair_src<GATHER>(d, 0, records, in_words);
 #pragma unroll
         for (int k = 0; k < (FULL ? 6 : 3); k++) cp_async16(dst + (uint32_t)k * 512u, p + 4 * k);
-        if (d.q != PAIR_NONE) {
-            const uint32_t* q = pair_src<GATHER>(d, 1, records, in_words);
+        const uint32_t* q = pair_src<GATHER>(d, 1, records, in_words);
 #pragma unroll
-            for (int k = 0; k < (FULL ? 6 : 3); k++) cp_async16(dst + (uint32_t)((FULL ? 6 : 3) + k) * 512u, q + 4 * k);
-        }
+        for (int k = 0; k < (FULL ? 6 : 3); k++) cp_async16(dst + (uint32_t)((FULL ? 6 : 3) + k) * 512u, q + 4 * k);
     }
     cp_async_commit();
 }
@@ -679,7 +745,8 @@ FF_DEV int pair_classify_global(const PairDesc& d, const uint32_t* __restrict__ 
 // MINB = resident CTAs per SM the kernel is compiled for: 4 (128 registers) or 3 (168 registers, no spills).
 template <bool GATHER, int MINB>
 __global__ void __launch_bounds__(PAIR_THREADS, MINB) k_pair_level2(const uint32_t* __restrict__ records /* level 0: dense bases / table; above: dense_in */,
-                                                         uint32_t in_words, const uint2* __restrict__ desc, const uint32_t* __restrict__ total_ptr,
+                                                         uint32_t in_words, const uint2* __restrict__ desc, const uint32_t* __restrict__ out_pos,
+                                                         const uint32_t* __restrict__ total_ptr,
                                                          uint32_t T_bound, uint32_t* __restrict__ prefix, uint32_t* __restrict__ dense_out,
                                                          uint32_t* __restrict__ sm_slots) {
     (void)T_bound;
@@ -696,18 +763,17 @@ __global__ void __launch_bounds__(PAIR_THREADS, MINB) k_pair_level2(const uint32
     __syncthreads();
     const int inv_warp = (int)(sh_slot & 3u);
     const uint32_t total = __ldg(total_ptr);
-    // Steps per lane from the level's ACTUAL output count: the host sizes the grid (whole waves) from an upper bound, Σ cnt/2 +
-    // #buckets, which overshoots by up to half a bucket per bucket — 11 % at the last of five levels at 2^24 points, more with
-    // more buckets — and every lane walks all T steps, so T from the bound made the whole grid that much slower.  Any partition
-    // works for Montgomery's trick and the outputs do not depend on it.
+    // Steps per lane from the level's ACTUAL pair count: the host sizes the grid (whole waves) from an upper bound, Σ cnt/2,
+    // and every lane walks all T steps, so T from the bound would make the whole grid that much slower.  Any partition works
+    // for Montgomery's trick and the outputs do not depend on it.
     const uint64_t lanes = (uint64_t)gridDim.x * PAIR_THREADS;
     const uint32_t T = total > lanes ? (uint32_t)((total + lanes - 1) / lanes) : 1u;      // ≤ T_bound
-    const uint64_t w0_64 = ((uint64_t)blockIdx.x * (PAIR_THREADS / 32) + (uint32_t)warp) * 32ull * T + (uint32_t)lane;   // this lane's first output
+    const uint64_t w0_64 = ((uint64_t)blockIdx.x * (PAIR_THREADS / 32) + (uint32_t)warp) * 32ull * T + (uint32_t)lane;   // this lane's first pair
     uint32_t nv = 0;                                                                   // steps that exist for this lane
     if (w0_64 < total) { const uint64_t left = (total - w0_64 + 31) / 32; nv = left < T ? (uint32_t)left : T; }
     const uint2* dlane = desc + w0_64;
+    const uint32_t* poslane = GATHER ? out_pos + w0_64 : nullptr;
     uint32_t* plane = prefix + w0_64 * 12;                                             // prefix of step j at plane + j·32·12
-    uint32_t* olane = dense_out + w0_64 * DENSE_WORDS;
 
     // ---------------- forward: running product of the denominators ----------------
     // A forward step is ONE multiplication, far shorter than a gathered DRAM access: the x-only operands (96 B per lane) fit
@@ -716,19 +782,20 @@ __global__ void __launch_bounds__(PAIR_THREADS, MINB) k_pair_level2(const uint32
     Fq run = Fq::one();
     {
         constexpr int PF = 3;                                                   // steps of lead; PF + 1 stages of 6 chunks
-        PairDesc q0 = pair_load_desc(0, nv, dlane), q1 = pair_load_desc(1, nv, dlane), q2 = pair_load_desc(2, nv, dlane);
+        PairDesc q0 = pair_load_desc<GATHER, false>(0, nv, dlane, poslane), q1 = pair_load_desc<GATHER, false>(1, nv, dlane, poslane),
+                 q2 = pair_load_desc<GATHER, false>(2, nv, dlane, poslane);
         pair_issue<GATHER, false>(q0, ring, 0, lane, records, in_words, 6);
         pair_issue<GATHER, false>(q1, ring, 1, lane, records, in_words, 6);
         pair_issue<GATHER, false>(q2, ring, 2, lane, records, in_words, 6);
-        PairDesc ahead = pair_load_desc(PF, nv, dlane);
+        PairDesc ahead = pair_load_desc<GATHER, false>(PF, nv, dlane, poslane);
         for (uint32_t j = 0; j < T; j++) {
             pair_issue<GATHER, false>(ahead, ring, (int)((j + PF) & 3u), lane, records, in_words, 6);       // step j+3 (descriptor loaded a step ago)
             const PairDesc cur = q0;
             q0 = q1; q1 = q2; q2 = ahead;
-            ahead = pair_load_desc((int64_t)j + PF + 1, nv, dlane);                              // not touched until the next iteration
+            ahead = pair_load_desc<GATHER, false>((int64_t)j + PF + 1, nv, dlane, poslane);                             // not touched until the next iteration
             cp_async_wait_3();
             Fq d = Fq::one();
-            if (cur.has2()) {
+            if (cur.valid) {
                 const uint4* slot_p = ring + (size_t)(j & 3u) * (6 * 32) + lane;
                 Fq x1 = ring_fq(slot_p), x2 = ring_fq(slot_p + 3 * 32);
                 if (x1 == x2 || x1.is_zero() || x2.is_zero()) {
@@ -746,23 +813,22 @@ __global__ void __launch_bounds__(PAIR_THREADS, MINB) k_pair_level2(const uint32
     Fq inv = cta_shared_inverse_by(run, sh_inv, inv_warp);
     // ---------------- backward: one inverse per pair, then the affine addition ----------------
     {
-        PairDesc cur = pair_load_desc((int64_t)T - 1, nv, dlane);
+        PairDesc cur = pair_load_desc<GATHER, true>((int64_t)T - 1, nv, dlane, poslane);
         pair_issue<GATHER, true>(cur, ring, 0, lane, records, in_words, 12);
-        PairDesc nxt = pair_load_desc((int64_t)T - 2, nv, dlane);
+        PairDesc nxt = pair_load_desc<GATHER, true>((int64_t)T - 2, nv, dlane, poslane);
         for (uint32_t k = 0; k < T; k++) {
             const uint32_t j = T - 1 - k;
             pair_issue<GATHER, true>(nxt, ring, (int)((k + 1) & 1u), lane, records, in_words, 12);
-            PairDesc nn = pair_load_desc((int64_t)j - 2, nv, dlane);
+            PairDesc nn = pair_load_desc<GATHER, true>((int64_t)j - 2, nv, dlane, poslane);
             Fq pf = Fq::one();
             if (cur.valid && j != 0) pf = Fq::load(plane + (size_t)(j - 1) * (32 * 12));     // behind the first multiplication
             cp_async_wait_1();
             const uint4* slot_p = ring + (size_t)(k & 1u) * RING_STAGE_U4 + lane;
-            // classify (same decisions as the forward pass)
+            // classify (same decisions as the forward pass); a step that does not exist multiplies by one and stores nothing
             int kind = PAIR_COPY1;
             Fq d = Fq::one(), num = Fq::zero();
-            const bool has2 = cur.has2();
-            const bool negP = GATHER && (cur.p >> 31), negQ = GATHER && has2 && (cur.q >> 31);
-            if (has2) {
+            const bool negP = GATHER && (cur.p >> 31), negQ = GATHER && (cur.q >> 31);
+            if (cur.valid) {
                 Fq x1 = ring_fq(slot_p), x2 = ring_fq(slot_p + 6 * 32);
                 if (x1 == x2 || x1.is_zero() || x2.is_zero()) {
                     DensePoint P, Q;
@@ -790,7 +856,7 @@ __global__ void __launch_bounds__(PAIR_THREADS, MINB) k_pair_level2(const uint32
             Fq lambda = num * inv_d;
             Fq x3 = lambda.sqr();
             {
-                Fq x1 = ring_fq(slot_p), x2 = has2 ? ring_fq(slot_p + 6 * 32) : x1;
+                Fq x1 = ring_fq(slot_p), x2 = ring_fq(slot_p + 6 * 32);
                 x3 = x3 - x1 - x2;
                 Fq t = x1 - x3;
                 Fq y3 = lambda * t;
@@ -807,7 +873,7 @@ __global__ void __launch_bounds__(PAIR_THREADS, MINB) k_pair_level2(const uint32
                         R.inf = R.x.is_zero() && R.y.is_zero();
                         if (((kind == PAIR_COPY2) ? negQ : negP) && !R.inf) R.y = R.y.neg();
                     }
-                    store_dense(olane + (size_t)j * (32 * DENSE_WORDS), R);
+                    store_dense(dense_out + (size_t)cur.o * DENSE_WORDS, R);      // consecutive pairs: consecutive outputs, but for singles between
                 }
             }
             cur = nxt; nxt = nn;
@@ -816,10 +882,12 @@ __global__ void __launch_bounds__(PAIR_THREADS, MINB) k_pair_level2(const uint32
     }
 }
 
-__global__ void k_halve_counts(const uint32_t* __restrict__ off_in, uint32_t* __restrict__ cnt_out, uint32_t total_buckets) {
+// a pair level's counts per bucket: outputs ⌈cnt/2⌉ and pairs ⌊cnt/2⌋
+__global__ void k_halve_counts(const uint32_t* __restrict__ off_in, uint32_t* __restrict__ cnt_out, uint32_t* __restrict__ pairs_out,
+                               uint32_t total_buckets) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < total_buckets) cnt_out[i] = (off_in[i + 1] - off_in[i] + 1u) >> 1;
-    else if (i == total_buckets) cnt_out[i] = 0;
+    if (i < total_buckets) { const uint32_t c = off_in[i + 1] - off_in[i]; cnt_out[i] = (c + 1u) >> 1; pairs_out[i] = c >> 1; }
+    else if (i == total_buckets) { cnt_out[i] = 0; pairs_out[i] = 0; }
 }
 __global__ void k_items_from_offsets(const uint32_t* __restrict__ off, uint32_t* __restrict__ items, uint32_t total_buckets, uint32_t cap,
                                      uint32_t* __restrict__ hot, uint32_t hot_max, uint32_t keep) {
@@ -837,10 +905,12 @@ __global__ void __launch_bounds__(MSM_ACC_THREADS, MSM_ACC_MINBLOCKS) k_bucket_a
     uint32_t total_buckets, uint32_t cap, uint32_t* __restrict__ partial) {
     uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
     uint32_t total_items = item_start[total_buckets];
+    const uint32_t t0 = t & ~31u;                         // the warp's first item (blockDim is a multiple of 32)
+    if (t0 >= total_items) return;                        // warp-uniform: the search below needs the whole warp
+    const uint32_t wb = warp_bucket_walk(item_start, total_buckets, warp_bucket_first(item_start, total_buckets, t0),
+                                         t < total_items ? t : total_items - 1u);
     if (t >= total_items) return;
-    uint32_t lo = 0, hi = total_buckets;
-    while (hi - lo > 1) { uint32_t mid = (lo + hi) >> 1; if (item_start[mid] <= t) lo = mid; else hi = mid; }
-    uint32_t wb = lo, seg = t - item_start[wb];
+    uint32_t seg = t - item_start[wb];
     uint32_t b0 = bucket_start[wb], b1 = bucket_start[wb + 1];
     uint32_t s0 = b0 + seg * cap, s1 = s0 + cap < b1 ? s0 + cap : b1;
     XYZZ acc = XYZZ::infinity();
@@ -1638,7 +1708,7 @@ int msm_core(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, co
     // ---- one scratch block, carved up ----
     uint32_t *hist, *bucket_start, *cursors, *items, *item_start, *items2, *sorted, *partial, *partial2, *red_a, *red_b;
     uint32_t *off_a = nullptr, *off_b = nullptr, *dense_a = nullptr, *dense_b = nullptr, *prefix = nullptr, *dense_bases = nullptr, *sm_slots = nullptr;
-    uint32_t *dense0 = nullptr, *cnt_tmp = nullptr, *hot_dev = nullptr;
+    uint32_t *dense0 = nullptr, *cnt_tmp = nullptr, *hot_dev = nullptr, *pair_cnt = nullptr, *pair_off = nullptr, *out_pos = nullptr;
     uint2* desc = nullptr;
     uint8_t* cub_tmp;
     Arena ar;
@@ -1668,6 +1738,9 @@ int msm_core(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, co
             if (levels > 1) dense_b = records && dense_cap_b * DENSE_WORDS <= entries_g * (size_t)rec_words ? dense0 : a.take<uint32_t>(dense_cap_b * DENSE_WORDS);
             prefix = a.take<uint32_t>(dense_cap_a * 12);
             desc = a.take<uint2>(dense_cap_a);
+            if (!records) out_pos = a.take<uint32_t>(dense_cap_a);
+            pair_cnt = a.take<uint32_t>((size_t)TBg + 1);
+            pair_off = a.take<uint32_t>((size_t)TBg + 1);
             sm_slots = a.take<uint32_t>(256);
         }
     };
@@ -1794,17 +1867,22 @@ int msm_core(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, co
                 for (int l = 0; l < levels; l++) {
                     uint32_t* off_out = off_bufs[l & 1];
                     uint32_t* dense_out = dense_bufs[l & 1];
-                    k_halve_counts<<<(tb + 256) / 256, 256, 0, stream>>>(off_in, cnt_tmp, tb);
+                    k_halve_counts<<<(tb + 256) / 256, 256, 0, stream>>>(off_in, cnt_tmp, pair_cnt, tb);
                     CUDA_TRY(cub::DeviceScan::ExclusiveSum(cub_tmp, cub_bytes, cnt_tmp, off_out, (int)(tb + 1), stream));
-                    bound = bound / 2 + tb;                              // Σ ceil(cnt/2) ≤ Σ cnt/2 + #buckets
+                    if (!pair_v1) CUDA_TRY(cub::DeviceScan::ExclusiveSum(cub_tmp, cub_bytes, pair_cnt, pair_off, (int)(tb + 1), stream));
+                    // pairs: Σ ⌊cnt/2⌋ ≤ Σ cnt/2; all outputs (pairs and single inputs): Σ ⌈cnt/2⌉ ≤ Σ cnt/2 + #buckets
+                    const size_t pair_bound = pair_v1 ? bound / 2 + tb : bound / 2;
+                    bound = bound / 2 + tb;
                     // Whole waves: 132 SMs × 4 resident CTAs × 128 threads = 67584 lanes run at once on an H100; give every lane
-                    // the same number T of outputs and launch an integer number of such waves, so no partial last wave
+                    // the same number T of pairs and launch an integer number of such waves, so no partial last wave
                     // idles most of the machine (a level is one long-running CTA per slot, not many short ones).
                     const size_t wave = (size_t)sm_count * (pair_v1 ? 4 : pair_minb) * 128;
-                    size_t waves = (bound + 1024 * wave - 1) / (1024 * wave);
+                    size_t waves = (pair_bound + 1024 * wave - 1) / (1024 * wave);
                     if (pair_waves) waves = pair_waves;
-                    size_t T = (bound + waves * wave - 1) / (waves * wave);
-                    const size_t nthreads = (bound + T - 1) / T;
+                    if (waves == 0) waves = 1;
+                    size_t T = (pair_bound + waves * wave - 1) / (waves * wave);
+                    if (T == 0) T = 1;
+                    const size_t nthreads = pair_bound > T ? (pair_bound + T - 1) / T : 1;
                     const unsigned lgrid = (unsigned)((nthreads + 127) / 128);
                     // level 0 reads absolute positions of `sorted` (off_in = bs); its outputs and all later levels are
                     // group-relative (the scans start at 0)
@@ -1814,18 +1892,22 @@ int msm_core(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, co
                         else
                             k_pair_level<false><<<lgrid, 128, 0, stream>>>(nullptr, nullptr, dense_in, off_in, off_out, tb, (uint32_t)T, prefix, dense_out);
                     } else {
-                        const unsigned dgrid = (unsigned)((bound + 255) / 256);
+                        // one thread per bucket (single inputs) and one warp per 32·DESC_CHUNKS pairs
+                        const size_t desc_warps = (pair_bound + 32 * DESC_CHUNKS - 1) / (32 * DESC_CHUNKS);
+                        const size_t desc_threads = desc_warps * 32 > (size_t)tb ? desc_warps * 32 : (size_t)tb;
+                        const unsigned dgrid = (unsigned)((desc_threads + 255) / 256);
+                        const uint32_t* pair_total = pair_off + tb;
                         if (l == 0 && !records) {
-                            k_pair_desc<true><<<dgrid, 256, 0, stream>>>(sorted, off_in, off_out, tb, desc, nullptr);
-                            if (pair_minb == 3) k_pair_level2<true, 3><<<lgrid, 128, PAIR2_SMEM, stream>>>(gather_src, BASE_WORDS, desc, off_out + tb, (uint32_t)T, prefix, dense_out, sm_slots);
-                            else k_pair_level2<true, 4><<<lgrid, 128, PAIR2_SMEM, stream>>>(gather_src, BASE_WORDS, desc, off_out + tb, (uint32_t)T, prefix, dense_out, sm_slots);
+                            k_pair_desc<true><<<dgrid, 256, 0, stream>>>(sorted, off_in, off_out, pair_off, tb, desc, out_pos, nullptr, gather_src, BASE_WORDS, dense_out);
+                            if (pair_minb == 3) k_pair_level2<true, 3><<<lgrid, 128, PAIR2_SMEM, stream>>>(gather_src, BASE_WORDS, desc, out_pos, pair_total, (uint32_t)T, prefix, dense_out, sm_slots);
+                            else k_pair_level2<true, 4><<<lgrid, 128, PAIR2_SMEM, stream>>>(gather_src, BASE_WORDS, desc, out_pos, pair_total, (uint32_t)T, prefix, dense_out, sm_slots);
                         } else {
-                            k_pair_desc<false><<<dgrid, 256, 0, stream>>>(nullptr, off_in, off_out, tb, desc, l == 0 ? bs : nullptr);
                             const uint32_t in_words = l == 0 ? rec_words : (uint32_t)DENSE_WORDS;
-                            if (pair_minb == 3) k_pair_level2<false, 3><<<lgrid, 128, PAIR2_SMEM, stream>>>(dense_in, in_words, desc, off_out + tb, (uint32_t)T, prefix, dense_out, sm_slots);
-                            else k_pair_level2<false, 4><<<lgrid, 128, PAIR2_SMEM, stream>>>(dense_in, in_words, desc, off_out + tb, (uint32_t)T, prefix, dense_out, sm_slots);
+                            k_pair_desc<false><<<dgrid, 256, 0, stream>>>(nullptr, off_in, off_out, pair_off, tb, desc, nullptr, l == 0 ? bs : nullptr, dense_in, in_words, dense_out);
+                            if (pair_minb == 3) k_pair_level2<false, 3><<<lgrid, 128, PAIR2_SMEM, stream>>>(dense_in, in_words, desc, nullptr, pair_total, (uint32_t)T, prefix, dense_out, sm_slots);
+                            else k_pair_level2<false, 4><<<lgrid, 128, PAIR2_SMEM, stream>>>(dense_in, in_words, desc, nullptr, pair_total, (uint32_t)T, prefix, dense_out, sm_slots);
                         }
-                        count_launch(1);
+                        count_launch(2);                                 // the pair scan and the descriptors
                     }
                     count_launch(3);
                     off_in = off_out;
