@@ -504,6 +504,26 @@ SNARKVM_API int snarkvm_b200_pairing_products_device(void* d_gt, uint32_t* d_is_
                                                      const uint32_t* d_g2_index, size_t npairs, const void* d_prepared, size_t nprepared,
                                                      const uint32_t* d_check_start, size_t nchecks, int64_t* bad_check, void* stream);
 
+/* Poseidon duplex sponge transcripts (PoseidonSponge<F, 2, 1>, algorithms/src/crypto_hash/poseidon.rs; snarkVM's Fiat–Shamir
+ * sponge is field = FQ), one thread per transcript.  d_params: the sponge's 39 × 3 round keys then its 3 × 3 MDS matrix, Montgomery
+ * F (snarkvm_b200/poseidon.py builds them).  Transcript t runs operations [d_op_start[t], d_op_start[t + 1]) of d_ops, each three
+ * u32 (kind, n, offset), on a sponge of its own:
+ *   ABSORB                    absorb_native_field_elements of d_in[offset … offset + n)  (Montgomery F, each below p)
+ *   SQUEEZE                   squeeze_native_field_elements(n) → d_out[offset …]         (Montgomery F)
+ *   SQUEEZE_NONNATIVE         squeeze_nonnative_field_elements::<Fr>(n) → d_out_fr[offset …]  (Montgomery Fr, 32 B)
+ *   SQUEEZE_SHORT_NONNATIVE   squeeze_short_nonnative_field_elements::<Fr>(n) (168-bit) → d_out_fr[offset …]
+ * Elements are 32 B (Fr) or 48 B (Fq); d_params, d_in, d_out and d_out_fr are 16-byte aligned.  n = 0 is no operation.  Two launches
+ * and one synchronisation per call.  An unknown kind, a range outside nin / nout / nout_fr, an absorbed element not below p or a
+ * d_op_start entry out of order or beyond nops returns cudaErrorInvalidValue, *bad_transcript (HOST, may be NULL) receives the
+ * lowest transcript concerned (-1 otherwise), and no output is written. */
+enum {
+    SNARKVM_B200_POSEIDON_ABSORB = 0, SNARKVM_B200_POSEIDON_SQUEEZE = 1, SNARKVM_B200_POSEIDON_SQUEEZE_NONNATIVE = 2,
+    SNARKVM_B200_POSEIDON_SQUEEZE_SHORT_NONNATIVE = 3
+};
+SNARKVM_API int snarkvm_b200_poseidon_transcripts_device(int field, const void* d_params, const uint32_t* d_ops, const uint32_t* d_op_start,
+                                                         size_t ntranscripts, size_t nops, const void* d_in, size_t nin, void* d_out,
+                                                         size_t nout, void* d_out_fr, size_t nout_fr, int64_t* bad_transcript, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

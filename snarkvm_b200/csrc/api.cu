@@ -27,6 +27,7 @@
 #include "ntt.cuh"
 #include "pairing.cuh"
 #include "poly.cuh"
+#include "poseidon.cuh"
 
 namespace b200 { void host_stream_copy(void* dst, const void* src, size_t n); }      // hostcopy.cpp: memcpy with non-temporal stores
 using namespace b200;
@@ -1230,6 +1231,12 @@ int snarkvm_b200_pairing_products_device(void* d_gt, uint32_t* d_is_one, void* d
                                          const uint32_t* d_check_start, size_t nchecks, int64_t* bad_check, void* stream) {
     return pairing_products_device(d_gt, d_is_one, d_miller, d_g1, g1_stride, d_g2_index, npairs, d_prepared, nprepared, d_check_start,
                                    nchecks, bad_check, (cudaStream_t)stream);
+}
+int snarkvm_b200_poseidon_transcripts_device(int field, const void* d_params, const uint32_t* d_ops, const uint32_t* d_op_start,
+                                             size_t ntranscripts, size_t nops, const void* d_in, size_t nin, void* d_out, size_t nout,
+                                             void* d_out_fr, size_t nout_fr, int64_t* bad_transcript, void* stream) {
+    return poseidon_transcripts_device(field, d_params, d_ops, d_op_start, ntranscripts, nops, d_in, nin, d_out, nout, d_out_fr, nout_fr,
+                                       bad_transcript, (cudaStream_t)stream);
 }
 
 int snarkvm_b200_register_bases(const void* host_points, size_t npoints, size_t stride) {

@@ -12,7 +12,7 @@ import ctypes
 import numpy as np
 import torch
 
-from . import _lib
+from . import _lib, poseidon
 from .cuda import NTTDirection, NTTInputOutputOrder, NTTType
 
 XYZZ_BYTES = 192
@@ -163,6 +163,43 @@ def pairing_products(g1: torch.Tensor, g2_index: torch.Tensor, prepared: torch.T
         err.check = bad.value if bad.value >= 0 else None
         raise err
     return (gt, is_one.bool(), mv) if miller else (gt, is_one.bool())
+
+
+POSEIDON_ABSORB, POSEIDON_SQUEEZE, POSEIDON_SQUEEZE_NONNATIVE, POSEIDON_SQUEEZE_SHORT_NONNATIVE = 0, 1, 2, 3
+
+
+def poseidon_transcripts(field: int, ops: torch.Tensor, op_start: torch.Tensor, inputs: torch.Tensor, nout: int, nout_fr: int):
+    """PoseidonSponge<F, 2, 1> transcripts, one per thread (snarkvm_b200_poseidon_transcripts_device): transcript t runs the
+    operations ops[op_start[t] : op_start[t + 1]] (int32 [nops, 3]: kind POSEIDON_*, n, offset) on a sponge of its own.  field:
+    poseidon.FIELD_FQ (snarkVM's Fiat–Shamir sponge) or FIELD_FR.  inputs: Montgomery F elements as int64 [nin, 6] (Fq) or
+    [nin, 4] (Fr).  → (native squeezes int64 [nout, limbs] Montgomery F, nonnative squeezes int64 [nout_fr, 4] Montgomery Fr), both in
+    HBM.  A malformed operation or an absorbed element ≥ p raises CudaError naming the lowest such transcript (.transcript), and no
+    output is written."""
+    if field not in poseidon.FIELDS:
+        raise ValueError(f"unknown field {field}")
+    words = poseidon.FIELDS[field][2]
+    dev = op_start.device
+    if op_start.dtype != torch.int32 or op_start.dim() != 1 or op_start.numel() < 1:
+        raise ValueError("op_start: int32, one entry more than there are transcripts")
+    if ops.dtype != torch.int32 or ops.dim() != 2 or ops.shape[1] != 3:
+        raise ValueError("ops: int32 [nops, 3]")
+    if inputs.dtype != torch.int64 or inputs.dim() != 2 or inputs.shape[1] != words // 2:
+        raise ValueError(f"inputs: int64 [nin, {words // 2}]")
+    ntranscripts, nops, nin = op_start.numel() - 1, ops.shape[0], inputs.shape[0]
+    out = torch.empty((nout, words // 2), dtype=torch.int64, device=dev)
+    out_fr = torch.empty((nout_fr, 4), dtype=torch.int64, device=dev)
+    params = poseidon.device_parameters(field, dev)
+    bad = ctypes.c_int64(-1)
+    with torch.cuda.device(dev):
+        code = _lib.lib().snarkvm_b200_poseidon_transcripts_device(
+            field, _check(params, "params"), _check(ops, "ops") if nops else None, _check(op_start, "op_start"), ntranscripts, nops,
+            _check(inputs, "inputs") if nin else None, nin, out.data_ptr() if nout else None, nout,
+            out_fr.data_ptr() if nout_fr else None, nout_fr, ctypes.byref(bad), _stream())
+    if code != 0:
+        err = _lib.CudaError(code, f"transcript {bad.value}" if bad.value >= 0 else "see cudaError_t")
+        err.transcript = bad.value if bad.value >= 0 else None
+        raise err
+    return out, out_fr
 
 
 def msm_window_sums(bases: torch.Tensor, scalars: torch.Tensor, stride: int = AFFINE_STRIDE, plan_npoints: int | None = None,

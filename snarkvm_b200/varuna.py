@@ -7,6 +7,7 @@ bulk field arithmetic — the five `AHPForR1CS::prover_*_round` functions and th
     ahp/matrices.rs:211-240                        Circuit.index_polynomials (MatrixArithmetization::new)
     varuna.rs:72-134, 226-233                      circuit_setup        (the verifying key's twelve index commitments)
     ahp/indexer/circuit.rs:109-121                 Circuit.id           (Blake2s of the index counts and the serialized matrices)
+    varuna.rs:155-165, 236-331                     certificate_challenges (the certificate's Poseidon transcript)
     varuna.rs:236-276                              prove_vk             (the verifying-key certificate)
     ahp/indexer/indexer.rs:232-260                 Circuit.evaluate_index_polynomials
     varuna.rs:280-331                              verify_vk            (up to the final pairing)
@@ -22,7 +23,8 @@ bulk field arithmetic — the five `AHPForR1CS::prover_*_round` functions and th
 for the NON-HIDING mode (VarunaNonHidingMode), one circuit, any batch of instances.  Everything O(n) runs in this library's
 kernels (NTT passes, PolyMultiplier pipeline, divide_by_vanishing_poly, batch inversion, sparse mat-vec, elementwise Fr ops);
 torch only owns the buffers and does index plumbing (gathers, concatenation).  Challenges are host scalars: the Fiat-Shamir
-sponge (Poseidon) is sequential and stays on the CPU (SURVEY §8 f3), so callers pass α, η, β, δ in.
+sponge (Poseidon) of the prover rounds is not on the device yet, so callers pass α, η, β, δ in; the certificate's transcript is
+(certificate_challenges, on csrc/poseidon.cu).
 Polynomials are CUDA tensors [m, 4] int64 (Montgomery Fr, low degree first, NOT trimmed: trailing zero coefficients may be present;
 `trimmed()` gives the reference's canonical form on the host).
 """
@@ -36,7 +38,7 @@ from dataclasses import dataclass
 import numpy as np
 import torch
 
-from . import device
+from . import device, poseidon
 from ._lib import CudaError
 from .algorithms import EvaluationDomain, _fr_int_to_mont, _fr_mont_to_int
 from .cuda import NTTDirection, NTTType
@@ -437,15 +439,82 @@ def _certificate_point(challenges) -> tuple:
     return challenges[-1], [1] + challenges[:-1]
 
 
-def prove_vk_batch(pks: list, challenges: list, opening_challenges: list) -> list:
-    """VarunaSNARK::prove_vk (varuna.rs:236-276) after the sponge, for every proving key: open Σ c_i·p_i over its twelve index
-    polynomials (c = [1] + challenges[k][:11] in label order) at z = challenges[k][11] → [Certificate] in input order.  The opening is
+PROTOCOL_NAME = b"VARUNA-2023"                                           # VarunaSNARK::PROTOCOL_NAME (varuna.rs:68)
+_CERTIFICATE_ELEMENTS = 40          # absorbed per certificate: name 1, CircuitInfo 2, twelve commitments × (x, y, infinity) 36, id 1
+_CERTIFICATE_SQUEEZES = 14          # nonnative Fr per certificate: twelve challenges, then ξ and the randomizer (short)
+
+
+def _certificate_transcripts(vks: list):
+    """init_sponge_for_certificate (varuna.rs:155-165) of every key, then its squeezes, as the op lists of
+    device.poseidon_transcripts → (ops, op_start, inputs) as host arrays.  Per key: absorb_bytes of the protocol name (to_bytes_le!
+    of a byte slice writes the bytes without a length prefix, utilities/src/bytes.rs:442-457), of CircuitInfo::to_bytes_le and of the
+    id, and absorb_native_field_elements of the twelve commitments as SWAffine::to_field_elements (x, y, infinity flag,
+    curves/src/templates/to_field_vec.rs:52-64); then squeeze_nonnative_field_elements(12) (varuna.rs:248, 293) and two
+    squeeze_short_nonnative_field_element calls: combine_for_open's challenge ξ and batch_open's `_randomizer` on the prover side
+    (sonic_pc/mod.rs:277, 329), accumulate_elems' curr_challenge and batch_check's next randomizer on the verifier side (:602, :405)
+    — the same two squeezes in the same order."""
+    fq = poseidon.FIELD_FQ
+    K = len(vks)
+    name = poseidon.to_mont_words(fq, poseidon.bytes_to_field_elements(PROTOCOL_NAME, fq))
+    one = poseidon.to_mont_words(fq, [1])[0]
+    inputs = np.zeros((K, _CERTIFICATE_ELEMENTS, 12), dtype=np.uint32)
+    for k, vk in enumerate(vks):
+        if vk.id is None:
+            raise ValueError(f"verifying key {k} has no circuit id; a certificate's transcript absorbs it")
+        comms = np.ascontiguousarray(vk.circuit_commitments, dtype=np.uint64).reshape(len(INDEX_POLYNOMIAL_NAMES), 18)
+        info = poseidon.to_mont_words(fq, poseidon.bytes_to_field_elements(vk.circuit_info.to_bytes_le(), fq))
+        ident = poseidon.to_mont_words(fq, poseidon.bytes_to_field_elements(bytes(vk.id), fq))
+        if len(name) + len(info) + 3 * comms.shape[0] + len(ident) != _CERTIFICATE_ELEMENTS:
+            raise ValueError(f"verifying key {k}: a 32-byte id and twelve commitments expected")
+        # a normalised projective image is (x, y, 1) or (0, 1, 0): its X, Y are the affine x, y of SWAffine, Affine::zero() included
+        c = np.zeros((comms.shape[0], 3, 12), dtype=np.uint32)
+        c[:, 0] = comms[:, 0:6].view(np.uint32)
+        c[:, 1] = comms[:, 6:12].view(np.uint32)
+        c[~comms[:, 12:18].any(axis=1), 2] = one
+        inputs[k] = np.concatenate([name, info, c.reshape(-1, 12), ident])
+    base_in = np.arange(K, dtype=np.int64)[:, None] * _CERTIFICATE_ELEMENTS
+    base_out = np.arange(K, dtype=np.int64)[:, None] * _CERTIFICATE_SQUEEZES
+    ops = np.zeros((K, 7, 3), dtype=np.int64)
+    short = poseidon.OP_SQUEEZE_SHORT_NONNATIVE
+    ops[:, :, 0] = [poseidon.OP_ABSORB] * 4 + [poseidon.OP_SQUEEZE_NONNATIVE, short, short]
+    ops[:, :, 1] = [1, 2, 36, 1, 12, 1, 1]
+    ops[:, :4, 2] = base_in + [0, 1, 3, 39]
+    ops[:, 4:, 2] = base_out + [0, 12, 13]
+    op_start = np.arange(0, 7 * K + 1, 7, dtype=np.int32)
+    return ops.reshape(-1, 3).astype(np.int32), op_start, inputs.reshape(-1, 12)
+
+
+def certificate_challenges(vks: list, device_=None) -> list:
+    """The Fiat–Shamir challenges of every key's certificate, as prove_vk and verify_vk draw them from PoseidonSponge<Fq, 2, 1>
+    (init_sponge_for_certificate, varuna.rs:155-165, then varuna.rs:248 / 293 and sonic_pc/mod.rs:277, 329 / 602, 405) → [(twelve
+    challenges, (ξ, randomizer))] in input order, canonical integers mod r.  The transcript depends only on the verifying key; all K
+    run in one device call, one thread each.  A key without a circuit id raises ValueError (a reference key always has its id)."""
+    if not vks:
+        raise ValueError("no verifying keys")
+    ops, op_start, inputs = _certificate_transcripts(vks)
+    dev = torch.device(device_) if device_ is not None else torch.device("cuda", torch.cuda.current_device())
+    _out, fr = device.poseidon_transcripts(
+        poseidon.FIELD_FQ, torch.from_numpy(ops).to(dev), torch.from_numpy(op_start).to(dev),
+        torch.from_numpy(inputs.view(np.int64)).to(dev), 0, _CERTIFICATE_SQUEEZES * len(vks))
+    vals = [_fr_mont_to_int(row) for row in fr.cpu().numpy().view(np.uint64)]
+    S = _CERTIFICATE_SQUEEZES
+    return [(vals[S * k: S * k + 12], (vals[S * k + 12], vals[S * k + 13])) for k in range(len(vks))]
+
+
+def prove_vk_batch(pks: list, challenges: list | None = None, opening_challenges: list | None = None) -> list:
+    """VarunaSNARK::prove_vk (varuna.rs:236-276) for every proving key: open Σ c_i·p_i over its twelve index polynomials
+    (c = [1] + challenges[k][:11] in label order) at z = challenges[k][11] → [Certificate] in input order.  The opening is
     SonicKZG10.batch_open of `circuit_check` with empty randomness: it consumes opening_challenges[k] (its combination challenge ξ,
     then the discarded randomizer) as open_combinations would, and scales the combination by ξ, which is folded into the
-    coefficients.  All interpolations share one batched iNTT, all K combinations one fr_lincomb launch, and all K witness
-    commitments one MSM pass."""
+    coefficients.  Omitted challenges (None) are the sponge's: certificate_challenges of the verifying keys, which needs each key's
+    id.  All interpolations share one batched iNTT, all K combinations one fr_lincomb launch, and all K witness commitments one MSM
+    pass."""
     if not pks:
         raise ValueError("no proving keys")
+    if challenges is None or opening_challenges is None:
+        derived = certificate_challenges([pk.circuit_verifying_key for pk in pks], _device_of([pk.circuit for pk in pks]))
+        challenges = [d[0] for d in derived] if challenges is None else challenges
+        opening_challenges = [d[1] for d in derived] if opening_challenges is None else opening_challenges
     if len(challenges) != len(pks) or len(opening_challenges) != len(pks):
         raise ValueError("one set of challenges and opening challenges per proving key")
     points = [_certificate_point(ch) for ch in challenges]
@@ -468,9 +537,10 @@ def prove_vk_batch(pks: list, challenges: list, opening_challenges: list) -> lis
     return [Certificate(w.copy()) for w in ws]
 
 
-def prove_vk(pk: CircuitProvingKey, challenges, opening_challenges) -> Certificate:
-    """VarunaSNARK::prove_vk (varuna.rs:236-276) after the sponge: prove_vk_batch of one proving key"""
-    return prove_vk_batch([pk], [challenges], [opening_challenges])[0]
+def prove_vk(pk: CircuitProvingKey, challenges=None, opening_challenges=None) -> Certificate:
+    """VarunaSNARK::prove_vk (varuna.rs:236-276): prove_vk_batch of one proving key (the sponge's challenges when omitted)"""
+    return prove_vk_batch([pk], None if challenges is None else [challenges],
+                          None if opening_challenges is None else [opening_challenges])[0]
 
 
 @dataclass
@@ -562,10 +632,11 @@ def _affine_neg(projective: np.ndarray) -> np.ndarray:
     return out
 
 
-def verify_vk_batch(circuits: list, vks: list, certificates: list, challenges: list, opening_challenges: list,
+def verify_vk_batch(circuits: list, vks: list, certificates: list, challenges: list | None = None, opening_challenges: list | None = None,
                     verifier: UniversalVerifier | None = None) -> list:
     """VarunaSNARK::verify_vk (varuna.rs:280-331) up to the pairing, for every (circuit, verifying key, certificate) → [VerifyingKeyCheck]
-    in input order.  The circuits are already indexed (Circuit).  The evaluation v comes from evaluate_index_polynomials;
+    in input order.  The circuits are already indexed (Circuit).  Omitted challenges (None) are the sponge's: certificate_challenges
+    of the verifying keys (their twelve challenges and ξ), which needs each key's id.  The evaluation v comes from evaluate_index_polynomials;
     check_combinations → batch_check → accumulate_elems for one point with randomizer one (sonic_pc/mod.rs:344-411, 477-544, 582-635)
     reduces to lhs = ξ·C_lc − ξ·v·G + z·W with C_lc = Σ c_i·C_i, ξ = opening_challenges[k]: a 14-point sum over the twelve commitments,
     G and W.  check_elems' pairing equation is then e(lhs, H) = e(W, β·H).  G is the universal verifier's g, the SRS's first power,
@@ -574,6 +645,12 @@ def verify_vk_batch(circuits: list, vks: list, certificates: list, challenges: l
     K = len(circuits)
     if K == 0:
         raise ValueError("no circuits to verify")
+    if challenges is None or opening_challenges is None:
+        if len(vks) != K:
+            raise ValueError("one verifying key per circuit")
+        derived = certificate_challenges(vks, _device_of(circuits))
+        challenges = [d[0] for d in derived] if challenges is None else challenges
+        opening_challenges = [d[1][0] for d in derived] if opening_challenges is None else opening_challenges
     if not (len(vks) == len(certificates) == len(challenges) == len(opening_challenges) == K):
         raise ValueError("one verifying key, certificate, set of challenges and opening challenge per circuit")
     points = [_certificate_point(ch) for ch in challenges]
@@ -606,10 +683,12 @@ def verify_vk_batch(circuits: list, vks: list, certificates: list, challenges: l
     return checks
 
 
-def verify_vk(circuit: Circuit, vk: CircuitVerifyingKey, certificate: Certificate, challenges, opening_challenge: int,
+def verify_vk(circuit: Circuit, vk: CircuitVerifyingKey, certificate: Certificate, challenges=None, opening_challenge: int | None = None,
               verifier: UniversalVerifier | None = None) -> VerifyingKeyCheck:
-    """VarunaSNARK::verify_vk (varuna.rs:280-331): verify_vk_batch of one circuit (up to the pairing without a verifier)"""
-    return verify_vk_batch([circuit], [vk], [certificate], [challenges], [opening_challenge], verifier)[0]
+    """VarunaSNARK::verify_vk (varuna.rs:280-331): verify_vk_batch of one circuit (up to the pairing without a verifier; the
+    sponge's challenges when omitted)"""
+    return verify_vk_batch([circuit], [vk], [certificate], None if challenges is None else [challenges],
+                           None if opening_challenge is None else [opening_challenge], verifier)[0]
 
 
 def witness_label(circuit_id: bytes, poly: str, i: int) -> str:
