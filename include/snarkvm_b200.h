@@ -524,6 +524,17 @@ SNARKVM_API int snarkvm_b200_poseidon_transcripts_device(int field, const void* 
                                                          size_t ntranscripts, size_t nops, const void* d_in, size_t nin, void* d_out,
                                                          size_t nout, void* d_out_fr, size_t nout_fr, int64_t* bad_transcript, void* stream);
 
+/* The same transcripts resumed from, and saved back to, d_state: one record per transcript, 16-byte aligned, of 3·(F's words) + 4
+ * u32 (Fr 28, Fq 40): the three state elements (Montgomery F, the capacity element first), then DuplexSpongeMode (0 absorbing,
+ * 1 squeezing), then next_absorb_index / next_squeeze_index (0 … 2), then two words written as zero.  A fresh sponge is all zeros.
+ * The record is read before the first operation and written after the last.  Besides the errors above, a record with an element
+ * not below p, an unknown mode or an index above 2 is reported in the same way (lowest transcript concerned), and then neither the
+ * outputs nor any record is written.  d_state may be NULL only when ntranscripts = 0. */
+SNARKVM_API int snarkvm_b200_poseidon_transcripts_resume_device(int field, const void* d_params, const uint32_t* d_ops,
+                                                                const uint32_t* d_op_start, size_t ntranscripts, size_t nops,
+                                                                const void* d_in, size_t nin, void* d_out, size_t nout, void* d_out_fr,
+                                                                size_t nout_fr, void* d_state, int64_t* bad_transcript, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

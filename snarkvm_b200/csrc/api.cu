@@ -1236,7 +1236,14 @@ int snarkvm_b200_poseidon_transcripts_device(int field, const void* d_params, co
                                              size_t ntranscripts, size_t nops, const void* d_in, size_t nin, void* d_out, size_t nout,
                                              void* d_out_fr, size_t nout_fr, int64_t* bad_transcript, void* stream) {
     return poseidon_transcripts_device(field, d_params, d_ops, d_op_start, ntranscripts, nops, d_in, nin, d_out, nout, d_out_fr, nout_fr,
-                                       bad_transcript, (cudaStream_t)stream);
+                                       nullptr, bad_transcript, (cudaStream_t)stream);
+}
+int snarkvm_b200_poseidon_transcripts_resume_device(int field, const void* d_params, const uint32_t* d_ops, const uint32_t* d_op_start,
+                                                    size_t ntranscripts, size_t nops, const void* d_in, size_t nin, void* d_out, size_t nout,
+                                                    void* d_out_fr, size_t nout_fr, void* d_state, int64_t* bad_transcript, void* stream) {
+    if (!d_state && ntranscripts) return (int)cudaErrorInvalidValue;
+    return poseidon_transcripts_device(field, d_params, d_ops, d_op_start, ntranscripts, nops, d_in, nin, d_out, nout, d_out_fr, nout_fr,
+                                       d_state, bad_transcript, (cudaStream_t)stream);
 }
 
 int snarkvm_b200_register_bases(const void* host_points, size_t npoints, size_t stride) {

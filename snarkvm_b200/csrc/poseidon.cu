@@ -18,7 +18,13 @@
 // most significant first, and consecutive groups of 252 (or 168) bits are read as big-endian integers — below 2^252 < r, so each is
 // already a reduced Fr, written in Montgomery form.  Bits beyond the last group are dropped (get_bits' truncate).
 //
-// The check kernel runs first; the sponge kernel reads its verdict and writes nothing when any transcript is malformed.
+// A resumable transcript keeps its sponge between calls in a state record (d_state, one per transcript): the three state elements
+// (Montgomery F), then one word for DuplexSpongeMode (0 absorbing, 1 squeezing) and one for next_absorb_index / next_squeeze_index
+// (0 … RATE), then two zero words, so that every record is a whole number of 16-byte lines.  The sponge kernel loads the record
+// before the first operation and stores it after the last; without records a transcript starts fresh (zeros, absorbing at 0) and
+// nothing is stored.  Both entry points are this one path.
+//
+// The check kernel runs first; the sponge kernel reads its verdict and writes nothing when any transcript or record is malformed.
 #include "msm.cuh"
 
 #define FF_CALL_MUL 1
@@ -34,6 +40,9 @@ constexpr int P_PARAMS = P_ROUNDS * P_WIDTH + P_WIDTH * P_WIDTH;           // ar
 constexpr uint32_t NO_BAD = 0xffffffffu;
 constexpr int FULL_NONNATIVE_BITS = 252, SHORT_NONNATIVE_BITS = 168;
 constexpr int THREADS = 128;
+constexpr uint32_t MODE_ABSORBING = 0, MODE_SQUEEZING = 1;
+
+template <class P> struct StateWords { static constexpr int value = P_WIDTH * P::N + 4; };   // a state record, in 32-bit words
 
 template <class P> struct FieldBits;                                         // MODULUS_BITS (F::size_in_bits())
 template <> struct FieldBits<FrParams> { static constexpr int value = 253; };
@@ -72,16 +81,25 @@ FF_DEV void permute(Fp<P> (&s)[P_WIDTH], const Fp<P>* ark, const Fp<P>* mds) {
     }
 }
 
-// one thread per transcript: every operation of [op_start[t], op_start[t + 1]) has a known kind and a range inside its array, and
-// every element it absorbs is below p; otherwise *bad_min receives t
+// one thread per transcript: its state record (when there are records) holds elements below p, a known mode and an index ≤ RATE,
+// every operation of [op_start[t], op_start[t + 1]) has a known kind and a range inside its array, and every element it absorbs is
+// below p; otherwise *bad_min receives t
 template <class P>
 __global__ void __launch_bounds__(THREADS) k_poseidon_check(const uint32_t* __restrict__ ops, const uint32_t* __restrict__ op_start,
                                                             uint32_t ntranscripts, uint32_t nops, const uint32_t* __restrict__ in,
-                                                            uint64_t nin, uint64_t nout, uint64_t nout_fr, uint32_t* __restrict__ bad_min) {
+                                                            uint64_t nin, uint64_t nout, uint64_t nout_fr, const uint32_t* __restrict__ state,
+                                                            uint32_t* __restrict__ bad_min) {
     const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= ntranscripts) return;
     const uint32_t s = op_start[t], e = op_start[t + 1];
     bool ok = s <= e && e <= nops;
+    if (state) {
+        const uint32_t* rec = state + (size_t)t * StateWords<P>::value;
+#pragma unroll 1
+        for (int i = 0; ok && i < P_WIDTH; i++) ok = is_canonical(Fp<P>::load(rec + i * P::N));
+        const uint32_t mode = rec[P_WIDTH * P::N], idx = rec[P_WIDTH * P::N + 1];
+        ok = ok && (mode == MODE_ABSORBING || mode == MODE_SQUEEZING) && idx <= (uint32_t)P_RATE;
+    }
 #pragma unroll 1
     for (uint32_t k = s; ok && k < e; k++) {
         const uint32_t kind = ops[3 * k], n = ops[3 * k + 1], off = ops[3 * k + 2];
@@ -134,7 +152,8 @@ template <class P>
 __global__ void __launch_bounds__(THREADS) k_poseidon_transcripts(const uint32_t* __restrict__ params, const uint32_t* __restrict__ ops,
                                                                   const uint32_t* __restrict__ op_start, uint32_t ntranscripts,
                                                                   const uint32_t* __restrict__ in, uint32_t* __restrict__ out,
-                                                                  uint32_t* __restrict__ out_fr, const uint32_t* __restrict__ bad_min) {
+                                                                  uint32_t* __restrict__ out_fr, uint32_t* __restrict__ state,
+                                                                  const uint32_t* __restrict__ bad_min) {
     using F = Fp<P>;
     __shared__ __align__(16) uint32_t sh[P_PARAMS * P::N];
     if (*bad_min != NO_BAD) return;                                          // a malformed transcript: no output at all
@@ -151,6 +170,13 @@ __global__ void __launch_bounds__(THREADS) k_poseidon_transcripts(const uint32_t
     F s[P_WIDTH] = {F::zero(), F::zero(), F::zero()};
     bool squeezing = false;                                                  // DuplexSpongeMode
     int idx = 0;                                                             // next_absorb_index / next_squeeze_index
+    uint32_t* rec = state ? state + (size_t)t * StateWords<P>::value : nullptr;
+    if (rec) {
+#pragma unroll
+        for (int i = 0; i < P_WIDTH; i++) s[i] = F::load(rec + i * P::N);
+        squeezing = rec[P_WIDTH * P::N] == MODE_SQUEEZING;
+        idx = (int)rec[P_WIDTH * P::N + 1];
+    }
     const uint32_t e = op_start[t + 1];
 #pragma unroll 1
     for (uint32_t k = op_start[t]; k < e; k++) {
@@ -187,19 +213,25 @@ __global__ void __launch_bounds__(THREADS) k_poseidon_transcripts(const uint32_t
             idx++;
         }
     }
+    if (rec) {
+#pragma unroll
+        for (int i = 0; i < P_WIDTH; i++) s[i].store(rec + i * P::N);
+        reinterpret_cast<uint4*>(rec + P_WIDTH * P::N)[0] = make_uint4(squeezing ? MODE_SQUEEZING : MODE_ABSORBING, (uint32_t)idx, 0u, 0u);
+    }
 }
 
 template <class P>
 int run(const void* d_params, const uint32_t* d_ops, const uint32_t* d_op_start, size_t ntranscripts, size_t nops, const void* d_in,
-        size_t nin, void* d_out, size_t nout, void* d_out_fr, size_t nout_fr, uint32_t* d_bad, cudaStream_t stream) {
+        size_t nin, void* d_out, size_t nout, void* d_out_fr, size_t nout_fr, void* d_state, uint32_t* d_bad, cudaStream_t stream) {
     const unsigned blocks = (unsigned)((ntranscripts + THREADS - 1) / THREADS);
     k_poseidon_check<P><<<blocks, THREADS, 0, stream>>>(d_ops, d_op_start, (uint32_t)ntranscripts, (uint32_t)nops, (const uint32_t*)d_in,
-                                                        nin, nout, nout_fr, d_bad);
+                                                        nin, nout, nout_fr, (const uint32_t*)d_state, d_bad);
     count_launch();
     int rc = (int)cudaGetLastError();
     if (rc != 0) return rc;
     k_poseidon_transcripts<P><<<blocks, THREADS, 0, stream>>>((const uint32_t*)d_params, d_ops, d_op_start, (uint32_t)ntranscripts,
-                                                              (const uint32_t*)d_in, (uint32_t*)d_out, (uint32_t*)d_out_fr, d_bad);
+                                                              (const uint32_t*)d_in, (uint32_t*)d_out, (uint32_t*)d_out_fr, (uint32_t*)d_state,
+                                                              d_bad);
     count_launch();
     return (int)cudaGetLastError();
 }
@@ -208,13 +240,14 @@ int run(const void* d_params, const uint32_t* d_ops, const uint32_t* d_op_start,
 
 int poseidon_transcripts_device(int field, const void* d_params, const uint32_t* d_ops, const uint32_t* d_op_start, size_t ntranscripts,
                                 size_t nops, const void* d_in, size_t nin, void* d_out, size_t nout, void* d_out_fr, size_t nout_fr,
-                                int64_t* bad_transcript, cudaStream_t stream) {
+                                void* d_state, int64_t* bad_transcript, cudaStream_t stream) {
     if (bad_transcript) *bad_transcript = -1;
     if (field != SNARKVM_B200_FIELD_FR && field != SNARKVM_B200_FIELD_FQ) return (int)cudaErrorInvalidValue;
     if (ntranscripts == 0) return 0;
     if (!d_params || !d_op_start || ntranscripts >= NO_BAD || nops >= NO_BAD) return (int)cudaErrorInvalidValue;
     if ((nops && !d_ops) || (nin && !d_in) || (nout && !d_out) || (nout_fr && !d_out_fr)) return (int)cudaErrorInvalidValue;
-    if (((uintptr_t)d_params | (uintptr_t)d_in | (uintptr_t)d_out | (uintptr_t)d_out_fr) & 15) return (int)cudaErrorInvalidValue;
+    if (((uintptr_t)d_params | (uintptr_t)d_in | (uintptr_t)d_out | (uintptr_t)d_out_fr | (uintptr_t)d_state) & 15)
+        return (int)cudaErrorInvalidValue;
     if (((uintptr_t)d_ops | (uintptr_t)d_op_start) & 3) return (int)cudaErrorInvalidValue;
     uint32_t* d_bad = nullptr;
     cudaError_t e = pool_alloc(&d_bad, 256, stream);
@@ -222,8 +255,10 @@ int poseidon_transcripts_device(int field, const void* d_params, const uint32_t*
     int rc = (int)cudaMemsetAsync(d_bad, 0xff, 4, stream);
     if (rc == 0) {
         rc = field == SNARKVM_B200_FIELD_FQ
-                 ? run<FqParams>(d_params, d_ops, d_op_start, ntranscripts, nops, d_in, nin, d_out, nout, d_out_fr, nout_fr, d_bad, stream)
-                 : run<FrParams>(d_params, d_ops, d_op_start, ntranscripts, nops, d_in, nin, d_out, nout, d_out_fr, nout_fr, d_bad, stream);
+                 ? run<FqParams>(d_params, d_ops, d_op_start, ntranscripts, nops, d_in, nin, d_out, nout, d_out_fr, nout_fr, d_state, d_bad,
+                                              stream)
+                 : run<FrParams>(d_params, d_ops, d_op_start, ntranscripts, nops, d_in, nin, d_out, nout, d_out_fr, nout_fr, d_state, d_bad,
+                                              stream);
     }
     uint32_t h_bad = NO_BAD;
     if (rc == 0) rc = (int)cudaMemcpyAsync(&h_bad, d_bad, 4, cudaMemcpyDeviceToHost, stream);

@@ -168,13 +168,18 @@ def pairing_products(g1: torch.Tensor, g2_index: torch.Tensor, prepared: torch.T
 POSEIDON_ABSORB, POSEIDON_SQUEEZE, POSEIDON_SQUEEZE_NONNATIVE, POSEIDON_SQUEEZE_SHORT_NONNATIVE = 0, 1, 2, 3
 
 
-def poseidon_transcripts(field: int, ops: torch.Tensor, op_start: torch.Tensor, inputs: torch.Tensor, nout: int, nout_fr: int):
+def poseidon_transcripts(field: int, ops: torch.Tensor, op_start: torch.Tensor, inputs: torch.Tensor, nout: int, nout_fr: int,
+                         state: torch.Tensor | None = None):
     """PoseidonSponge<F, 2, 1> transcripts, one per thread (snarkvm_b200_poseidon_transcripts_device): transcript t runs the
     operations ops[op_start[t] : op_start[t + 1]] (int32 [nops, 3]: kind POSEIDON_*, n, offset) on a sponge of its own.  field:
     poseidon.FIELD_FQ (snarkVM's Fiat–Shamir sponge) or FIELD_FR.  inputs: Montgomery F elements as int64 [nin, 6] (Fq) or
     [nin, 4] (Fr).  → (native squeezes int64 [nout, limbs] Montgomery F, nonnative squeezes int64 [nout_fr, 4] Montgomery Fr), both in
     HBM.  A malformed operation or an absorbed element ≥ p raises CudaError naming the lowest such transcript (.transcript), and no
-    output is written."""
+    output is written.
+    `state`: None starts every transcript from a fresh sponge.  Otherwise one state record per transcript (int64 CUDA tensor
+    [ntranscripts, poseidon.state_words(field) // 2], poseidon.fresh_states makes fresh ones): each transcript resumes from its
+    record and the record is updated in place (snarkvm_b200_poseidon_transcripts_resume_device).  A malformed record raises like a
+    malformed operation, and then no record is written either."""
     if field not in poseidon.FIELDS:
         raise ValueError(f"unknown field {field}")
     words = poseidon.FIELDS[field][2]
@@ -188,13 +193,19 @@ def poseidon_transcripts(field: int, ops: torch.Tensor, op_start: torch.Tensor, 
     ntranscripts, nops, nin = op_start.numel() - 1, ops.shape[0], inputs.shape[0]
     out = torch.empty((nout, words // 2), dtype=torch.int64, device=dev)
     out_fr = torch.empty((nout_fr, 4), dtype=torch.int64, device=dev)
+    if state is not None and (state.dtype != torch.int64 or state.shape != (ntranscripts, poseidon.state_words(field) // 2)):
+        raise ValueError(f"state: int64 [{ntranscripts}, {poseidon.state_words(field) // 2}], one record per transcript")
     params = poseidon.device_parameters(field, dev)
     bad = ctypes.c_int64(-1)
-    with torch.cuda.device(dev):
-        code = _lib.lib().snarkvm_b200_poseidon_transcripts_device(
-            field, _check(params, "params"), _check(ops, "ops") if nops else None, _check(op_start, "op_start"), ntranscripts, nops,
+    args = (field, _check(params, "params"), _check(ops, "ops") if nops else None, _check(op_start, "op_start"), ntranscripts, nops,
             _check(inputs, "inputs") if nin else None, nin, out.data_ptr() if nout else None, nout,
-            out_fr.data_ptr() if nout_fr else None, nout_fr, ctypes.byref(bad), _stream())
+            out_fr.data_ptr() if nout_fr else None, nout_fr)
+    with torch.cuda.device(dev):
+        if state is None:
+            code = _lib.lib().snarkvm_b200_poseidon_transcripts_device(*args, ctypes.byref(bad), _stream())
+        else:
+            code = _lib.lib().snarkvm_b200_poseidon_transcripts_resume_device(*args, _check(state, "state") if ntranscripts else None,
+                                                                              ctypes.byref(bad), _stream())
     if code != 0:
         err = _lib.CudaError(code, f"transcript {bad.value}" if bad.value >= 0 else "see cudaError_t")
         err.transcript = bad.value if bad.value >= 0 else None

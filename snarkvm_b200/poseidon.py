@@ -8,8 +8,9 @@ and fq.rs:180-188.  Snarkvm's Fiat–Shamir sponge is PoseidonSponge<Fq, 2, 1> (
 31 partial rounds.  The reference pins only Fr's parameters; tests/test_poseidon_oracle.py checks this generator against them,
 which is what pins Fq's too.
 
-Everything here is host work: parameters are computed once per process and uploaded once per device; `bytes_to_field_elements`
-and the Montgomery conversions are the O(|input|) encodings a caller does before a `device.poseidon_transcripts` call.
+Everything here is host work: parameters are computed once per process and uploaded once per device; `bytes_to_field_elements`,
+`nonnative_field_elements` and the Montgomery conversions are the O(|input|) encodings a caller does before a
+`device.poseidon_transcripts` call; `fresh_states` makes the state records a resumable transcript starts from.
 """
 from __future__ import annotations
 
@@ -141,6 +142,17 @@ def device_parameters(field: int, dev) -> torch.Tensor:
 _uploaded: dict = {}
 
 
+def state_words(field: int) -> int:
+    """32-bit words of one state record of a resumable transcript: the three state elements, the mode, the index, two zero words"""
+    return 3 * FIELDS[field][2] + 4
+
+
+def fresh_states(field: int, count: int, dev) -> torch.Tensor:
+    """`count` state records of a new sponge (state zero, absorbing at index 0) as the int64 CUDA tensor device.poseidon_transcripts
+    resumes from and updates"""
+    return torch.zeros((count, state_words(field) // 2), dtype=torch.int64, device=dev)
+
+
 def bytes_to_field_elements(data: bytes, field: int) -> list:
     """AlgebraicSponge::absorb_bytes's packing (algorithms/src/traits/algebraic_sponge.rs:47-68): the bytes' bits, most significant
     bit of each byte first, cut into chunks of size_in_bits − 1 bits; each chunk (the last one may be shorter) is read as a
@@ -155,3 +167,62 @@ def bytes_to_field_elements(data: bytes, field: int) -> list:
         out.append((v >> (total - start - width)) & ((1 << width) - 1))
     return out
 
+
+
+# OptimizationType (algorithms/src/traits/algebraic_sponge.rs:156-163)
+OPT_CONSTRAINTS, OPT_WEIGHT = 0, 1
+
+
+def find_parameters(base_field_prime_length: int, target_field_prime_bit_length: int, optimization_type: int) -> tuple:
+    """nonnative_params::find_parameters (algebraic_sponge.rs:166-229): the limb count and limb size of least cost → (num_limbs,
+    bits_per_limb)"""
+    surfeit = 10
+    max_limb_size = min((base_field_prime_length - 1 - surfeit - 1) // 2 - 1, target_field_prime_bit_length)
+    best = None
+    for limb_size in range(1, max_limb_size + 1):
+        num_of_limbs = (target_field_prime_bit_length + limb_size - 1) // limb_size
+        group_size = (base_field_prime_length - 1 - surfeit - 1 - 1 - limb_size + limb_size - 1) // limb_size
+        num_of_groups = (2 * num_of_limbs - 1 + group_size - 1) // group_size
+        t = target_field_prime_bit_length
+        if optimization_type == OPT_CONSTRAINTS:
+            cost = 2 * num_of_limbs - 1 + t + t + num_of_limbs + num_of_groups + (num_of_groups - 1) * (limb_size * 2 + surfeit) + 1
+        else:
+            cost = (6 * num_of_limbs * num_of_limbs + 4 * t + 4 * t + num_of_limbs + num_of_limbs * num_of_limbs + 2 * (2 * num_of_limbs - 1)
+                    + num_of_limbs + num_of_groups + 6 * num_of_groups + (num_of_groups - 1) * (2 * limb_size + surfeit) * 4 + 2)
+        if best is None or cost < best[0]:
+            best = (cost, num_of_limbs, limb_size)
+    return best[1], best[2]
+
+
+def overhead(x: int) -> int:
+    """the `overhead!` macro (algebraic_sponge.rs:105-134) on a non-zero integer: its bit length, plus one unless it is a power of two"""
+    return x.bit_length() + (0 if x & (x - 1) == 0 else 1)
+
+
+# absorb_nonnative_field_elements::<Fr> into the Fq sponge (poseidon.rs:168, 337-432): get_params(253, 377, Weight)
+NONNATIVE_LIMBS, NONNATIVE_LIMB_BITS = find_parameters(FIELDS[FIELD_FQ][1], FIELDS[FIELD_FR][1], OPT_WEIGHT)
+assert (NONNATIVE_LIMBS, NONNATIVE_LIMB_BITS) == (5, 51)
+# every limb is pushed with noise one, so each carries a budget of bits_per_limb + overhead!(1 + 1) bits; two consecutive limbs merge
+# when their budgets fit in the Fq sponge's capacity, size_in_bits − 1
+_LIMB_BUDGET = NONNATIVE_LIMB_BITS + overhead(2)
+_MERGE = 2 * _LIMB_BUDGET <= FIELDS[FIELD_FQ][1] - 1
+
+
+def nonnative_field_elements(values) -> list:
+    """the Fq elements one absorb_nonnative_field_elements call of Fr values absorbs natively (push_elements_to_sponge, poseidon.rs:
+    412-432): each value (canonical, < r) split into NONNATIVE_LIMBS limbs of NONNATIVE_LIMB_BITS bits, big limb first
+    (get_limbs_representations), then compress_elements (:343-377) over the whole stream: a limb and the next merge as
+    first · 2^budget + second while two budgets fit in the capacity; a last odd limb stays alone.  No values give no element."""
+    mask = (1 << NONNATIVE_LIMB_BITS) - 1
+    limbs = []
+    for v in values:
+        v = int(v)
+        if not 0 <= v < R_MOD:
+            raise ValueError("a nonnative value is not below r")
+        limbs += [(v >> (NONNATIVE_LIMB_BITS * i)) & mask for i in reversed(range(NONNATIVE_LIMBS))]
+    if not _MERGE:
+        return limbs
+    out = [(limbs[i] << _LIMB_BUDGET) + limbs[i + 1] for i in range(0, len(limbs) - 1, 2)]
+    if len(limbs) % 2:
+        out.append(limbs[-1])
+    return out

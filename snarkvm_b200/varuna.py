@@ -11,6 +11,8 @@ bulk field arithmetic — the five `AHPForR1CS::prover_*_round` functions and th
     varuna.rs:236-276                              prove_vk             (the verifying-key certificate)
     ahp/indexer/indexer.rs:232-260                 Circuit.evaluate_index_polynomials
     varuna.rs:280-331                              verify_vk            (up to the final pairing)
+    varuna.rs:136-194, 336-620                     prove_batch          (the transcript, the rounds, the commitments and openings → Proof)
+    ahp/verifier/verifier.rs:39-197                Transcript squeezes  (the verifier's messages the prover draws)
     ahp/prover/round_functions/mod.rs:43-192, ahp/prover/state.rs:107-178   init_prover   (z_A, z_B, z_C by sparse mat-vec, x_poly)
     ahp/prover/round_functions/first.rs:129-160    prover_first_round   (w)
     ahp/prover/round_functions/third.rs:207-234    calculate_assignments (z)
@@ -22,15 +24,16 @@ bulk field arithmetic — the five `AHPForR1CS::prover_*_round` functions and th
 
 for the NON-HIDING mode (VarunaNonHidingMode), one circuit, any batch of instances.  Everything O(n) runs in this library's
 kernels (NTT passes, PolyMultiplier pipeline, divide_by_vanishing_poly, batch inversion, sparse mat-vec, elementwise Fr ops);
-torch only owns the buffers and does index plumbing (gathers, concatenation).  Challenges are host scalars: the Fiat-Shamir
-sponge (Poseidon) of the prover rounds is not on the device yet, so callers pass α, η, β, δ in; the certificate's transcript is
-(certificate_challenges, on csrc/poseidon.cu).
+torch only owns the buffers and does index plumbing (gathers, concatenation).  The rounds take their challenges as host scalars;
+prove_batch draws them from its own Fiat–Shamir transcript (Transcript, a resumable PoseidonSponge<Fq, 2, 1> on csrc/poseidon.cu),
+and certificate_challenges draws a certificate's.
 Polynomials are CUDA tensors [m, 4] int64 (Montgomery Fr, low degree first, NOT trimmed: trailing zero coefficients may be present;
 `trimmed()` gives the reference's canonical form on the host).
 """
 from __future__ import annotations
 
 import hashlib
+import random
 import struct
 from concurrent.futures import ThreadPoolExecutor
 from dataclasses import dataclass
@@ -444,6 +447,18 @@ _CERTIFICATE_ELEMENTS = 40          # absorbed per certificate: name 1, CircuitI
 _CERTIFICATE_SQUEEZES = 14          # nonnative Fr per certificate: twelve challenges, then ξ and the randomizer (short)
 
 
+def _commitment_elements(comms) -> np.ndarray:
+    """commitments (normalised projective uint64[k, 18]) → their SWAffine::to_field_elements (x, y, infinity flag,
+    curves/src/templates/to_field_vec.rs:52-64) as Montgomery Fq words uint32[3k, 12].  A normalised projective image is (x, y, 1) or
+    (0, 1, 0): its X, Y are the affine x, y of SWAffine, Affine::zero() included."""
+    comms = np.ascontiguousarray(comms, dtype=np.uint64).reshape(-1, 18)
+    c = np.zeros((comms.shape[0], 3, 12), dtype=np.uint32)
+    c[:, 0] = comms[:, 0:6].view(np.uint32)
+    c[:, 1] = comms[:, 6:12].view(np.uint32)
+    c[~comms[:, 12:18].any(axis=1), 2] = poseidon.to_mont_words(poseidon.FIELD_FQ, [1])[0]
+    return c.reshape(-1, 12)
+
+
 def _certificate_transcripts(vks: list):
     """init_sponge_for_certificate (varuna.rs:155-165) of every key, then its squeezes, as the op lists of
     device.poseidon_transcripts → (ops, op_start, inputs) as host arrays.  Per key: absorb_bytes of the protocol name (to_bytes_le!
@@ -456,7 +471,6 @@ def _certificate_transcripts(vks: list):
     fq = poseidon.FIELD_FQ
     K = len(vks)
     name = poseidon.to_mont_words(fq, poseidon.bytes_to_field_elements(PROTOCOL_NAME, fq))
-    one = poseidon.to_mont_words(fq, [1])[0]
     inputs = np.zeros((K, _CERTIFICATE_ELEMENTS, 12), dtype=np.uint32)
     for k, vk in enumerate(vks):
         if vk.id is None:
@@ -466,12 +480,7 @@ def _certificate_transcripts(vks: list):
         ident = poseidon.to_mont_words(fq, poseidon.bytes_to_field_elements(bytes(vk.id), fq))
         if len(name) + len(info) + 3 * comms.shape[0] + len(ident) != _CERTIFICATE_ELEMENTS:
             raise ValueError(f"verifying key {k}: a 32-byte id and twelve commitments expected")
-        # a normalised projective image is (x, y, 1) or (0, 1, 0): its X, Y are the affine x, y of SWAffine, Affine::zero() included
-        c = np.zeros((comms.shape[0], 3, 12), dtype=np.uint32)
-        c[:, 0] = comms[:, 0:6].view(np.uint32)
-        c[:, 1] = comms[:, 6:12].view(np.uint32)
-        c[~comms[:, 12:18].any(axis=1), 2] = one
-        inputs[k] = np.concatenate([name, info, c.reshape(-1, 12), ident])
+        inputs[k] = np.concatenate([name, info, _commitment_elements(comms), ident])
     base_in = np.arange(K, dtype=np.int64)[:, None] * _CERTIFICATE_ELEMENTS
     base_out = np.arange(K, dtype=np.int64)[:, None] * _CERTIFICATE_SQUEEZES
     ops = np.zeros((K, 7, 3), dtype=np.int64)
@@ -1194,3 +1203,283 @@ def test_circuit_csr(a: int, b: int, mul_depth: int, num_constraints: int, num_v
     z[padded:] = _mont(a)
     z[vb] = _mont(b)
     return circuit, torch.from_numpy(z.view(np.int64)).to(dev)
+
+
+# ---- prove_batch: the prover's Fiat–Shamir transcript and the Proof (varuna.rs:136-194, 336-620; data_structures/proof.rs) ----
+
+class Transcript:
+    """The prover's PoseidonSponge<Fq, 2, 1>, its state kept in HBM between calls as one state record
+    (device.poseidon_transcripts with `state`).  Absorbs only queue operations; `squeeze` runs everything queued and its squeezes
+    in one device call, so a round costs one call.  `calls` and `permutations` count what the sponge has run: the permutations are
+    counted on the host from the mode and index alone, with the kernel's lazy rule (a permutation before the first element of a full
+    rate, or of a change of direction)."""
+
+    def __init__(self, dev):
+        self.dev = torch.device(dev)
+        self.state = poseidon.fresh_states(poseidon.FIELD_FQ, 1, self.dev)
+        self._ops, self._inputs, self._nin = [], [], 0
+        self._squeezing, self._idx = False, 0
+        self.calls = self.permutations = 0
+
+    def _advance(self, absorb: bool, count: int):
+        if count == 0:
+            return
+        if absorb == self._squeezing:
+            self._idx, self._squeezing = poseidon.RATE, not absorb
+        first = poseidon.RATE - self._idx                                 # elements that fit before the next permutation
+        if count > first:
+            self.permutations += -(-(count - first) // poseidon.RATE)
+            self._idx = (count - first - 1) % poseidon.RATE + 1
+        else:
+            self._idx += count
+
+    def absorb_native(self, words: np.ndarray):
+        """absorb_native_field_elements of Montgomery Fq words uint32[n, 12]"""
+        words = np.ascontiguousarray(words, dtype=np.uint32).reshape(-1, 12)
+        if words.shape[0]:
+            self._ops.append((poseidon.OP_ABSORB, words.shape[0], self._nin))
+            self._inputs.append(words)
+            self._nin += words.shape[0]
+            self._advance(True, words.shape[0])
+
+    def absorb_bytes(self, data: bytes):
+        self.absorb_native(poseidon.to_mont_words(poseidon.FIELD_FQ, poseidon.bytes_to_field_elements(data, poseidon.FIELD_FQ)))
+
+    def absorb_nonnative(self, values):
+        """absorb_nonnative_field_elements of canonical Fr values: one call, compressed over its own stream"""
+        self.absorb_native(poseidon.to_mont_words(poseidon.FIELD_FQ, poseidon.nonnative_field_elements(values)))
+
+    def absorb_commitments(self, comms):
+        """absorb_native_field_elements of commitments (normalised projective uint64[k, 18])"""
+        self.absorb_native(_commitment_elements(comms))
+
+    def squeeze(self, counts: list, short: bool = False) -> list:
+        """one squeeze_nonnative_field_elements(n) call (squeeze_short_… when `short`) per entry of `counts`, after everything
+        queued, in one device call → [[canonical Fr] per call]"""
+        kind = poseidon.OP_SQUEEZE_SHORT_NONNATIVE if short else poseidon.OP_SQUEEZE_NONNATIVE
+        width = 168 if short else 252
+        off = 0
+        for n in counts:
+            self._ops.append((kind, n, off))
+            off += n
+            self._advance(False, -(-n * width // (poseidon.FIELDS[poseidon.FIELD_FQ][1] - 1)))
+        ops = torch.from_numpy(np.array(self._ops, dtype=np.int32).reshape(-1, 3)).to(self.dev)
+        start = torch.tensor([0, len(self._ops)], dtype=torch.int32, device=self.dev)
+        inputs = np.concatenate(self._inputs) if self._inputs else np.zeros((0, 12), dtype=np.uint32)
+        _out, fr = device.poseidon_transcripts(poseidon.FIELD_FQ, ops, start, torch.from_numpy(inputs.view(np.int64)).to(self.dev), 0,
+                                               off, self.state)
+        self.calls += 1
+        self._ops, self._inputs, self._nin = [], [], 0
+        vals = [_fr_mont_to_int(row) for row in fr.cpu().numpy().view(np.uint64)] if off else []
+        out, k = [], 0
+        for n in counts:
+            out.append(vals[k: k + n])
+            k += n
+        return out
+
+
+@dataclass
+class Commitments:
+    """data_structures/proof.rs Commitments: normalised projective uint64[18] each, circuits in id order"""
+    witness_commitments: list                  # w of every instance, circuit by circuit
+    mask_poly: np.ndarray | None               # the hiding mode only
+    h_0: np.ndarray
+    g_1: np.ndarray
+    h_1: np.ndarray
+    g_a_commitments: list
+    g_b_commitments: list
+    g_c_commitments: list
+    h_2: np.ndarray
+
+
+@dataclass
+class Evaluations:
+    """data_structures/proof.rs Evaluations: g_1(β) and every circuit's g_a, g_b, g_c at γ, canonical integers"""
+    g_1_eval: int
+    g_a_evals: list
+    g_b_evals: list
+    g_c_evals: list
+
+    def to_field_elements(self) -> list:
+        """the order prove_batch absorbs them in (proof.rs:212-219)"""
+        return [self.g_1_eval] + list(self.g_a_evals) + list(self.g_b_evals) + list(self.g_c_evals)
+
+
+@dataclass
+class Proof:
+    """data_structures/proof.rs Proof, in memory: per circuit (id order) its batch size; the commitments; the evaluations; the third
+    round's sums (per circuit, per instance (sum_a, sum_b, sum_c)) and the fourth round's (per circuit); the BatchLCProof — one
+    (w uint64[18], random_v: Montgomery Fr uint64[4] in the hiding mode, else None) per query point (α, β, γ)."""
+    batch_sizes: list
+    commitments: Commitments
+    evaluations: Evaluations
+    third_sums: list
+    fourth_sums: list
+    pc_proof: list
+
+    def check_batch_sizes(self) -> None:
+        """Proof::check_batch_sizes (proof.rs): every per-instance and per-circuit list matches the batch sizes; ValueError if not"""
+        K, total = len(self.batch_sizes), sum(self.batch_sizes)
+        c, e = self.commitments, self.evaluations
+        if (len(c.witness_commitments) != total or any(b == 0 for b in self.batch_sizes)
+                or not len(c.g_a_commitments) == len(c.g_b_commitments) == len(c.g_c_commitments) == K
+                or not len(e.g_a_evals) == len(e.g_b_evals) == len(e.g_c_evals) == K
+                or [len(s) for s in self.third_sums] != list(self.batch_sizes) or len(self.fourth_sums) != K):
+            raise ValueError("InvalidBatchSize: the proof's lists do not match its batch sizes")
+
+
+def _union_committer_key(cks: list):
+    """CommitterUnionKey::union (sonic_pc/data_structures.rs) of committer keys trimmed from one SRS: the longest powers, every
+    enforced degree bound"""
+    from .sonic_pc import CommitterKey
+    if len(cks) == 1:
+        return cks[0]
+    if len({ck.max_degree for ck in cks}) != 1:
+        raise ValueError("the committer keys come from different universal parameters")
+    longest = max(cks, key=lambda ck: ck.powers_of_beta_g.shape[0])
+    bounds = sorted({b for ck in cks for b in (ck.enforced_degree_bounds or [])})
+    shifted, gamma = None, {}
+    for ck in cks:
+        if ck.enforced_degree_bounds:
+            gamma.update(ck.shifted_powers_of_beta_times_gamma_g)
+            if ck.enforced_degree_bounds[-1] == bounds[-1]:
+                shifted = ck.shifted_powers_of_beta_g
+    return CommitterKey(longest.powers_of_beta_g, longest.powers_of_beta_times_gamma_g, {}, shifted, gamma or None, bounds or None,
+                        longest.max_degree)
+
+
+def _nonzero_vanishing(domain: EvaluationDomain, x: int, name: str):
+    """the verifier's check that v_domain(x) ≠ 0 (verifier.rs:151, 165, 208)"""
+    if _vanish(domain, x) == 0:
+        raise ValueError(f"the vanishing polynomial of the largest domain is zero at {name}")
+
+
+def _public_inputs(prover: "BatchProver") -> list:
+    """every instance's padded public input as canonical integers: per circuit (id order), per instance"""
+    out = []
+    for c, zs in zip(prover.circuits, prover.z):
+        host = device.fr_from_mont(torch.cat([z[: c.num_public] for z in zs])).cpu().numpy().view(np.uint64)
+        vals = [sum(int(v) << (64 * t) for t, v in enumerate(row)) for row in host]
+        out.append([vals[j * c.num_public: (j + 1) * c.num_public] for j in range(len(zs))])
+    return out
+
+
+def _prove_batch(pks_to_assignments: list, zk: bool = False, rng=None):
+    """prove_batch (below) → (Proof, challenges, transcript): challenges is a dict of everything the transcript yielded"""
+    from .sonic_pc import LabeledPolynomial, Randomness, SonicKZG10
+    if not pks_to_assignments:
+        raise ValueError("EmptyBatch: no circuits to prove")
+    if zk and rng is None:
+        rng = random.SystemRandom()
+    prover = BatchProver([(pk.circuit, list(zs)) for pk, zs in pks_to_assignments])
+    pks = [pks_to_assignments[k][0] for k in prover.positions]
+    K, dev = len(pks), prover.dev
+    ck = _union_committer_key([pk.committer_key for pk in pks])
+    rand_fr = lambda n: [rng.randrange(R_MOD) for _ in range(n)]          # noqa: E731
+
+    # init_sponge (varuna.rs:136-153)
+    transcript = Transcript(dev)
+    transcript.absorb_bytes(PROTOCOL_NAME)
+    for b, inputs in zip(prover.batch, _public_inputs(prover)):
+        transcript.absorb_bytes(struct.pack("<Q", b))
+        for x in inputs:
+            transcript.absorb_nonnative(x)
+    for pk in pks:
+        transcript.absorb_commitments(pk.circuit_verifying_key.circuit_commitments)
+
+    def commit(labeled):
+        blind = [None if lp.hiding_bound is None else
+                 torch.from_numpy(np.array([_mont(v) for v in rand_fr(lp.hiding_bound + 2)], dtype=np.uint64).view(np.int64)).to(dev)
+                 for lp in labeled]
+        comms, rands = SonicKZG10.commit(ck, labeled, blind)
+        return list(comms), list(rands)
+
+    label = prover._labels()
+    rounds = {}
+
+    def round_commit(r):
+        rounds[r] = prover.labeled_oracles(zk, label, rounds=(r,))[r]
+        return commit(rounds[r])
+
+    # round 1
+    if zk:
+        prover.set_mask_poly(rand_fr(4), rand_fr(6))
+    prover.first_round()
+    prover.assignments()
+    c1, r1 = round_commit(1)
+    transcript.absorb_commitments(np.stack(c1))
+    elems = transcript.squeeze([b - 1 + (1 if i else 0) for i, b in enumerate(prover.batch)])
+    combs = [(e[b - 1] if i else 1, [1] + e[: b - 1]) for i, (b, e) in enumerate(zip(prover.batch, elems))]
+    # round 2
+    prover.second_round(combs)
+    c2, r2 = round_commit(2)
+    transcript.absorb_commitments(np.stack(c2))
+    alpha, eta_b, eta_c = transcript.squeeze([3])[0]
+    _nonzero_vanishing(prover.max_constraint_domain, alpha, "α")
+    # round 3
+    prover.third_round(alpha, eta_b, eta_c, combs)
+    c3, r3 = round_commit(3)
+    transcript.absorb_commitments(np.stack(c3))
+    for sums in prover.third_sums:
+        for s in sums:
+            transcript.absorb_nonnative(s)
+    beta = transcript.squeeze([1])[0][0]
+    _nonzero_vanishing(prover.max_variable_domain, beta, "β")
+    # round 4
+    prover.fourth_round(alpha, beta)
+    c4, r4 = round_commit(4)
+    transcript.absorb_commitments(np.stack(c4))
+    for s in prover.fourth_sums:
+        transcript.absorb_nonnative(s)
+    d = transcript.squeeze([2] + [3] * (K - 1))
+    deltas = [[1] + d[0]] + d[1:]
+    # round 5
+    prover.fifth_round(deltas)
+    c5, r5 = round_commit(5)
+    transcript.absorb_commitments(np.stack(c5))
+    gamma = transcript.squeeze([1])[0][0]
+    _nonzero_vanishing(prover.max_non_zero_domain, gamma, "γ")
+
+    lcs, query_set = prover.linear_combinations(alpha, eta_b, eta_c, beta, deltas, gamma, combs, label)
+    evaluations = Evaluations(BatchProver._eval(prover.g_1, beta), *([BatchProver._eval(gs[m], gamma) for gs in prover.gs] for m in range(3)))
+    transcript.absorb_nonnative(evaluations.to_field_elements())
+    # open_combinations: per point (by name), one short challenge per linear combination opened there, then `_randomizer`
+    per_point = {}
+    for _lc, (point_name, _x) in query_set:
+        per_point[point_name] = per_point.get(point_name, 0) + 1
+    opening = [x for [x] in transcript.squeeze([1] * sum(n + 1 for n in per_point.values()), short=True)]
+    polys = prover.polynomials(label)
+    ab = [LabeledPolynomial(k, v, None, None) for k, v in polys.items() if "_a_poly_" in k or "_b_poly_" in k]
+    labeled = ab + [lp for r in sorted(rounds) for lp in rounds[r]]
+    rands = [Randomness() for _ in ab] + r1 + r2 + r3 + r4 + r5
+    pc_proof = SonicKZG10.open_combinations(ck, lcs, labeled, rands, query_set, iter(opening))
+
+    nw = sum(prover.batch)
+    gs = [c4[3 * i: 3 * i + 3] for i in range(K)]
+    commitments = Commitments(c1[:nw], c1[nw] if zk else None, c2[0], c3[0], c3[1], [g[0] for g in gs], [g[1] for g in gs],
+                              [g[2] for g in gs], c5[0])
+    proof = Proof(list(prover.batch), commitments, evaluations, [[list(s) for s in sums] for sums in prover.third_sums],
+                  [list(s) for s in prover.fourth_sums], pc_proof)
+    proof.check_batch_sizes()
+    challenges = {"batch_combiners": combs, "alpha": alpha, "eta_b": eta_b, "eta_c": eta_c, "beta": beta, "deltas": deltas,
+                  "gamma": gamma, "opening": opening}
+    return proof, challenges, transcript
+
+
+def prove_batch(pks_to_assignments: list, zk: bool = False, rng=None) -> Proof:
+    """VarunaSNARK::prove_batch (varuna.rs:336-620) → Proof.  `pks_to_assignments`: [(CircuitProvingKey, [assignment, …])], an
+    assignment as BatchProver takes it; the circuits are proved in id order, so the order of the list changes nothing.  Every
+    challenge comes from the prover's own Fiat–Shamir transcript (PoseidonSponge<Fq, 2, 1>, one device call per round):
+        init_sponge      the protocol name; per circuit its batch size (u64 LE) and each instance's padded public input (nonnative);
+                         every circuit's twelve vk commitments
+        round 1          w of every instance (and mask_poly) → per circuit batch_size − 1 (+ 1 after the first circuit) combiners
+        round 2          h_0 → α, η_b, η_c          round 3   g_1, h_1, every instance's sums → β
+        round 4          every g_a, g_b, g_c, every circuit's sums → δ (two for the first circuit, three for each further one)
+        round 5          h_2 → γ
+        openings         the evaluations (nonnative) → per query point one short challenge per linear combination, then the randomizer
+    The vanishing polynomial of the largest constraint, variable and non-zero domain must not vanish at α, β and γ (ValueError).
+    The committer key is the union of the proving keys' keys.  In the hiding mode (zk) the mask polynomial (4 then 6 coefficients)
+    and each hiding commitment's blinding polynomial (3 coefficients, in commitment order) are drawn from `rng` (anything with
+    randrange; a SystemRandom when None).  That stream cannot equal the reference's ChaCha stream, so a hiding proof is valid but not
+    the reference's bytes; a non-hiding proof is deterministic."""
+    return _prove_batch(pks_to_assignments, zk, rng)[0]
