@@ -535,6 +535,16 @@ SNARKVM_API int snarkvm_b200_poseidon_transcripts_resume_device(int field, const
                                                                 const void* d_in, size_t nin, void* d_out, size_t nout, void* d_out_fr,
                                                                 size_t nout_fr, void* d_state, int64_t* bad_transcript, void* stream);
 
+/* Validation of G1 points taken from outside (Affine::check of the reference: curves/src/bls12_377/g1.rs:98-106).  d_points holds n
+ * Affine<G1> images (x, y Montgomery Fq, infinity flag; stride ≥ 104, a multiple of 8, 8-byte aligned); d_status[i] (device int32)
+ * receives point i's status: VALID (the point at infinity included), NOT_CANONICAL (a coordinate image not below q), NOT_ON_CURVE
+ * (y² ≠ x³ + 1) or NOT_IN_SUBGROUP ([x²]·φ(P) + P ≠ O, x the BLS parameter, φ(x, y) = (PHI·x, y)), the first test that fails.  One
+ * launch, one thread per point, no synchronisation. */
+enum {
+    SNARKVM_B200_G1_VALID = 0, SNARKVM_B200_G1_NOT_CANONICAL = 1, SNARKVM_B200_G1_NOT_ON_CURVE = 2, SNARKVM_B200_G1_NOT_IN_SUBGROUP = 3
+};
+SNARKVM_API int snarkvm_b200_g1_validate_device(int32_t* d_status, const void* d_points, size_t n, size_t stride, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

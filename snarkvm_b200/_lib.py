@@ -39,7 +39,7 @@ SYMBOLS = (
     "snarkvm_b200_fr_lincomb_terms_device", "snarkvm_b200_sparse_matvec_batch_device", "snarkvm_b200_polymul_batch_device",
     "snarkvm_b200_varuna_round4_evals_device", "snarkvm_b200_g2_prepare_device", "snarkvm_b200_pairing_products_device",
     "snarkvm_b200_test_tower_op_device", "snarkvm_b200_poseidon_transcripts_device",
-    "snarkvm_b200_poseidon_transcripts_resume_device",
+    "snarkvm_b200_poseidon_transcripts_resume_device", "snarkvm_b200_g1_validate_device",
 )
 
 
@@ -187,6 +187,7 @@ def lib():
     L.snarkvm_b200_poseidon_transcripts_device.argtypes = [i32, vp, vp, vp, sz, sz, vp, sz, vp, sz, vp, sz, ctypes.POINTER(ctypes.c_int64), vp]
     L.snarkvm_b200_poseidon_transcripts_resume_device.argtypes = [i32, vp, vp, vp, sz, sz, vp, sz, vp, sz, vp, sz, vp,
                                                                   ctypes.POINTER(ctypes.c_int64), vp]
+    L.snarkvm_b200_g1_validate_device.argtypes = [vp, vp, sz, sz, vp]
     L.snarkvm_b200_msm_batch_device.argtypes = [vp, vp, sz, vp, vp, sz, vp]
     L.snarkvm_b200_msm_window_sums_plan_device.argtypes = [vp, vp, sz, vp, sz, vp, sz, vp]
     L.snarkvm_b200_kzg_commit_batch_hiding_device.argtypes = [vp, vp, sz, vp, vp, vp, vp, vp, sz, vp]

@@ -93,6 +93,14 @@ FF_DEV void store_affine(uint8_t* base, size_t stride, size_t i, const AffinePoi
     *reinterpret_cast<unsigned long long*>(p + 96) = a.inf ? 1ull : 0ull;
 }
 
+// a < q on the raw limbs: a coordinate image ≥ q is no field element
+FF_DEV bool fq_is_canonical(const Fq& a) {
+    (void)ptx_sub_cc(a.v[0], FqParams::mod(0));
+#pragma unroll
+    for (int i = 1; i < 12; i++) (void)ptx_subc_cc(a.v[i], FqParams::mod(i));
+    return ptx_subc(0u, 0u) != 0u;
+}
+
 template <class F>
 struct XyzzT {
     F X, Y, ZZ, ZZZ;

@@ -32,14 +32,6 @@ static constexpr uint32_t NO_BAD = 0xffffffffu;
 __constant__ uint32_t G2_B1[12] = {0x66666685u, 0x80722666u, 0x899999a9u, 0x8df55926u, 0xd64f34cfu, 0x7fe4561au,
                                    0xb6e4f01bu, 0xb95da6d8u, 0xfc142743u, 0x4b747cccu, 0x70f49f43u, 0x0039c3fau};
 
-// a < q on the raw limbs: a coordinate image ≥ q is no field element
-FF_DEV bool fq_is_canonical(const Fq& a) {
-    (void)ptx_sub_cc(a.v[0], FqParams::mod(0));
-#pragma unroll
-    for (int i = 1; i < 12; i++) (void)ptx_subc_cc(a.v[i], FqParams::mod(i));
-    return ptx_subc(0u, 0u) != 0u;
-}
-
 struct G2Hom { Fq2 x, y, z; };
 
 // (0, b1)·a = (−5·b1·a1, b1·a0)

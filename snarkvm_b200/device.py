@@ -165,6 +165,20 @@ def pairing_products(g1: torch.Tensor, g2_index: torch.Tensor, prepared: torch.T
     return (gt, is_one.bool(), mv) if miller else (gt, is_one.bool())
 
 
+G1_VALID, G1_NOT_CANONICAL, G1_NOT_ON_CURVE, G1_NOT_IN_SUBGROUP = 0, 1, 2, 3
+
+
+def g1_validate(points: torch.Tensor, stride: int = AFFINE_STRIDE) -> torch.Tensor:
+    """Affine::check of every Affine<G1> image in HBM (snarkvm_b200_g1_validate_device) → int32 status per point in HBM: G1_VALID
+    (infinity included), G1_NOT_CANONICAL (a coordinate image ≥ q), G1_NOT_ON_CURVE or G1_NOT_IN_SUBGROUP, the first test failed."""
+    n = _nbytes(points) // stride
+    status = torch.empty(n, dtype=torch.int32, device=points.device)
+    if n:
+        with torch.cuda.device(points.device):
+            _lib.check(_lib.lib().snarkvm_b200_g1_validate_device(status.data_ptr(), _check(points, "points"), n, stride, _stream()))
+    return status
+
+
 POSEIDON_ABSORB, POSEIDON_SQUEEZE, POSEIDON_SQUEEZE_NONNATIVE, POSEIDON_SQUEEZE_SHORT_NONNATIVE = 0, 1, 2, 3
 
 

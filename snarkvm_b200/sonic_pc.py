@@ -6,6 +6,8 @@ Mirror of /root/reference/algorithms/src/polycommit/sonic_pc:
     mod.rs:259-284    combine_for_open      SonicKZG10.combine_for_open
     mod.rs:286-342    batch_open            SonicKZG10.batch_open
     mod.rs:413-475    open_combinations     SonicKZG10.open_combinations
+    mod.rs:344-411, 477-544, 582-677   check_combinations → batch_check → accumulate_elems → check_elems' inputs as scalars
+                                       check_combinations_scalars
     data_structures.rs:310-341   shifted_powers_of_beta_g / lagrange_basis
 and of kzg10/mod.rs:98-156 (commit), :220-277 (open) through algorithms.KZG10.
 
@@ -249,6 +251,51 @@ class SonicKZG10:
             lc_polys.append(LabeledPolynomial(lc_label, poly if poly is not None else _zeros(0, dev), degree_bound, hiding_bound))
             lc_rands.append(rand)
         return SonicKZG10.batch_open(ck, lc_polys, query_set, lc_rands, challenges)
+
+
+def check_combinations_scalars(linear_combinations: list, query_set: list, evaluations: dict, degree_bounds: dict, random_vs: list,
+                               challenges) -> dict:
+    """check_combinations (mod.rs:477-544) → batch_check (:344-411) → accumulate_elems (:582-635), with every G1 sum kept as one scalar
+    per base point, so that a caller runs check_elems' MSMs (:637-677) as one pass.  linear_combinations: [(lc label, [(coefficient,
+    base label or None for LCTerm::One)])]; query_set: [(lc label, (point name, point))]; evaluations: {lc label: value at its point};
+    degree_bounds: {base label: bound} of the bounded commitments; random_vs: per point name in sorted order, the opening's random_v
+    (canonical) or None; `challenges` yields the sponge's short squeezes in order.  The opening witness of the q-th point is the base
+    "w_{q}", G is "g" and γ·G "gamma_g".  → {degree bound or None: {base label: scalar}, "witness": {base label: scalar}}: the
+    None group already minus the combined adjusted witness (both pair with H), "witness" the negated combined witness (it pairs
+    with β·H), each bounded group pairing with its negative power of β·H."""
+    terms, values = {}, {}
+    for lc_label, lc in linear_combinations:
+        bounded = [lab for _k, lab in lc if lab in degree_bounds]
+        if bounded and (len(lc) != 1 or lc[0][0] % _R_MOD != 1):
+            raise ValueError(f"EquationHasDegreeBounds({lc_label})")
+        terms[lc_label] = [(k, lab) for k, lab in lc if lab is not None]
+        # LCTerm::One moves into the evaluation (mod.rs:504-510)
+        values[lc_label] = (evaluations[lc_label] - sum(k for k, lab in lc if lab is None)) % _R_MOD
+    by_point = {}
+    for lc_label, (name, z) in query_set:
+        by_point.setdefault(name, (z, []))[1].append(lc_label)
+    if len(by_point) != len(random_vs):
+        raise ValueError(f"{len(random_vs)} openings for {len(by_point)} query points")
+    groups, witness, r = {None: {}}, {}, 1
+
+    def add(group, label, v):
+        group[label] = (group.get(label, 0) + v) % _R_MOD
+    for q, name in enumerate(sorted(by_point)):
+        z, labels = by_point[name]
+        combined = 0
+        for lc_label in sorted(labels):
+            challenge = int(next(challenges))
+            combined += challenge * values[lc_label]
+            for k, lab in terms[lc_label]:
+                add(groups.setdefault(degree_bounds.get(lab), {}), lab, r * challenge % _R_MOD * k)
+        none = groups[None]
+        add(none, "g", -r * combined)
+        add(none, f"w_{q}", r * z)
+        if random_vs[q] is not None:
+            add(none, "gamma_g", -r * random_vs[q])
+        witness[f"w_{q}"] = (-r) % _R_MOD
+        r = int(next(challenges))
+    return {**groups, "witness": witness}
 
 
 def synthetic_srs(max_degree: int, beta: int, gamma: int, dev="cuda"):

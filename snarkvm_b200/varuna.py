@@ -45,6 +45,7 @@ from . import device, poseidon
 from ._lib import CudaError
 from .algorithms import EvaluationDomain, _fr_int_to_mont, _fr_mont_to_int
 from .cuda import NTTDirection, NTTType
+from .sonic_pc import check_combinations_scalars
 
 R_MOD = 8444461749428370424248824938781546531375899335154063827935233455917409239041   # curves/src/bls12_377/fr.rs:138-145
 
@@ -584,44 +585,123 @@ def _g2_affine(p) -> np.ndarray:
     return out
 
 
-class UniversalVerifier:
-    """The pairing half of the universal verifier (kzg10/data_structures.rs UniversalParams: h, prepared_h, prepared_beta_h; g is
-    the first power of β·G): g as a 104-byte Affine<G1> image, h (the G2 generator) and β·h as 200-byte Affine<G2> images, and
-    `prepared`, h and β·h prepared once on the device ([2, device.G2_PREPARED_BYTES], h first)."""
+def _g1_affine(p) -> np.ndarray:
+    """(x, y) of plain integers, or None → the 104-byte Affine<G1> image (Montgomery; Affine::zero() = (0, 1, true))"""
+    (x, y), inf = ((0, 1), 1) if p is None else (p, 0)
+    out = np.zeros(104, dtype=np.uint8)
+    out[:96] = np.frombuffer(b"".join((v * _FQ_R % Q_MOD).to_bytes(48, "little") for v in (x, y)), dtype=np.uint8)
+    out[96] = inf
+    return out
 
-    def __init__(self, beta_h: np.ndarray, device_="cuda"):
+
+def _parse_g1(blob: bytes, what: str) -> np.ndarray:
+    """a 96-byte uncompressed G1 point (x, y 48 B LE each; bit 6 of the last byte = infinity, bit 7 = y's sign,
+    utilities/src/serialize/flags.rs) → its Affine image; a coordinate ≥ q raises ValueError"""
+    b = bytearray(blob)
+    infinity = bool(b[95] & 0x40)
+    b[95] &= 0x3F
+    v = [int.from_bytes(bytes(b[48 * i: 48 * i + 48]), "little") for i in range(2)]
+    if any(x >= Q_MOD for x in v):
+        raise ValueError(f"a coordinate of {what} is not below q")
+    return _g1_affine(None if infinity else (v[0], v[1]))
+
+
+def _parse_g2(blob: bytes, what: str) -> np.ndarray:
+    """a 192-byte uncompressed G2 point (x.c0, x.c1, y.c0, y.c1, 48 B LE each; the flags in the last byte) → its Affine image; a
+    coordinate ≥ q raises ValueError"""
+    if len(blob) != 192:
+        raise ValueError(f"a G2 point is 192 bytes, not {len(blob)}")
+    b = bytearray(blob)
+    infinity = bool(b[191] & 0x40)
+    b[191] &= 0x3F
+    v = [int.from_bytes(bytes(b[48 * i: 48 * i + 48]), "little") for i in range(4)]
+    if any(x >= Q_MOD for x in v):
+        raise ValueError(f"a coordinate of {what} is not below q")
+    return _g2_affine(None if infinity else ((v[0], v[1]), (v[2], v[3])))
+
+
+def _u64_map(blob: bytes, entry: int, what: str) -> list:
+    """a serialised BTreeMap<usize, point>: a u64 count, then (u64 key, `entry` bytes) per entry → [(key, bytes)]"""
+    if len(blob) < 8:
+        raise ValueError(f"{what}: no entry count")
+    (n,) = struct.unpack_from("<Q", blob, 0)
+    if len(blob) != 8 + n * (8 + entry):
+        raise ValueError(f"{what}: {len(blob)} bytes do not hold {n} entries of {8 + entry} bytes")
+    out = []
+    for k in range(n):
+        off = 8 + k * (8 + entry)
+        out.append((struct.unpack_from("<Q", blob, off)[0], blob[off + 8: off + 8 + entry]))
+    return out
+
+
+def parse_neg_powers(blob: bytes) -> dict:
+    """`neg-powers-of-beta.usrs` (a BTreeMap<usize, G2Affine>) → {degree bound: 200-byte Affine<G2> image of β^{-(D − d)}·H}"""
+    return {d: _parse_g2(p, f"the negative power for bound {d}") for d, p in _u64_map(blob, 192, "negative powers of β·H")}
+
+
+def parse_gamma_powers(blob: bytes) -> dict:
+    """`powers-of-beta-gamma.usrs` (a BTreeMap<usize, G1Affine>) → {i: 104-byte Affine<G1> image of γβ^i·G}"""
+    return {i: _parse_g1(p, f"γβ^{i}·G") for i, p in _u64_map(blob, 96, "powers of β·γ·G")}
+
+
+class UniversalVerifier:
+    """The pairing half of the universal verifier (kzg10/data_structures.rs UniversalParams: h, prepared_h, prepared_beta_h,
+    gamma_g, prepared_negative_powers_of_beta_h; g is the first power of β·G): g and gamma_g (γ·G, None when unknown) as 104-byte
+    Affine<G1> images, h (the G2 generator) and β·h as 200-byte Affine<G2> images, and `prepared`, h, β·h and then the negative
+    powers of β·H in increasing degree bound, prepared once on the device ([2 + bounds, device.G2_PREPARED_BYTES]).
+    `neg_index` maps each degree bound d to the row of `prepared` that holds β^{-(D − d)}·H, D the SRS's maximum degree."""
+
+    def __init__(self, beta_h: np.ndarray, device_="cuda", gamma_g: np.ndarray | None = None, neg_powers: dict | None = None):
         dev = torch.device(device_)
         self.h = _g2_affine(G2_GENERATOR)
         self.beta_h = np.ascontiguousarray(beta_h, dtype=np.uint8).reshape(200)
         self.g = device.generator_mul(torch.from_numpy(np.array([[1, 0, 0, 0]], dtype=np.uint64).view(np.int64)).to(dev)).cpu().numpy()[0]
-        self.prepared = device.g2_prepare(torch.from_numpy(np.stack([self.h, self.beta_h])).to(dev))
+        self.gamma_g = None if gamma_g is None else np.ascontiguousarray(gamma_g, dtype=np.uint8).reshape(104)
+        bounds = sorted(neg_powers or {})
+        self.neg_index = {d: 2 + k for k, d in enumerate(bounds)}
+        g2 = [self.h, self.beta_h] + [np.ascontiguousarray(neg_powers[d], dtype=np.uint8).reshape(200) for d in bounds]
+        self.prepared = device.g2_prepare(torch.from_numpy(np.stack(g2)).to(dev))
         self.device = self.prepared.device
 
     @classmethod
     def from_usrs(cls, blob: bytes, device_="cuda") -> "UniversalVerifier":
         """β·H from the mainnet `beta-h.usrs` bytes: x.c0, x.c1, y.c0, y.c1 (48 B LE each), bit 6 of the last byte = infinity and
         bit 7 = y's sign (utilities/src/serialize/flags.rs).  A coordinate ≥ q raises ValueError."""
-        if len(blob) != 192:
-            raise ValueError(f"a G2 point is 192 bytes, not {len(blob)}")
-        b = bytearray(blob)
-        infinity = bool(b[191] & 0x40)
-        b[191] &= 0x3F
-        v = [int.from_bytes(bytes(b[48 * i: 48 * i + 48]), "little") for i in range(4)]
-        if any(x >= Q_MOD for x in v):
-            raise ValueError("a coordinate of β·H is not below q")
-        return cls(_g2_affine(None if infinity else ((v[0], v[1]), (v[2], v[3]))), device_)
+        return cls(_parse_g2(blob, "β·H"), device_)
 
     @classmethod
-    def synthetic(cls, beta: int, device_="cuda") -> "UniversalVerifier":
-        """the verifier of a setup with a known β (sonic_pc.synthetic_srs): β·H by the G2 MSM of one point"""
+    def from_mainnet(cls, beta_h: bytes, neg_powers: bytes, gamma_powers: bytes, device_="cuda") -> "UniversalVerifier":
+        """the mainnet verifier from the bytes of `beta-h.usrs`, `neg-powers-of-beta.usrs` (every degree bound 2^k − 2 with its
+        β^{-(D − d)}·H) and `powers-of-beta-gamma.usrs` (its key 0 is γ·G).  A coordinate ≥ q raises ValueError."""
+        gammas = parse_gamma_powers(gamma_powers)
+        if 0 not in gammas:
+            raise ValueError("the powers of β·γ·G hold no γ·G")
+        return cls(_parse_g2(beta_h, "β·H"), device_, gammas[0], parse_neg_powers(neg_powers))
+
+    @classmethod
+    def synthetic(cls, beta: int, device_="cuda", max_degree: int | None = None, gamma: int | None = None,
+                  bounds=()) -> "UniversalVerifier":
+        """the verifier of a setup with a known β (sonic_pc.synthetic_srs): β·H by the G2 MSM of one point; with `gamma`, γ·G; for
+        each degree bound d of `bounds`, β^{-(max_degree − d)}·H by the same G2 MSM (max_degree: the SRS's highest power of β)"""
         dev = torch.device(device_)
         beta %= R_MOD
-        scalar = torch.from_numpy(np.array([[(beta >> (64 * i)) & (2**64 - 1) for i in range(4)]], dtype=np.uint64).view(np.int64)).to(dev)
-        proj = device.msm_g2(torch.from_numpy(_g2_affine(G2_GENERATOR)[None]).to(dev), scalar)       # normalised: (x, y, 1) or (0, 1, 0)
-        img = np.zeros(200, dtype=np.uint8)
-        img[:192] = proj[:24].view(np.uint8)
-        img[192] = 0 if proj[24:].any() else 1
-        return cls(img, device_)
+
+        def g2_mul(k: int) -> np.ndarray:
+            scalar = torch.from_numpy(np.array([[(k >> (64 * i)) & (2**64 - 1) for i in range(4)]], dtype=np.uint64).view(np.int64)).to(dev)
+            proj = device.msm_g2(torch.from_numpy(_g2_affine(G2_GENERATOR)[None]).to(dev), scalar)   # normalised: (x, y, 1) or (0, 1, 0)
+            img = np.zeros(200, dtype=np.uint8)
+            img[:192] = proj[:24].view(np.uint8)
+            img[192] = 0 if proj[24:].any() else 1
+            return img
+        if bounds and max_degree is None:
+            raise ValueError("negative powers of β·H need the SRS's max_degree")
+        neg = {int(d): g2_mul(pow(beta, -(max_degree - int(d)), R_MOD)) for d in bounds}
+        gamma_g = None
+        if gamma is not None:
+            k = gamma % R_MOD
+            scal = torch.from_numpy(np.array([[(k >> (64 * i)) & (2**64 - 1) for i in range(4)]], dtype=np.uint64).view(np.int64)).to(dev)
+            gamma_g = device.generator_mul(scal).cpu().numpy()[0]
+        return cls(g2_mul(beta), device_, gamma_g, neg)
 
 
 def _affine(projective: np.ndarray) -> np.ndarray:
@@ -984,13 +1064,7 @@ class BatchProver:
     def _labels(self):
         """label(i, name, j) of circuit i's polynomial: the reference's witness_label names (ahp.rs:46-50; a_poly / b_poly as
         construct_matrix_linear_combinations names them, ahp.rs:408-409)"""
-        ids = circuit_ids(self.circuits)
-
-        def label(i, name, j=0):
-            if name in ("a_poly", "b_poly"):
-                return f"circuit_{ids[i].hex()}_{name}_{'abc'[j]}"
-            return witness_label(ids[i], name, j)
-        return label
+        return _label_fn(circuit_ids(self.circuits))
 
     def polynomials(self, label=None) -> dict:
         """label → device polynomial, everything prove_batch hands to open_combinations, in its order (varuna.rs:509-517): the a and b
@@ -1050,54 +1124,69 @@ class BatchProver:
         return _fr_mont_to_int(device.poly_evaluate(poly.contiguous(), _mont(point))) if poly.shape[0] else 0
 
     def linear_combinations(self, alpha, eta_b, eta_c, beta, deltas, gamma, batch_combiners=None, label=None):
-        """AHPForR1CS::construct_linear_combinations (ahp/ahp.rs:172-389) and the verifier's query set for K circuits → (lcs, query_set):
-        lcs = [(label, [(coefficient, polynomial label or None for LCTerm::One)])] in the reference's BTreeMap order, query_set =
-        [(lc label, (point name, point))].  Each circuit's terms are scaled by the selector of its domain inside the max domain at α, β
-        and γ.  The coefficients are host integers; the evaluations they need (g_1(β), g_M(γ), x(β)) are device Horner passes."""
-        combs = self._combiners(batch_combiners)
-        label = label or self._labels()
-        cs = self.circuits
-        R, C, K = self.max_constraint_domain, self.max_variable_domain, self.max_non_zero_domain
-        lcs = {}
-        const = 0
-        for c, (cc, inst), sums in zip(cs, combs, self.third_sums):
-            term = sum(comb * (s[0] * s[1] - s[2]) for comb, s in zip(inst, sums)) % R_MOD
-            const = (const + cc * _selector(R, c.constraint_domain, alpha) % R_MOD * term) % R_MOD
-        lcs["rowcheck_zerocheck"] = [(const, None), ((-_vanish(R, alpha)) % R_MOD, "h_0")]
-        lcs["g_1"] = [(1, "g_1")]
-        g_1_at_beta = self._eval(self.g_1, beta)
-        lineval = [(1, "mask_poly")] if self.mask_poly is not None else []
-        batch_lineval_sum = 0
-        for i, (c, (cc, inst)) in enumerate(zip(cs, combs)):
-            sums4 = [s * a.domain.size % R_MOD for s, a in zip(self.fourth_sums[i], c.ariths)]
-            weight = (sums4[0] + sums4[1] * eta_b + sums4[2] * eta_c) % R_MOD
-            v_x_beta, sel = _vanish(c.input_domain, beta), _selector(C, c.variable_domain, beta)
-            for j, comb in enumerate(inst):
-                k = cc * comb % R_MOD * sel % R_MOD
-                lineval.append((k * weight % R_MOD * self._eval(self.x_polys[i][j], beta) % R_MOD, None))
-                lineval.append((k * weight % R_MOD * v_x_beta % R_MOD, label(i, "w", j)))
-            batch_lineval_sum += cc * sum(comb * (s[0] + eta_b * s[1] + eta_c * s[2]) for comb, s in zip(inst, self.third_sums[i]))
-        batch_lineval_sum = batch_lineval_sum % R_MOD * pow(C.size, -1, R_MOD) % R_MOD
-        lineval += [((-_vanish(C, beta)) % R_MOD, "h_1"), ((-beta * g_1_at_beta) % R_MOD, None), ((-batch_lineval_sum) % R_MOD, None)]
-        lcs["lineval_sumcheck"] = lineval
-        if len(deltas) != len(cs) or any(len(d) != 3 for d in deltas):
-            raise ValueError(f"one (δ_a, δ_b, δ_c) per circuit: {len(cs)} circuits")
-        points = {"rowcheck_zerocheck": ("alpha", alpha), "g_1": ("beta", beta), "lineval_sumcheck": ("beta", beta),
-                  "matrix_sumcheck": ("gamma", gamma)}
-        matrix = []
-        for i, c in enumerate(cs):
-            for m, (g, s, delta, a) in enumerate(zip(self.gs[i], self.fourth_sums[i], deltas[i], c.ariths)):
-                g_label = label(i, f"g_{'abc'[m]}", 0)
-                lcs[g_label] = [(1, g_label)]
-                points[g_label] = ("gamma", gamma)
-                selector = _selector(K, a.domain, gamma)
-                b_term = (gamma * self._eval(g, gamma) + s) % R_MOD
-                matrix.append((delta * selector % R_MOD, label(i, "a_poly", m)))
-                matrix.append(((-delta * selector % R_MOD * b_term) % R_MOD, label(i, "b_poly", m)))
-        matrix.append(((-_vanish(K, gamma)) % R_MOD, "h_2"))
-        lcs["matrix_sumcheck"] = matrix
-        order = sorted(lcs)
-        return [(k, lcs[k]) for k in order], [(k, points[k]) for k in order]
+        """AHPForR1CS::construct_linear_combinations (ahp/ahp.rs:172-389) on the prover's side and the query set for K circuits
+        (linear_combinations below), with the evaluations it needs (g_1(β), g_M(γ), x(β)) from device Horner passes"""
+        if len(deltas) != len(self.circuits) or any(len(d) != 3 for d in deltas):
+            raise ValueError(f"one (δ_a, δ_b, δ_c) per circuit: {len(self.circuits)} circuits")
+        return linear_combinations(self.circuits, self._combiners(batch_combiners), self.third_sums, self.fourth_sums,
+                                   (alpha, eta_b, eta_c, beta, deltas, gamma), self._eval(self.g_1, beta),
+                                   [[self._eval(g, gamma) for g in gs] for gs in self.gs],
+                                   [[self._eval(x, beta) for x in xs] for xs in self.x_polys], label or self._labels(),
+                                   self.mask_poly is not None)
+
+
+def linear_combinations(circuits: list, combs: list, third_sums: list, fourth_sums: list, challenges: tuple, g_1_at_beta: int,
+                        g_at_gamma: list, x_at_beta: list, label, mask: bool):
+    """AHPForR1CS::construct_linear_combinations (ahp/ahp.rs:172-389) and the verifier's query set for K circuits → (lcs, query_set):
+    lcs = [(label, [(coefficient, polynomial label or None for LCTerm::One)])] in the reference's BTreeMap order, query_set =
+    [(lc label, (point name, point))].  Only numbers go in, so the prover and the verifier share it: per circuit (id order) its
+    domains (`circuits[i]` has constraint_domain, variable_domain, input_domain and non_zero_domains), (circuit combiner, instance
+    combiners), third sums (per instance) and fourth sums; challenges = (α, η_b, η_c, β, [(δ_a, δ_b, δ_c)], γ); g_1(β); per
+    circuit (g_a(γ), g_b(γ), g_c(γ)); per circuit, per instance x(β).  Each circuit's terms are scaled by the selector of its
+    domain inside the max domain at α, β and γ.  The matrix sumcheck names each circuit's a_poly / b_poly (the prover's
+    polynomials; the verifier expands them into index commitments, ahp.rs:408-445)."""
+    alpha, eta_b, eta_c, beta, deltas, gamma = challenges
+    cs = circuits
+    R = _largest(c.constraint_domain for c in cs)
+    C = _largest(c.variable_domain for c in cs)
+    K = _largest(d for c in cs for d in c.non_zero_domains)
+    lcs = {}
+    const = 0
+    for c, (cc, inst), sums in zip(cs, combs, third_sums):
+        term = sum(comb * (s[0] * s[1] - s[2]) for comb, s in zip(inst, sums)) % R_MOD
+        const = (const + cc * _selector(R, c.constraint_domain, alpha) % R_MOD * term) % R_MOD
+    lcs["rowcheck_zerocheck"] = [(const, None), ((-_vanish(R, alpha)) % R_MOD, "h_0")]
+    lcs["g_1"] = [(1, "g_1")]
+    lineval = [(1, "mask_poly")] if mask else []
+    batch_lineval_sum = 0
+    for i, (c, (cc, inst)) in enumerate(zip(cs, combs)):
+        sums4 = [s * d.size % R_MOD for s, d in zip(fourth_sums[i], c.non_zero_domains)]
+        weight = (sums4[0] + sums4[1] * eta_b + sums4[2] * eta_c) % R_MOD
+        v_x_beta, sel = _vanish(c.input_domain, beta), _selector(C, c.variable_domain, beta)
+        for j, comb in enumerate(inst):
+            k = cc * comb % R_MOD * sel % R_MOD
+            lineval.append((k * weight % R_MOD * x_at_beta[i][j] % R_MOD, None))
+            lineval.append((k * weight % R_MOD * v_x_beta % R_MOD, label(i, "w", j)))
+        batch_lineval_sum += cc * sum(comb * (s[0] + eta_b * s[1] + eta_c * s[2]) for comb, s in zip(inst, third_sums[i]))
+    batch_lineval_sum = batch_lineval_sum % R_MOD * pow(C.size, -1, R_MOD) % R_MOD
+    lineval += [((-_vanish(C, beta)) % R_MOD, "h_1"), ((-beta * g_1_at_beta) % R_MOD, None), ((-batch_lineval_sum) % R_MOD, None)]
+    lcs["lineval_sumcheck"] = lineval
+    points = {"rowcheck_zerocheck": ("alpha", alpha), "g_1": ("beta", beta), "lineval_sumcheck": ("beta", beta),
+              "matrix_sumcheck": ("gamma", gamma)}
+    matrix = []
+    for i, c in enumerate(cs):
+        for m, (g_at, s, delta, d) in enumerate(zip(g_at_gamma[i], fourth_sums[i], deltas[i], c.non_zero_domains)):
+            g_label = label(i, f"g_{'abc'[m]}", 0)
+            lcs[g_label] = [(1, g_label)]
+            points[g_label] = ("gamma", gamma)
+            selector = _selector(K, d, gamma)
+            b_term = (gamma * g_at + s) % R_MOD
+            matrix.append((delta * selector % R_MOD, label(i, "a_poly", m)))
+            matrix.append(((-delta * selector % R_MOD * b_term) % R_MOD, label(i, "b_poly", m)))
+    matrix.append(((-_vanish(K, gamma)) % R_MOD, "h_2"))
+    lcs["matrix_sumcheck"] = matrix
+    order = sorted(lcs)
+    return [(k, lcs[k]) for k in order], [(k, points[k]) for k in order]
 
 
 def _short_label(_i, name, j=0):
@@ -1207,19 +1296,16 @@ def test_circuit_csr(a: int, b: int, mul_depth: int, num_constraints: int, num_v
 
 # ---- prove_batch: the prover's Fiat–Shamir transcript and the Proof (varuna.rs:136-194, 336-620; data_structures/proof.rs) ----
 
-class Transcript:
-    """The prover's PoseidonSponge<Fq, 2, 1>, its state kept in HBM between calls as one state record
-    (device.poseidon_transcripts with `state`).  Absorbs only queue operations; `squeeze` runs everything queued and its squeezes
-    in one device call, so a round costs one call.  `calls` and `permutations` count what the sponge has run: the permutations are
-    counted on the host from the mode and index alone, with the kernel's lazy rule (a permutation before the first element of a full
-    rate, or of a change of direction)."""
+class TranscriptOps:
+    """The operation list of one PoseidonSponge<Fq, 2, 1> transcript, queued on the host in the layout of
+    device.poseidon_transcripts: absorbs take their elements from this transcript's own inputs, squeezes write this transcript's own
+    outputs (offsets from zero).  `permutations` counts what running the list costs, from the mode and index alone, with the kernel's
+    lazy rule (a permutation before the first element of a full rate, or of a change of direction)."""
 
-    def __init__(self, dev):
-        self.dev = torch.device(dev)
-        self.state = poseidon.fresh_states(poseidon.FIELD_FQ, 1, self.dev)
-        self._ops, self._inputs, self._nin = [], [], 0
+    def __init__(self):
+        self._ops, self._inputs, self._nin, self._nout = [], [], 0, 0
         self._squeezing, self._idx = False, 0
-        self.calls = self.permutations = 0
+        self.permutations = 0
 
     def _advance(self, absorb: bool, count: int):
         if count == 0:
@@ -1253,23 +1339,41 @@ class Transcript:
         """absorb_native_field_elements of commitments (normalised projective uint64[k, 18])"""
         self.absorb_native(_commitment_elements(comms))
 
+    def queue_squeeze(self, counts: list, short: bool = False):
+        """one squeeze_nonnative_field_elements(n) call (squeeze_short_… when `short`) per entry of `counts`"""
+        kind = poseidon.OP_SQUEEZE_SHORT_NONNATIVE if short else poseidon.OP_SQUEEZE_NONNATIVE
+        width = 168 if short else 252
+        for n in counts:
+            self._ops.append((kind, n, self._nout))
+            self._nout += n
+            self._advance(False, -(-n * width // (poseidon.FIELDS[poseidon.FIELD_FQ][1] - 1)))
+
+    def inputs(self) -> np.ndarray:
+        return np.concatenate(self._inputs) if self._inputs else np.zeros((0, 12), dtype=np.uint32)
+
+
+class Transcript(TranscriptOps):
+    """The prover's PoseidonSponge<Fq, 2, 1>, its state kept in HBM between calls as one state record
+    (device.poseidon_transcripts with `state`).  Absorbs only queue operations; `squeeze` runs everything queued and its squeezes
+    in one device call, so a round costs one call.  `calls` and `permutations` count what the sponge has run."""
+
+    def __init__(self, dev):
+        super().__init__()
+        self.dev = torch.device(dev)
+        self.state = poseidon.fresh_states(poseidon.FIELD_FQ, 1, self.dev)
+        self.calls = 0
+
     def squeeze(self, counts: list, short: bool = False) -> list:
         """one squeeze_nonnative_field_elements(n) call (squeeze_short_… when `short`) per entry of `counts`, after everything
         queued, in one device call → [[canonical Fr] per call]"""
-        kind = poseidon.OP_SQUEEZE_SHORT_NONNATIVE if short else poseidon.OP_SQUEEZE_NONNATIVE
-        width = 168 if short else 252
-        off = 0
-        for n in counts:
-            self._ops.append((kind, n, off))
-            off += n
-            self._advance(False, -(-n * width // (poseidon.FIELDS[poseidon.FIELD_FQ][1] - 1)))
+        self.queue_squeeze(counts, short)
+        off = self._nout
         ops = torch.from_numpy(np.array(self._ops, dtype=np.int32).reshape(-1, 3)).to(self.dev)
         start = torch.tensor([0, len(self._ops)], dtype=torch.int32, device=self.dev)
-        inputs = np.concatenate(self._inputs) if self._inputs else np.zeros((0, 12), dtype=np.uint32)
-        _out, fr = device.poseidon_transcripts(poseidon.FIELD_FQ, ops, start, torch.from_numpy(inputs.view(np.int64)).to(self.dev), 0,
-                                               off, self.state)
+        _out, fr = device.poseidon_transcripts(poseidon.FIELD_FQ, ops, start, torch.from_numpy(self.inputs().view(np.int64)).to(self.dev),
+                                               0, off, self.state)
         self.calls += 1
-        self._ops, self._inputs, self._nin = [], [], 0
+        self._ops, self._inputs, self._nin, self._nout = [], [], 0, 0
         vals = [_fr_mont_to_int(row) for row in fr.cpu().numpy().view(np.uint64)] if off else []
         out, k = [], 0
         for n in counts:
@@ -1379,13 +1483,7 @@ def _prove_batch(pks_to_assignments: list, zk: bool = False, rng=None):
 
     # init_sponge (varuna.rs:136-153)
     transcript = Transcript(dev)
-    transcript.absorb_bytes(PROTOCOL_NAME)
-    for b, inputs in zip(prover.batch, _public_inputs(prover)):
-        transcript.absorb_bytes(struct.pack("<Q", b))
-        for x in inputs:
-            transcript.absorb_nonnative(x)
-    for pk in pks:
-        transcript.absorb_commitments(pk.circuit_verifying_key.circuit_commitments)
+    _init_sponge(transcript, prover.batch, _public_inputs(prover), [pk.circuit_verifying_key.circuit_commitments for pk in pks])
 
     def commit(labeled):
         blind = [None if lp.hiding_bound is None else
@@ -1483,3 +1581,366 @@ def prove_batch(pks_to_assignments: list, zk: bool = False, rng=None) -> Proof:
     randrange; a SystemRandom when None).  That stream cannot equal the reference's ChaCha stream, so a hiding proof is valid but not
     the reference's bytes; a non-hiding proof is deterministic."""
     return _prove_batch(pks_to_assignments, zk, rng)[0]
+
+
+# ---- verify_batch: the verifier (varuna.rs:625-933; sonic_pc/mod.rs:344-411, 477-544, 582-677) ----
+
+class _KeyDomains:
+    """the domains of a verifying key's CircuitInfo, under Circuit's attribute names (what linear_combinations reads)"""
+
+    def __init__(self, info: CircuitInfo):
+        self.constraint_domain = EvaluationDomain.new(info.num_constraints)
+        self.variable_domain = EvaluationDomain.new(info.num_public_and_private_variables)
+        self.input_domain = EvaluationDomain.new(info.num_public_inputs)
+        self.non_zero_domains = [EvaluationDomain.new(n) for n in (info.num_non_zero_a, info.num_non_zero_b, info.num_non_zero_c)]
+        if None in [self.constraint_domain, self.variable_domain, self.input_domain] + self.non_zero_domains:
+            raise ValueError("a domain of the circuit info is above the 2-adicity of Fr")
+
+
+_FQ_ONE = np.frombuffer(_FQ_R.to_bytes(48, "little"), dtype=np.uint64)
+_OPENING_POINTS = ("alpha", "beta", "gamma")          # the query set's point names, in the BTreeMap order batch_check walks
+
+
+def _fr_value(v, what: str) -> int:
+    v = int(v)
+    if not 0 <= v < R_MOD:
+        raise ValueError(f"{what} is not below r")
+    return v
+
+
+def _outside_image(comm, what: str) -> np.ndarray:
+    """a normalised projective image (X, Y, one) or (·, ·, zero) from the caller → its Affine image"""
+    limbs = np.ascontiguousarray(comm, dtype=np.uint64).reshape(-1)
+    if limbs.size != 18 or not (not limbs[12:].any() or (limbs[12:] == _FQ_ONE).all()):
+        raise ValueError(f"{what} is not a normalised projective image")
+    return _affine(limbs)
+
+
+class _ProofView:
+    """one (keys_to_inputs, proof) entry after the checks verify_batch makes before the transcript: circuits in id order, their
+    domains, the padded public inputs, and every G1 point taken from the caller (labels, names, Affine images)"""
+
+    def __init__(self, keys_to_inputs: list, proof: Proof):
+        if not keys_to_inputs:
+            raise ValueError("EmptyBatch: no verifying keys")
+        proof.check_batch_sizes()
+        if len(proof.batch_sizes) != len(keys_to_inputs):
+            raise ValueError(f"batch_sizes: the proof has {len(proof.batch_sizes)} circuits, the call {len(keys_to_inputs)}")
+        for k, (vk, _inputs) in enumerate(keys_to_inputs):
+            if vk.id is None:
+                raise ValueError(f"verifying key {k} has no circuit id")
+        order = sorted(range(len(keys_to_inputs)), key=lambda k: bytes(keys_to_inputs[k][0].id))
+        self.vks = [keys_to_inputs[k][0] for k in order]
+        self.ids = [bytes(vk.id) for vk in self.vks]
+        if len(set(self.ids)) != len(self.ids):
+            raise ValueError("two verifying keys have equal circuit ids")
+        self.domains = [_KeyDomains(vk.circuit_info) for vk in self.vks]
+        self.inputs = []
+        for i, (k, b) in enumerate(zip(order, proof.batch_sizes)):
+            inputs, size = keys_to_inputs[k][1], self.domains[i].input_domain.size
+            if not inputs:
+                raise ValueError(f"public inputs of verifying key {k}: EmptyBatch")
+            if len(inputs) != b:
+                raise ValueError(f"public inputs of verifying key {k}: {len(inputs)} inputs for a batch of {b}")
+            padded = []
+            for j, x in enumerate(inputs):
+                x = [_fr_value(v, f"public input {j} of verifying key {k}") for v in x]
+                if not x or x[0] != 1:
+                    raise ValueError(f"public input {j} of verifying key {k}: the first element is not one")
+                if len(x) > size:
+                    raise ValueError(f"public input {j} of verifying key {k}: {len(x)} elements for an input domain of {size}")
+                padded.append(x + [0] * (size - len(x)))
+            self.inputs.append(padded)
+        if len(proof.pc_proof) != len(_OPENING_POINTS) or any(len(e) != 2 for e in proof.pc_proof):
+            raise ValueError(f"pc_proof: one (w, random_v) per query point ({len(_OPENING_POINTS)}) expected")
+        for name, vals in (("third_sums", [s for sums in proof.third_sums for t in sums for s in t]),
+                           ("fourth_sums", [s for t in proof.fourth_sums for s in t]), ("evaluations", proof.evaluations.to_field_elements())):
+            for v in vals:
+                _fr_value(v, name)
+        if any(len(t) != 3 for sums in proof.third_sums for t in sums) or any(len(t) != 3 for t in proof.fourth_sums):
+            raise ValueError("third_sums / fourth_sums: three sums per entry expected")
+        self.random_v = [None if v is None else _fr_mont_to_int(v) for _w, v in proof.pc_proof]
+        self.label = _label_fn(self.ids)
+        c = proof.commitments
+        pts = []                                                         # (label, name, commitment)
+        for i, vk in enumerate(self.vks):
+            comms = np.ascontiguousarray(vk.circuit_commitments, dtype=np.uint64).reshape(-1, 18)
+            if comms.shape[0] != len(INDEX_POLYNOMIAL_NAMES):
+                raise ValueError(f"verifying key {order[i]}: {comms.shape[0]} circuit commitments")
+            pts += [(f"circuit_{self.ids[i].hex()}_{n}", f"verifying key {order[i]} commitment {n}", x)
+                    for n, x in zip(INDEX_POLYNOMIAL_NAMES, comms)]
+        it = iter(c.witness_commitments)
+        for i, b in enumerate(proof.batch_sizes):
+            pts += [(self.label(i, "w", j), f"witness_commitments[{sum(proof.batch_sizes[:i]) + j}]", next(it)) for j in range(b)]
+        if c.mask_poly is not None:
+            pts.append(("mask_poly", "mask_poly", c.mask_poly))
+        pts += [("h_0", "h_0", c.h_0), ("g_1", "g_1", c.g_1), ("h_1", "h_1", c.h_1)]
+        for i in range(len(self.vks)):
+            for m in "abc":
+                pts.append((self.label(i, f"g_{m}", 0), f"g_{m}_commitments[{i}]", getattr(c, f"g_{m}_commitments")[i]))
+        pts.append(("h_2", "h_2", c.h_2))
+        pts += [(f"w_{p}", f"pc_proof[{p}].w", w) for p, (w, _v) in enumerate(proof.pc_proof)]
+        self.labels = [lab for lab, _n, _x in pts]
+        self.names = [n for _l, n, _x in pts]
+        self.images = [_outside_image(x, n) for _l, n, x in pts]
+        self.proof = proof
+        # degree bounds of the bounded commitments (third and fourth round polynomial info): g_1, every g_M
+        C = _largest(d.variable_domain for d in self.domains)
+        self.bounds = {"g_1": C.size - 2}
+        for i, d in enumerate(self.domains):
+            for m, K in zip("abc", d.non_zero_domains):
+                self.bounds[self.label(i, f"g_{m}", 0)] = K.size - 2
+
+    def transcript(self) -> TranscriptOps:
+        """the verifier's sponge (varuna.rs:136-153, 770-860; verifier.rs; sonic_pc/mod.rs:405, 602), every squeeze queued: the
+        same operations prove_batch runs"""
+        p, c = self.proof, self.proof.commitments
+        t = TranscriptOps()
+        _init_sponge(t, p.batch_sizes, self.inputs, [vk.circuit_commitments for vk in self.vks])
+        t.absorb_commitments(np.stack(list(c.witness_commitments) + ([c.mask_poly] if c.mask_poly is not None else [])))
+        t.queue_squeeze([b - 1 + (1 if i else 0) for i, b in enumerate(p.batch_sizes)])
+        t.absorb_commitments(np.stack([c.h_0]))
+        t.queue_squeeze([3])
+        t.absorb_commitments(np.stack([c.g_1, c.h_1]))
+        for sums in p.third_sums:
+            for s in sums:
+                t.absorb_nonnative(s)
+        t.queue_squeeze([1])
+        t.absorb_commitments(np.stack([g for i in range(len(self.vks)) for g in (c.g_a_commitments[i], c.g_b_commitments[i],
+                                                                                 c.g_c_commitments[i])]))
+        for s in p.fourth_sums:
+            t.absorb_nonnative(s)
+        t.queue_squeeze([2] + [3] * (len(self.vks) - 1))
+        t.absorb_commitments(np.stack([c.h_2]))
+        t.queue_squeeze([1])
+        t.absorb_nonnative(p.evaluations.to_field_elements())
+        t.queue_squeeze([1] * (3 * len(self.vks) + 7), short=True)       # per point one per lc (1, 2, 3K + 1), then the randomizer
+        return t
+
+    def challenges(self, vals: list) -> dict:
+        """the transcript's squeezes (canonical, in order) → the challenges, as _prove_batch names them"""
+        it = iter(vals)
+        take = lambda n: [next(it) for _ in range(n)]                     # noqa: E731
+        combs = []
+        for i, b in enumerate(self.proof.batch_sizes):
+            e = take(b - 1 + (1 if i else 0))
+            combs.append((e[b - 1] if i else 1, [1] + e[: b - 1]))
+        alpha, eta_b, eta_c = take(3)
+        beta = take(1)[0]
+        d = [take(2)] + [take(3) for _ in self.vks[1:]]
+        deltas = [[1] + d[0]] + d[1:]
+        gamma = take(1)[0]
+        return {"batch_combiners": combs, "alpha": alpha, "eta_b": eta_b, "eta_c": eta_c, "beta": beta, "deltas": deltas,
+                "gamma": gamma, "opening": list(it)}
+
+    def check_scalars(self, ch: dict, x_at_beta: list, zk: bool) -> dict:
+        """construct_linear_combinations on the verifier's side (a_poly / b_poly expanded into the index commitments, ahp.rs:408-445),
+        then check_combinations → batch_check → accumulate_elems folded into scalars: {degree bound or None: {label: scalar}}, with
+        the None group minus the adjusted witness (g, each w, γ·G), and {"witness": {label: scalar}}, −Σ r_q·w_q"""
+        p, ev = self.proof, self.proof.evaluations
+        alpha, beta, gamma = ch["alpha"], ch["beta"], ch["gamma"]
+        lcs, query_set = linear_combinations(
+            self.domains, ch["batch_combiners"], p.third_sums, p.fourth_sums, (alpha, ch["eta_b"], ch["eta_c"], beta, ch["deltas"], gamma),
+            ev.g_1_eval, [list(g) for g in zip(ev.g_a_evals, ev.g_b_evals, ev.g_c_evals)], x_at_beta, self.label, zk)
+        expand = {}
+        for i, d in enumerate(self.domains):
+            v_rc = _vanish(d.constraint_domain, alpha) * _vanish(d.variable_domain, beta) % R_MOD
+            rc = d.constraint_domain.size * d.variable_domain.size % R_MOD
+            for j, m in enumerate("abc"):
+                idx = f"circuit_{self.ids[i].hex()}_{{}}_{m}".format
+                expand[self.label(i, "a_poly", j)] = [(v_rc, idx("row_col_val"))]
+                expand[self.label(i, "b_poly", j)] = [(rc * alpha % R_MOD * beta % R_MOD, None), ((-rc * alpha) % R_MOD, idx("col")),
+                                                      ((-rc * beta) % R_MOD, idx("row")), (rc, idx("row_col"))]
+        evals = {"g_1": ev.g_1_eval}
+        for i in range(len(self.vks)):
+            for m, vals in zip("abc", (ev.g_a_evals, ev.g_b_evals, ev.g_c_evals)):
+                evals[self.label(i, f"g_{m}", 0)] = vals[i]
+        lcs = [(lc_label, [(k * k2 % R_MOD, lab2) for k, lab in lc for k2, lab2 in (expand[lab] if lab in expand else [(1, lab)])])
+               for lc_label, lc in lcs]
+        return check_combinations_scalars(lcs, query_set, {lab: evals.get(lab, 0) for lab, _lc in lcs}, self.bounds, self.random_v,
+                                          iter(ch["opening"]))
+
+
+def _label_fn(ids: list):
+    """label(i, name, j) of circuit i's polynomial: the reference's witness_label names (ahp.rs:46-50; a_poly / b_poly as
+    construct_matrix_linear_combinations names them, ahp.rs:408-409)"""
+    def label(i, name, j=0):
+        if name in ("a_poly", "b_poly"):
+            return f"circuit_{ids[i].hex()}_{name}_{'abc'[j]}"
+        return witness_label(ids[i], name, j)
+    return label
+
+
+def _init_sponge(t: TranscriptOps, batch_sizes: list, public_inputs: list, vk_commitments: list) -> None:
+    """init_sponge (varuna.rs:136-153): the protocol name; per circuit (id order) its batch size (u64 LE) and each instance's padded
+    public input (nonnative); every circuit's twelve vk commitments"""
+    t.absorb_bytes(PROTOCOL_NAME)
+    for b, inputs in zip(batch_sizes, public_inputs):
+        t.absorb_bytes(struct.pack("<Q", b))
+        for x in inputs:
+            t.absorb_nonnative(x)
+    for comms in vk_commitments:
+        t.absorb_commitments(comms)
+
+
+_G1_STATUS = {device.G1_NOT_CANONICAL: "a coordinate is not below q", device.G1_NOT_ON_CURVE: "not on the curve",
+              device.G1_NOT_IN_SUBGROUP: "not in the prime-order subgroup"}
+
+
+def verify_batch_many(verifier: UniversalVerifier, batch: list, zk: bool = False, stats: dict | None = None) -> list:
+    """VarunaSNARK::verify_batch (varuna.rs:625-933) for many proofs in one call: `batch` is [(keys_to_inputs, proof)], keys_to_inputs
+    [(CircuitVerifyingKey, [public input, …])] with each public input a list of canonical Fr integers, formatted (first element one)
+    → one verdict per proof, in input order.  The circuits of a proof are taken in id order, so the order of keys_to_inputs changes
+    nothing.  The work of all proofs shares each device call:
+        validation    every vk commitment, proof commitment and opening w as Affine::check (device.g1_validate), one launch
+        transcript    each proof's whole PoseidonSponge<Fq, 2, 1> operation list, built on the host because the verifier knows every
+                      absorbed element up front; all proofs as transcripts of one device.poseidon_transcripts call
+        x(β)          every instance's Σ x_i·L_i(β) over its input domain, one device.matrix_evals_at_points pass
+        scalars       on the host: the verifier's linear combinations, and check_combinations / batch_check folded into one scalar per
+                      base point for each degree-bound group (None, |C_max| − 2, every |K_M| − 2), the None group minus the adjusted
+                      witness
+        MSM           every group of every proof and each proof's −Σ r_q·w_q as jobs of one device.sonic_commit_batch pass
+        pairing       each proof one check of one device.pairing_products call: the None group with H, each bounded group with its
+                      negative power of β·H, −Σ r_q·w_q with β·H
+    ValueError, naming the lowest proof at fault and the field, for what the reference returns as an error: an empty batch, the proof's
+    lists not matching its batch sizes, a count of public inputs other than the batch size, an input longer than its input domain or
+    not starting with one, a pc_proof without exactly one (w, random_v) per query point, a G1 point failing validation, the largest
+    domains' vanishing polynomial zero at α, β or γ, a degree bound the verifier holds no negative power for, a hiding proof and a
+    verifier without γ·G.  False when the proof's hiding mode is not `zk` (varuna.rs:716-727) or the pairing check fails.  `stats`,
+    when given, receives the seconds of each stage and the transcripts' permutation counts."""
+    import time
+    clock = time.perf_counter
+    t0 = clock()
+    if not batch:
+        raise ValueError("no proofs to verify")
+    n = len(batch)
+    errors, verdict, views = {}, [None] * n, [None] * n
+    for k, (keys_to_inputs, proof) in enumerate(batch):
+        try:
+            views[k] = _ProofView(list(keys_to_inputs), proof)
+        except ValueError as e:
+            errors[k] = str(e)
+
+    def live():
+        return [k for k in range(n) if k not in errors and verdict[k] is None]
+    dev = verifier.device
+    # validation: every outside point of every proof in one launch
+    todo = live()
+    pts = np.stack([img for k in todo for img in views[k].images] + [verifier.g] + ([verifier.gamma_g] if verifier.gamma_g is not None else []))
+    pts_dev = torch.from_numpy(pts).to(dev)
+    t1 = clock()
+    nout = sum(len(views[k].images) for k in todo)
+    status = device.g1_validate(pts_dev[:nout]).cpu().numpy() if nout else np.zeros(0, dtype=np.int32)
+    t2 = clock()
+    base, row = {}, 0
+    for k in todo:
+        v = views[k]
+        base[k] = row
+        bad = np.nonzero(status[row: row + len(v.images)])[0]
+        if bad.size:
+            errors[k] = f"{v.names[bad[0]]}: {_G1_STATUS[int(status[row + bad[0]])]}"
+        row += len(v.images)
+    for k in live():
+        c = views[k].proof
+        hiding, mask = any(v is not None for _w, v in c.pc_proof), c.commitments.mask_poly is not None
+        if not ((hiding and mask) if zk else (not hiding and not mask)):
+            verdict[k] = False
+    # transcripts: one thread per proof
+    todo = live()
+    ops_all, starts, inputs, nin, nfr, transcripts = [], [0], [], 0, 0, {}
+    for k in todo:
+        t = views[k].transcript()
+        transcripts[k] = (t, nfr)
+        ops = np.array(t._ops, dtype=np.int64).reshape(-1, 3)
+        ops[:, 2] += np.where(ops[:, 0] == poseidon.OP_ABSORB, nin, nfr)
+        ops_all.append(ops)
+        starts.append(starts[-1] + ops.shape[0])
+        inputs.append(t.inputs())
+        nin += t._nin
+        nfr += t._nout
+    t3 = clock()
+    vals = []
+    if todo:
+        _out, fr = device.poseidon_transcripts(
+            poseidon.FIELD_FQ, torch.from_numpy(np.concatenate(ops_all).astype(np.int32)).to(dev),
+            torch.tensor(starts, dtype=torch.int32, device=dev), torch.from_numpy(np.concatenate(inputs).view(np.int64)).to(dev), 0, nfr)
+        vals = [_fr_mont_to_int(r) for r in fr.cpu().numpy().view(np.uint64)]
+    t4 = clock()
+    chs = {}
+    for k in todo:
+        t, off = transcripts[k]
+        v = views[k]
+        ch = chs[k] = v.challenges(vals[off: off + t._nout])
+        for name, x, doms in (("α", ch["alpha"], [d.constraint_domain for d in v.domains]),
+                              ("β", ch["beta"], [d.variable_domain for d in v.domains]),
+                              ("γ", ch["gamma"], [d for dd in v.domains for d in dd.non_zero_domains])):
+            if _vanish(_largest(doms), x) == 0:
+                errors[k] = f"the vanishing polynomial of the largest domain is zero at {name}"
+                break
+    # x(β): every instance of every proof in one pass
+    todo = live()
+    xs = [(k, i, x) for k in todo for i, ins in enumerate(views[k].inputs) for x in ins]
+    t5 = clock()
+    x_at = {}
+    if xs:
+        flat = torch.from_numpy(np.stack([_mont(v) for _k, _i, x in xs for v in x]).view(np.int64)).to(dev)
+        jobs, off = [], 0
+        for k, _i, x in xs:
+            sl = flat[off: off + len(x)]
+            jobs.append((sl, sl, sl, _mont(chs[k]["beta"])))
+            off += len(x)
+        dots = device.matrix_evals_at_points(jobs)
+        for (k, i, _x), d in zip(xs, dots):
+            x_at.setdefault(k, [[] for _ in views[k].inputs])[i].append(_fr_mont_to_int(d[0]))
+    t6 = clock()
+    # scalars, then every MSM job of every proof in one pass
+    jobs, pairs = [], []
+    g_row, gamma_row = nout, nout + 1
+    for k in todo:
+        v = views[k]
+        groups = v.check_scalars(chs[k], x_at[k], zk)
+        for d in groups:
+            if d not in (None, "witness") and d not in verifier.neg_index:
+                errors[k] = f"UnsupportedDegreeBound({d}): the verifier holds no negative power of β·H for it"
+        if "gamma_g" in groups[None] and verifier.gamma_g is None:
+            errors[k] = "the proof is hiding and the verifier holds no γ·G"
+        if k in errors:
+            continue
+        local = {lab: base[k] + j for j, lab in enumerate(v.labels)}
+        local.update({"g": g_row, "gamma_g": gamma_row})
+        for d in [None] + sorted(d for d in groups if d not in (None, "witness")) + ["witness"]:
+            items = sorted(groups[d].items())
+            jobs.append(([local[lab] for lab, _s in items], [s for _l, s in items]))
+            pairs.append((k, 0 if d is None else 1 if d == "witness" else verifier.neg_index[d]))
+    if errors:
+        k = min(errors)
+        raise ValueError(f"proof {k}: {errors[k]}")
+    t7 = clock()
+    todo = live()
+    if jobs:
+        idx = torch.tensor([i for rows, _s in jobs for i in rows], dtype=torch.int64, device=dev)
+        bases = pts_dev[idx]
+        scal = torch.from_numpy(np.stack([_mont(s) for _r, ss in jobs for s in ss]).view(np.int64)).to(dev)
+        offs = np.concatenate([[0], np.cumsum([len(r) for r, _s in jobs])]).tolist()
+        sums = device.sonic_commit_batch([bases[a: b] for a, b in zip(offs, offs[1:])], [scal[a: b] for a, b in zip(offs, offs[1:])])
+        t8 = clock()
+        g1 = torch.from_numpy(np.stack([_affine(s) for s in sums])).to(dev)
+        g2_index = torch.tensor([q for _k, q in pairs], dtype=torch.int32, device=dev)
+        per_proof = [sum(1 for o, _q in pairs if o == k) for k in todo]
+        check_start = torch.tensor(np.concatenate([[0], np.cumsum(per_proof)]), dtype=torch.int32, device=dev)
+        _gt, is_one = device.pairing_products(g1, g2_index, verifier.prepared, check_start)
+        for k, one in zip(todo, is_one.cpu().tolist()):
+            verdict[k] = bool(one)
+    else:
+        t8 = t7
+    t9 = clock()
+    if stats is not None:
+        stats.update({"validation": t2 - t1, "transcript": t4 - t3, "x_at_beta": t6 - t5, "msm": t8 - t7, "pairing": t9 - t8,
+                      "host": (t1 - t0) + (t3 - t2) + (t5 - t4) + (t7 - t6),
+                      "permutations": [transcripts[k][0].permutations for k in transcripts]})
+    return verdict
+
+
+def verify_batch(verifier: UniversalVerifier, keys_to_inputs: list, proof: Proof, zk: bool = False) -> bool:
+    """VarunaSNARK::verify_batch (varuna.rs:625-933) of one proof: verify_batch_many with one entry"""
+    return verify_batch_many(verifier, [(keys_to_inputs, proof)], zk)[0]
