@@ -419,36 +419,16 @@ __global__ void __launch_bounds__(MSM_ACC_THREADS, MSM_ACC_MINBLOCKS) k_bucket_a
 // Batched-affine pair levels (the reference's own idea — batch_add, batched.rs:175-325: pair up the
 // points of a bucket, add all pairs with ONE field inversion per batch via Montgomery's trick,
 // affine.rs:224-273 — restated for the GPU).  One level halves every bucket: output element i of a
-// bucket is in[2i] + in[2i+1] (or a copy of in[2i] when the count is odd).  A thread owns T consecutive
-// OUTPUT elements (across bucket boundaries, so hot buckets are spread over many threads), walks them
-// forward accumulating the running product of the denominators (x2 − x1, or 2·y1 for a doubling) into
-// `prefix`, inverts once (Fermat, ≈ 570 Fq mul amortised over T = 64…1024 additions), then walks them
-// backward peeling off one inverse per pair: 6 Fq mul per addition instead of 10 for an XYZZ mixed add.
+// bucket is in[2i] + in[2i+1] (or a copy of in[2i] when the count is odd).  A lane owns T pairs (across
+// bucket boundaries, so hot buckets are spread over many lanes), walks them forward accumulating the
+// running product of the denominators (x2 − x1, or 2·y1 for a doubling) into `prefix`, takes one
+// inversion shared by its CTA (cta_inverse.cuh), then walks them backward peeling off one inverse per
+// pair: 6 Fq mul per addition instead of 10 for an XYZZ mixed add.
 // Dense points are 96 B (x, y Montgomery); infinity is encoded as (0, 0), which is not on y² = x³ + 1.
 // =================================================================================================
-// Level-0 inputs are gathered through `sorted` from a dense, 128-byte-aligned copy of the bases made once
-// per call by k_densify_bases: a gathered point then costs one DRAM line instead of the two or three that
+// Without pair levels, the XYZZ accumulation gathers its inputs through `sorted` from a dense, 128-byte-aligned copy of the
+// bases made once per call by k_densify_bases: a gathered point then costs one DRAM line instead of the two or three that
 // the reference's 104-byte stride straddles.
-template <bool GATHER>
-FF_DEV DensePoint load_level_input(const uint32_t* __restrict__ dense_bases, const uint32_t* __restrict__ sorted,
-                                   const uint32_t* __restrict__ dense_in, uint32_t idx) {
-    DensePoint d;
-    if (GATHER) {
-        uint32_t e = sorted[idx];
-        d = load_dense(dense_bases + (size_t)(e & 0x7fffffffu) * BASE_WORDS);
-        if ((e >> 31) && !d.inf) d.y = d.y.neg();
-    } else {
-        d = load_dense(dense_in + (size_t)idx * DENSE_WORDS);
-    }
-    return d;
-}
-// address of the record (forward pass reads x only: the denominator x2 − x1 needs nothing else unless the x's collide)
-template <bool GATHER>
-FF_DEV const uint32_t* level_input_ptr(const uint32_t* __restrict__ dense_bases, const uint32_t* __restrict__ sorted,
-                                       const uint32_t* __restrict__ dense_in, uint32_t idx) {
-    if (GATHER) return dense_bases + (size_t)(sorted[idx] & 0x7fffffffu) * BASE_WORDS;
-    return dense_in + (size_t)idx * DENSE_WORDS;
-}
 __global__ void k_densify_bases(const uint8_t* __restrict__ points, size_t stride, size_t n, uint32_t* __restrict__ out) {
     size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
@@ -484,9 +464,14 @@ __global__ void __launch_bounds__(CTA_INV_THREADS) k_precompute_tables(const uin
 }
 
 static constexpr int PAIR_THREADS = CTA_INV_THREADS;
+// Resident CTAs per SM that k_pair_level2 is built for (128 registers per thread) and that the host sizes its waves by.
+static constexpr int PAIR_MIN_BLOCKS = 4;
+// The pair-level kernels run as k_pair_desc<false> and k_pair_level2<false, PAIR_MIN_BLOCKS>, their only instances.  Their
+// template arguments keep the kernel names that profiles and the MSM path tests identify the pair levels by; the bool
+// selects nothing.
 enum PairKind { PAIR_COPY1 = 0, PAIR_COPY2 = 1, PAIR_INF = 2, PAIR_ADD = 3, PAIR_DBL = 4 };
-FF_DEV int classify_pair(const DensePoint& P, const DensePoint& Q, bool has2, Fq& d) {
-    if (!has2 || Q.inf) return PAIR_COPY1;
+FF_DEV int classify_pair(const DensePoint& P, const DensePoint& Q, Fq& d) {
+    if (Q.inf) return PAIR_COPY1;
     if (P.inf) return PAIR_COPY2;
     if (P.x == Q.x) {
         if (P.y == Q.y && !P.y.is_zero()) { d = P.y.dbl(); return PAIR_DBL; }
@@ -496,92 +481,20 @@ FF_DEV int classify_pair(const DensePoint& P, const DensePoint& Q, bool has2, Fq
     return PAIR_ADD;
 }
 
-template <bool GATHER>
-__global__ void __launch_bounds__(PAIR_THREADS, 4) k_pair_level(const uint32_t* __restrict__ dense_bases,
-                                                        const uint32_t* __restrict__ sorted, const uint32_t* __restrict__ dense_in,
-                                                        const uint32_t* __restrict__ off_in, const uint32_t* __restrict__ off_out,
-                                                        uint32_t total_buckets, uint32_t T, uint32_t* __restrict__ prefix,
-                                                        uint32_t* __restrict__ dense_out) {
-    __shared__ uint4 sh_inv4[PAIR_THREADS * 3];           // one Fq per thread for the CTA-wide shared inversion
-    uint32_t* sh_inv = reinterpret_cast<uint32_t*>(sh_inv4);
-    const uint32_t total = off_out[total_buckets];
-    const uint64_t o0_64 = (uint64_t)(blockIdx.x * blockDim.x + threadIdx.x) * T;
-    // threads past the end stay for the barriers of the shared inversion with an empty range
-    const uint32_t o0 = o0_64 < total ? (uint32_t)o0_64 : total;
-    const uint32_t o1 = (o0_64 + T < total) ? o0 + T : total;
-    uint32_t lo = 0, hi = total_buckets;                  // off_out[lo] <= o0 < off_out[hi]
-    if (o0 < o1) while (hi - lo > 1) { uint32_t mid = (lo + hi) >> 1; if (off_out[mid] <= o0) lo = mid; else hi = mid; }
-    uint32_t b = lo;
-
-    // ---- forward: running product of denominators (x coordinates only on the common path) ----
-    Fq run = Fq::one();
-    for (uint32_t o = o0; o < o1; o++) {
-        while (o >= off_out[b + 1]) b++;
-        const uint32_t i = o - off_out[b], base_in = off_in[b], cnt = off_in[b + 1] - base_in;
-        const bool has2 = 2 * i + 1 < cnt;
-        if (has2) {
-            const uint32_t* pp = level_input_ptr<GATHER>(dense_bases, sorted, dense_in, base_in + 2 * i);
-            const uint32_t* qp = level_input_ptr<GATHER>(dense_bases, sorted, dense_in, base_in + 2 * i + 1);
-            Fq x1 = Fq::load_ldg(pp), x2 = Fq::load_ldg(qp);
-            if (x1 == x2 || x1.is_zero() || x2.is_zero()) {
-                // rare: equal x (doubling / cancellation) or a possible infinity — take the full path
-                DensePoint P = load_level_input<GATHER>(dense_bases, sorted, dense_in, base_in + 2 * i);
-                DensePoint Q = load_level_input<GATHER>(dense_bases, sorted, dense_in, base_in + 2 * i + 1);
-                Fq d;
-                int kind = classify_pair(P, Q, true, d);
-                if (kind >= PAIR_ADD) run = run * d;
-            } else {
-                run = run * (x2 - x1);
-            }
-        }
-        run.store(prefix + (size_t)o * 12);
-    }
-    Fq inv = cta_shared_inverse(run, sh_inv);
-    // ---- backward: one inverse per pair, then the affine addition / doubling ----
-    for (uint32_t o = o1; o-- > o0;) {
-        while (o < off_out[b]) b--;
-        const uint32_t i = o - off_out[b], base_in = off_in[b], cnt = off_in[b + 1] - base_in;
-        const bool has2 = 2 * i + 1 < cnt;
-        DensePoint P = load_level_input<GATHER>(dense_bases, sorted, dense_in, base_in + 2 * i);
-        DensePoint Q = P;
-        if (has2) Q = load_level_input<GATHER>(dense_bases, sorted, dense_in, base_in + 2 * i + 1);
-        Fq d;
-        int kind = classify_pair(P, Q, has2, d);
-        DensePoint R;
-        if (kind == PAIR_COPY1) R = P;
-        else if (kind == PAIR_COPY2) R = Q;
-        else if (kind == PAIR_INF) { R.inf = true; R.x = Fq::zero(); R.y = Fq::zero(); }
-        else {
-            Fq inv_d = (o == o0) ? inv : inv * Fq::load(prefix + (size_t)(o - 1) * 12);
-            inv = inv * d;
-            Fq lambda;
-            if (kind == PAIR_ADD) lambda = (Q.y - P.y) * inv_d;
-            else { Fq xx = P.x.sqr(); lambda = (xx.dbl() + xx) * inv_d; }
-            Fq x3 = lambda.sqr() - P.x - Q.x;                // Q.x == P.x in the doubling case
-            R.y = lambda * (P.x - x3) - P.y;
-            R.x = x3;
-            R.inf = false;
-        }
-        store_dense(dense_out + (size_t)o * DENSE_WORDS, R);
-    }
-}
-
-
 // =================================================================================================
-// Pair level, second design (round 2): warp-interleaved outputs + a shared-memory operand ring.
+// The pair level kernel: warp-interleaved steps and a shared-memory operand ring.
 //
-// v1 above gives every THREAD a run of T consecutive outputs: the 32 lanes of a load instruction then touch 32
-// different DRAM pages / L1 lines (sorted[], prefix[], the level's dense input), every record is fetched with the
-// multiplier idle behind a 4-deep dependent chain (off_out → off_in → sorted → record), and ncu shows 2.5–4.3
-// long-scoreboard stall cycles per issued instruction at 65–72 % of the multiplier pipe.  Here a WARP owns 32·T
-// consecutive outputs and lane l takes outputs W0 + 32·j + l, j < T — any partition works for Montgomery's trick —
-// so sorted[], prefix[] and the dense inputs/outputs of a step are contiguous across the warp, and the operands of
-// step j+1 are already on their way into shared memory (cp.async / LDGSTS, 16-byte granules into a per-warp
-// [stage][chunk][lane] ring, conflict-free for LDS.128) while step j multiplies: the index chain runs two steps
-// ahead (bucket walk + sorted[] entry), the record copies one step ahead, and the multiplier calls read their
-// operands from shared memory when they need them, so nothing but the running inverse is live across a call.
-// Each record still crosses DRAM once per pass (forward: x only; backward: x and y); prefix products go to HBM
-// coalesced (48 B per output) and come back one step late behind the first multiplication of the step.
+// A WARP owns 32·T consecutive pairs and lane l takes pairs W0 + 32·j + l, j < T — any partition works for Montgomery's
+// trick.  A lane that owned T consecutive pairs instead would make the 32 lanes of every load touch 32 different DRAM
+// pages / L1 lines (ncu: 2.5–4.3 long-scoreboard stall cycles per issued instruction at 65–72 % of the multiplier pipe);
+// interleaved, the descriptors, prefix[] and the dense inputs/outputs of a step are contiguous across the warp.  The
+// operands of later steps are already on their way into shared memory (cp.async / LDGSTS, 16-byte granules into a
+// per-warp [stage][chunk][lane] ring, conflict-free for LDS.128) while the current step multiplies: a descriptor is
+// loaded one step before its copies are issued, the copies run three steps ahead in the forward pass and one in the
+// backward pass, and the multiplier calls read their operands from shared memory when they need them, so nothing but
+// the running inverse is live across a call.  Each record crosses DRAM once per pass (forward: x only; backward: x and
+// y); prefix products go to HBM coalesced (48 B per pair) and come back one step late behind the first multiplication
+// of the step.
 // =================================================================================================
 FF_DEV uint32_t smem_addr_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 FF_DEV void cp_async16(uint32_t dst, const void* src) {
@@ -640,32 +553,24 @@ FF_DEV uint32_t warp_bucket_walk(const uint32_t* __restrict__ off, uint32_t nb, 
 // its instruction stream: it reads 8 bytes per pair, coalesced, two steps ahead.  Only real pairs (both inputs present) get a
 // descriptor and a lane step: pair j of the level is the i-th pair of its bucket b, i = j − pair_off[b] (pair_off = scan of
 // ⌊cnt/2⌋), its inputs are off_in[b] + 2i and the one after, and it writes output off_out[b] + i (off_out = scan of ⌈cnt/2⌉,
-// so the output layout is that of all outputs, the pairs of a bucket first).
-//   level 0, gather:  desc = the two sorted entries (point index | sign << 31); out_pos[j] = the output position
-//   dense inputs:     desc = (index of the first input in dense_in, output position)
+// so the output layout is that of all outputs, the pairs of a bucket first).  desc[j] = (index of the first input in the
+// level's dense input, output position).
 // The single input of a bucket with an odd count is not a step: the same kernel copies it to the bucket's last output.
 static constexpr int DESC_CHUNKS = 8;                    // 32-pair chunks per warp: one binary search per 256 pairs
-template <bool GATHER>
-__global__ void __launch_bounds__(256) k_pair_desc(const uint32_t* __restrict__ sorted, const uint32_t* __restrict__ off_in,
+template <bool>
+__global__ void __launch_bounds__(256) k_pair_desc(const uint32_t* __restrict__ off_in,
                                                    const uint32_t* __restrict__ off_out, const uint32_t* __restrict__ pair_off,
-                                                   uint32_t total_buckets, uint2* __restrict__ desc, uint32_t* __restrict__ out_pos,
-                                                   const uint32_t* __restrict__ in_base_ptr /* dense inputs: *in_base_ptr = position of element 0, or null */,
+                                                   uint32_t total_buckets, uint2* __restrict__ desc,
+                                                   const uint32_t* __restrict__ in_base_ptr /* *in_base_ptr = position of element 0, or null */,
                                                    const uint32_t* __restrict__ records, uint32_t in_words, uint32_t* __restrict__ dense_out) {
     const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
-    const uint32_t in_base = (!GATHER && in_base_ptr) ? __ldg(in_base_ptr) : 0u;
+    const uint32_t in_base = in_base_ptr ? __ldg(in_base_ptr) : 0u;
     // ---- single inputs: one thread per bucket ----
     if (t < total_buckets) {
         const uint32_t end = __ldg(off_in + t + 1);
         if ((end - __ldg(off_in + t)) & 1u) {
             const uint32_t idx = end - 1u;
-            DensePoint P;
-            if (GATHER) {
-                const uint32_t s = __ldg(sorted + idx);
-                P = load_dense(records + (size_t)(s & 0x7fffffffu) * BASE_WORDS);
-                if ((s >> 31) && !P.inf) P.y = P.y.neg();
-            } else {
-                P = load_dense(records + (size_t)(idx - in_base) * in_words);
-            }
+            const DensePoint P = load_dense(records + (size_t)(idx - in_base) * in_words);
             store_dense(dense_out + (size_t)(__ldg(off_out + t + 1) - 1u) * DENSE_WORDS, P);
         }
     }
@@ -683,69 +588,58 @@ __global__ void __launch_bounds__(256) k_pair_desc(const uint32_t* __restrict__ 
         if (j0 + lane < total) {
             const uint32_t i = j - __ldg(pair_off + bj);
             const uint32_t idx = __ldg(off_in + bj) + 2u * i, o = __ldg(off_out + bj) + i;
-            uint2 d;
-            if (GATHER) { d.x = __ldg(sorted + idx); d.y = __ldg(sorted + idx + 1); out_pos[j] = o; }
-            else { d.x = idx - in_base; d.y = o; }
-            desc[j] = d;
+            desc[j] = make_uint2(idx - in_base, o);
         }
     }
 }
 
 struct PairDesc {            // one lane's pair of one step
-    uint32_t p, q, o;        // inputs and output position as written by k_pair_desc — possibly still in flight: only touch them
-                             // when the step is issued / computed (dense inputs: the second input is p + 1)
+    uint32_t p, o;           // first input (the second is p + 1) and output position as written by k_pair_desc — possibly
+                             // still in flight: only touch them when the step is issued / computed
     bool valid;              // the pair exists (known from the indices alone, never from loaded data)
 };
-// descriptor of step j for this lane (dlane = desc + W0 + lane, olane = out_pos + W0 + lane); steps outside [0, nv) do not
-// exist.  POS: load the output position too (backward pass).
-template <bool GATHER, bool POS>
-FF_DEV PairDesc pair_load_desc(int64_t j, uint32_t nv, const uint2* __restrict__ dlane, const uint32_t* __restrict__ olane) {
-    PairDesc d; d.p = 0; d.q = 0; d.o = 0; d.valid = false;
+// descriptor of step j for this lane (dlane = desc + W0 + lane); steps outside [0, nv) do not exist
+FF_DEV PairDesc pair_load_desc(int64_t j, uint32_t nv, const uint2* __restrict__ dlane) {
+    PairDesc d; d.p = 0; d.o = 0; d.valid = false;
     if (j < 0 || j >= (int64_t)nv) return d;
     const uint2 v = __ldg(dlane + 32 * j);
-    d.p = v.x; d.q = v.y; d.valid = true;
-    if (POS) d.o = GATHER ? __ldg(olane + 32 * j) : v.y;
+    d.p = v.x; d.o = v.y; d.valid = true;
     return d;
 }
 // in_words: stride of the dense inputs — the call's record stride at level 0 (BASE_WORDS or DENSE_WORDS, see
 // REC_LINE_MIN_ENTRIES), DENSE_WORDS above
-template <bool GATHER>
 FF_DEV const uint32_t* pair_src(const PairDesc& d, int which, const uint32_t* __restrict__ records, uint32_t in_words) {
-    if (GATHER) return records + (size_t)((which ? d.q : d.p) & 0x7fffffffu) * BASE_WORDS;
     return records + (size_t)(d.p + (uint32_t)which) * in_words;
 }
 // copies of step operands into ring stage `st` of `chunks` 16-byte chunks per lane: backward (FULL) x1 y1 x2 y2 in 12 chunks,
 // forward x1 x2 in 6 chunks
-template <bool GATHER, bool FULL>
+template <bool FULL>
 FF_DEV void pair_issue(const PairDesc& d, uint4* ring, int st, int lane, const uint32_t* __restrict__ records, uint32_t in_words, int chunks) {
     if (d.valid) {
         const uint32_t dst = smem_addr_u32(ring + (size_t)st * (size_t)(chunks * 32) + lane);
-        const uint32_t* p = pair_src<GATHER>(d, 0, records, in_words);
+        const uint32_t* p = pair_src(d, 0, records, in_words);
 #pragma unroll
         for (int k = 0; k < (FULL ? 6 : 3); k++) cp_async16(dst + (uint32_t)k * 512u, p + 4 * k);
-        const uint32_t* q = pair_src<GATHER>(d, 1, records, in_words);
+        const uint32_t* q = pair_src(d, 1, records, in_words);
 #pragma unroll
         for (int k = 0; k < (FULL ? 6 : 3); k++) cp_async16(dst + (uint32_t)((FULL ? 6 : 3) + k) * 512u, q + 4 * k);
     }
     cp_async_commit();
 }
 // full classification of one pair from global memory (rare path of the forward pass: equal x, or an x that is 0)
-template <bool GATHER>
 FF_DEV int pair_classify_global(const PairDesc& d, const uint32_t* __restrict__ records, uint32_t in_words, Fq& den) {
-    DensePoint P = load_dense(pair_src<GATHER>(d, 0, records, in_words));
-    DensePoint Q = load_dense(pair_src<GATHER>(d, 1, records, in_words));
-    if (GATHER) { if ((d.p >> 31) && !P.inf) P.y = P.y.neg(); if ((d.q >> 31) && !Q.inf) Q.y = Q.y.neg(); }
-    return classify_pair(P, Q, true, den);
+    const DensePoint P = load_dense(pair_src(d, 0, records, in_words));
+    const DensePoint Q = load_dense(pair_src(d, 1, records, in_words));
+    return classify_pair(P, Q, den);
 }
 
 // The shared inversion is a bubble — one warp works while the CTA's other warps wait at the barrier, and CTAs that start
 // together reach it together — so (i) the inverting warp computes ONE inverse limb-per-lane (coop_inverse, ff.cuh) instead
 // of 32 redundant copies, and (ii) every CTA takes a slot number from a per-SM counter: slot & 3 names the inverting warp, so
 // the CTAs resident on an SM invert on different sub-partitions whatever the block → SM mapping is.
-// MINB = resident CTAs per SM the kernel is compiled for: 4 (128 registers) or 3 (168 registers, no spills).
-template <bool GATHER, int MINB>
-__global__ void __launch_bounds__(PAIR_THREADS, MINB) k_pair_level2(const uint32_t* __restrict__ records /* level 0: dense bases / table; above: dense_in */,
-                                                         uint32_t in_words, const uint2* __restrict__ desc, const uint32_t* __restrict__ out_pos,
+template <bool, int MINB>
+__global__ void __launch_bounds__(PAIR_THREADS, MINB) k_pair_level2(const uint32_t* __restrict__ records /* the level's dense input */,
+                                                         uint32_t in_words, const uint2* __restrict__ desc,
                                                          const uint32_t* __restrict__ total_ptr,
                                                          uint32_t T_bound, uint32_t* __restrict__ prefix, uint32_t* __restrict__ dense_out,
                                                          uint32_t* __restrict__ sm_slots) {
@@ -772,27 +666,25 @@ __global__ void __launch_bounds__(PAIR_THREADS, MINB) k_pair_level2(const uint32
     uint32_t nv = 0;                                                                   // steps that exist for this lane
     if (w0_64 < total) { const uint64_t left = (total - w0_64 + 31) / 32; nv = left < T ? (uint32_t)left : T; }
     const uint2* dlane = desc + w0_64;
-    const uint32_t* poslane = GATHER ? out_pos + w0_64 : nullptr;
     uint32_t* plane = prefix + w0_64 * 12;                                             // prefix of step j at plane + j·32·12
 
     // ---------------- forward: running product of the denominators ----------------
-    // A forward step is ONE multiplication, far shorter than a gathered DRAM access: the x-only operands (96 B per lane) fit
+    // A forward step is ONE multiplication, far shorter than a DRAM access: the x-only operands (96 B per lane) fit
     // FOUR ring stages where the backward pass has two, so the copies run three steps ahead of the multiplier
     // (ncu, round 2: with one step of lead the forward loop held 21 % of the kernel's stall samples for 4 % of its instructions).
     Fq run = Fq::one();
     {
         constexpr int PF = 3;                                                   // steps of lead; PF + 1 stages of 6 chunks
-        PairDesc q0 = pair_load_desc<GATHER, false>(0, nv, dlane, poslane), q1 = pair_load_desc<GATHER, false>(1, nv, dlane, poslane),
-                 q2 = pair_load_desc<GATHER, false>(2, nv, dlane, poslane);
-        pair_issue<GATHER, false>(q0, ring, 0, lane, records, in_words, 6);
-        pair_issue<GATHER, false>(q1, ring, 1, lane, records, in_words, 6);
-        pair_issue<GATHER, false>(q2, ring, 2, lane, records, in_words, 6);
-        PairDesc ahead = pair_load_desc<GATHER, false>(PF, nv, dlane, poslane);
+        PairDesc q0 = pair_load_desc(0, nv, dlane), q1 = pair_load_desc(1, nv, dlane), q2 = pair_load_desc(2, nv, dlane);
+        pair_issue<false>(q0, ring, 0, lane, records, in_words, 6);
+        pair_issue<false>(q1, ring, 1, lane, records, in_words, 6);
+        pair_issue<false>(q2, ring, 2, lane, records, in_words, 6);
+        PairDesc ahead = pair_load_desc(PF, nv, dlane);
         for (uint32_t j = 0; j < T; j++) {
-            pair_issue<GATHER, false>(ahead, ring, (int)((j + PF) & 3u), lane, records, in_words, 6);       // step j+3 (descriptor loaded a step ago)
+            pair_issue<false>(ahead, ring, (int)((j + PF) & 3u), lane, records, in_words, 6);       // step j+3 (descriptor loaded a step ago)
             const PairDesc cur = q0;
             q0 = q1; q1 = q2; q2 = ahead;
-            ahead = pair_load_desc<GATHER, false>((int64_t)j + PF + 1, nv, dlane, poslane);                             // not touched until the next iteration
+            ahead = pair_load_desc((int64_t)j + PF + 1, nv, dlane);                             // not touched until the next iteration
             cp_async_wait_3();
             Fq d = Fq::one();
             if (cur.valid) {
@@ -800,7 +692,7 @@ __global__ void __launch_bounds__(PAIR_THREADS, MINB) k_pair_level2(const uint32
                 Fq x1 = ring_fq(slot_p), x2 = ring_fq(slot_p + 3 * 32);
                 if (x1 == x2 || x1.is_zero() || x2.is_zero()) {
                     Fq den;
-                    if (pair_classify_global<GATHER>(cur, records, in_words, den) >= PAIR_ADD) d = den;
+                    if (pair_classify_global(cur, records, in_words, den) >= PAIR_ADD) d = den;
                 } else {
                     d = x2 - x1;
                 }
@@ -813,13 +705,13 @@ __global__ void __launch_bounds__(PAIR_THREADS, MINB) k_pair_level2(const uint32
     Fq inv = cta_shared_inverse_by(run, sh_inv, inv_warp);
     // ---------------- backward: one inverse per pair, then the affine addition ----------------
     {
-        PairDesc cur = pair_load_desc<GATHER, true>((int64_t)T - 1, nv, dlane, poslane);
-        pair_issue<GATHER, true>(cur, ring, 0, lane, records, in_words, 12);
-        PairDesc nxt = pair_load_desc<GATHER, true>((int64_t)T - 2, nv, dlane, poslane);
+        PairDesc cur = pair_load_desc((int64_t)T - 1, nv, dlane);
+        pair_issue<true>(cur, ring, 0, lane, records, in_words, 12);
+        PairDesc nxt = pair_load_desc((int64_t)T - 2, nv, dlane);
         for (uint32_t k = 0; k < T; k++) {
             const uint32_t j = T - 1 - k;
-            pair_issue<GATHER, true>(nxt, ring, (int)((k + 1) & 1u), lane, records, in_words, 12);
-            PairDesc nn = pair_load_desc<GATHER, true>((int64_t)j - 2, nv, dlane, poslane);
+            pair_issue<true>(nxt, ring, (int)((k + 1) & 1u), lane, records, in_words, 12);
+            PairDesc nn = pair_load_desc((int64_t)j - 2, nv, dlane);
             Fq pf = Fq::one();
             if (cur.valid && j != 0) pf = Fq::load(plane + (size_t)(j - 1) * (32 * 12));     // behind the first multiplication
             cp_async_wait_1();
@@ -827,27 +719,22 @@ __global__ void __launch_bounds__(PAIR_THREADS, MINB) k_pair_level2(const uint32
             // classify (same decisions as the forward pass); a step that does not exist multiplies by one and stores nothing
             int kind = PAIR_COPY1;
             Fq d = Fq::one(), num = Fq::zero();
-            const bool negP = GATHER && (cur.p >> 31), negQ = GATHER && (cur.q >> 31);
             if (cur.valid) {
                 Fq x1 = ring_fq(slot_p), x2 = ring_fq(slot_p + 6 * 32);
                 if (x1 == x2 || x1.is_zero() || x2.is_zero()) {
                     DensePoint P, Q;
                     P.x = x1; P.y = ring_fq(slot_p + 3 * 32); P.inf = P.x.is_zero() && P.y.is_zero();
                     Q.x = x2; Q.y = ring_fq(slot_p + 9 * 32); Q.inf = Q.x.is_zero() && Q.y.is_zero();
-                    if (negP && !P.inf) P.y = P.y.neg();
-                    if (negQ && !Q.inf) Q.y = Q.y.neg();
                     Fq den;
-                    kind = classify_pair(P, Q, true, den);
+                    kind = classify_pair(P, Q, den);
                     if (kind >= PAIR_ADD) d = den;
                     if (kind == PAIR_ADD) num = Q.y - P.y;
                     else if (kind == PAIR_DBL) { Fq xx = P.x.sqr(); num = xx.dbl() + xx; }
                 } else {
                     kind = PAIR_ADD;
                     d = x2 - x1;
-                    Fq y1 = ring_fq(slot_p + 3 * 32), y2 = ring_fq(slot_p + 9 * 32);
-                    // (±y2) − (±y1) without negating first: one subtraction or one addition, then at most one negation
-                    if (negP == negQ) { num = y2 - y1; if (negP) num = num.neg(); }
-                    else { num = y2 + y1; if (negQ) num = num.neg(); }
+                    const Fq y1 = ring_fq(slot_p + 3 * 32), y2 = ring_fq(slot_p + 9 * 32);
+                    num = y2 - y1;
                 }
             }
             Fq inv_next = inv * d;
@@ -864,14 +751,13 @@ __global__ void __launch_bounds__(PAIR_THREADS, MINB) k_pair_level2(const uint32
                     DensePoint R;
                     if (kind >= PAIR_ADD) {
                         Fq y1 = ring_fq(slot_p + 3 * 32);
-                        R.x = x3; R.y = negP ? y3 + y1 : y3 - y1; R.inf = false;           // y3 − (±y1)
+                        R.x = x3; R.y = y3 - y1; R.inf = false;
                     } else if (kind == PAIR_INF) {
                         R.inf = true; R.x = Fq::zero(); R.y = Fq::zero();
                     } else {
                         const int c0 = (kind == PAIR_COPY2) ? 6 : 0;
                         R.x = ring_fq(slot_p + c0 * 32); R.y = ring_fq(slot_p + (c0 + 3) * 32);
                         R.inf = R.x.is_zero() && R.y.is_zero();
-                        if (((kind == PAIR_COPY2) ? negQ : negP) && !R.inf) R.y = R.y.neg();
                     }
                     store_dense(dense_out + (size_t)cur.o * DENSE_WORDS, R);      // consecutive pairs: consecutive outputs, but for singles between
                 }
@@ -1036,13 +922,9 @@ __global__ void __launch_bounds__(128) k_group_sum(const uint32_t* __restrict__ 
 // =================================================================================================
 // Latency path for small MSMs (≤ 2^18 points: a few thousand buckets, every kernel a handful of CTAs).  A lone thread's Fq
 // multiplications are latency-bound, so a chain of 16 mixed additions per work item, 32 + 24 per reduction chunk and 8 per tree
-// level dominated the call at 2^12–2^16 points.  Here the chains are cut with warp shuffles:
+// level dominated the call at 2^12–2^16 points.  Here the chains are cut across lanes:
 //   * k_bucket_accumulate_g8 — EIGHT lanes per work item: each lane adds every 8th entry, then a 3-step shuffle butterfly;
-//   * k_bucket_reduce_warp   — one warp per 32 buckets: a 5-step suffix scan gives the running sums Σ_{b' ≥ b} S_b', a 5-step
-//                              reduction of those gives Σ (b − lo + 1)·S_b (the reference's running-sum trick,
-//                              batched.rs:356-361, as a parallel scan);
-//   * k_window_combine_warp  — one warp per bucket set folds its ≤ 32 chunk results: Σ acc_j + 32·Σ j·run_j, the weighted sum
-//                              again as scan + reduction, the factor 32 as five doublings.
+//   * the reduction tail below — four lanes per point operation.
 // =================================================================================================
 FF_DEV XYZZ shfl_xor_xyzz(const XYZZ& a, int m) {
     XYZZ r;
@@ -1052,27 +934,6 @@ FF_DEV XYZZ shfl_xor_xyzz(const XYZZ& a, int m) {
         r.ZZ.v[j] = __shfl_xor_sync(0xffffffffu, a.ZZ.v[j], m); r.ZZZ.v[j] = __shfl_xor_sync(0xffffffffu, a.ZZZ.v[j], m);
     }
     return r;
-}
-FF_DEV XYZZ shfl_down_xyzz(const XYZZ& a, int d) {
-    XYZZ r;
-#pragma unroll
-    for (int j = 0; j < 12; j++) {
-        r.X.v[j] = __shfl_down_sync(0xffffffffu, a.X.v[j], d); r.Y.v[j] = __shfl_down_sync(0xffffffffu, a.Y.v[j], d);
-        r.ZZ.v[j] = __shfl_down_sync(0xffffffffu, a.ZZ.v[j], d); r.ZZZ.v[j] = __shfl_down_sync(0xffffffffu, a.ZZZ.v[j], d);
-    }
-    return r;
-}
-// every lane ends with Σ over the warp (butterfly: the two partners of a step compute the same sum)
-FF_DEV XYZZ warp_sum_xyzz(XYZZ a) {
-#pragma unroll 1
-    for (int m = 16; m >= 1; m >>= 1) { XYZZ o = shfl_xor_xyzz(a, m); a.add(o); }
-    return a;
-}
-// lane l ends with Σ_{l' ≥ l} a_l'
-FF_DEV XYZZ warp_suffix_scan_xyzz(XYZZ a, int lane) {
-#pragma unroll 1
-    for (int d = 1; d < 32; d <<= 1) { XYZZ o = shfl_down_xyzz(a, d); if (lane + d < 32) a.add(o); }
-    return a;
 }
 
 static constexpr int ACC_G = 8;
@@ -1105,45 +966,8 @@ __global__ void __launch_bounds__(128, 4) k_bucket_accumulate_g8(const uint32_t*
     if (valid && sub == 0) acc.store(partial + (size_t)item * XYZZ_WORDS);
 }
 
-// out[(set·chunks + chunk)·2] = Σ_l (l + 1)·S_{32·chunk + l},  out[… + 1] = Σ_l S_{32·chunk + l}
-__global__ void __launch_bounds__(128) k_bucket_reduce_warp(const uint32_t* __restrict__ partial, const uint32_t* __restrict__ item_start,
-                                                            uint32_t nbuckets, uint32_t chunks, uint32_t nsets, uint32_t* __restrict__ out) {
-    const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31u;
-    if (warp >= nsets * chunks) return;                                 // whole warps only
-    const uint32_t set = warp / chunks, ch = warp % chunks, b = ch * 32u + lane;
-    XYZZ s = XYZZ::infinity();
-    if (b < nbuckets) s = bucket_sum(partial, item_start, set * nbuckets + b);
-    const XYZZ run = warp_suffix_scan_xyzz(s, (int)lane);
-    const XYZZ acc = warp_sum_xyzz(run);
-    if (lane == 0) {
-        acc.store(out + (size_t)warp * 2 * XYZZ_WORDS);
-        run.store(out + ((size_t)warp * 2 + 1) * XYZZ_WORDS);
-    }
-}
-// window sum = Σ_j acc_j + 32·Σ_j j·run_j over the set's chunks (chunks ≤ 32)
-__global__ void __launch_bounds__(32) k_window_combine_warp(const uint32_t* __restrict__ in, uint32_t chunks, uint32_t* __restrict__ out,
-                                                            SetOffsets so) {
-    const uint32_t set = blockIdx.x, lane = threadIdx.x;
-    XYZZ a = XYZZ::infinity(), r = XYZZ::infinity();
-    if (lane < chunks) {
-        a = XYZZ::load(in + ((size_t)set * chunks + lane) * 2 * XYZZ_WORDS);
-        r = XYZZ::load(in + (((size_t)set * chunks + lane) * 2 + 1) * XYZZ_WORDS);
-    }
-    XYZZ total = warp_sum_xyzz(a);
-    if (chunks > 1) {
-        XYZZ suf = warp_suffix_scan_xyzz(r, (int)lane);                 // Σ_{i ≥ j} run_i
-        if (lane == 0) suf = XYZZ::infinity();                          // Σ_{j ≥ 1} suffix_j = Σ_j j·run_j
-        XYZZ w = warp_sum_xyzz(suf);
-        for (int k = 0; k < 5; k++) w.dbl();
-        total.add(w);
-    }
-    const uint32_t off = so.of(set);
-    if (off != 0u) { const XYZZ run = warp_sum_xyzz(r); total.add(run.mul_u32(off)); }
-    if (lane == 0) total.store(out + (size_t)set * XYZZ_WORDS);
-}
-
 // =================================================================================================
-// The same tail with FOUR LANES PER POINT (quad.cuh): an XYZZ addition costs 4 dependent multiplications instead of 14.
+// The reduction tail with FOUR LANES PER POINT (quad.cuh): an XYZZ addition costs 4 dependent multiplications instead of 14.
 //   * k_bucket_accumulate_q8 — one WARP per work item: quad s adds every 8th entry (mixed additions), 3-step butterfly
 //                              over the eight quads (sizes where the whole problem is a few thousand items);
 //   * k_bucket_reduce_quad   — one warp per 8 buckets: 3-step suffix scan + 3-step sum give (Σ (l+1)·S_l, Σ S_l);
@@ -1570,14 +1394,11 @@ int msm_core(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, co
     const size_t set_cap = flat ? max_job_n * (size_t)plan.nwin : max_job_n;   // most entries one bucket set (or one bucket) can hold
     // pair levels: the sort scatters level-0 records (k_scatter_records) and every level is dense; the XYZZ-only path keeps
     // the index sort + gather
-    bool records = levels > 0;
-    if (const char* e = getenv("SNARKVM_B200_MSM_RECORDS")) records = records && atoi(e) != 0;
-    if (const char* e = getenv("SNARKVM_B200_MSM_PAIR_V1")) { if (atoi(e) != 0) records = false; }      // the round-1 kernel gathers
     const uint32_t rec_words = !flat && max_entries >= REC_LINE_MIN_ENTRIES ? BASE_WORDS : DENSE_WORDS;   // level-0 record stride
     // a scalar segment must lie inside one base array (the record scatter reads its points through one pointer)
     std::vector<const uint8_t*> seg_points((size_t)nsegs, nullptr);
     std::vector<size_t> seg_stride((size_t)nsegs, 0);
-    if (records && !flat) {
+    if (levels > 0 && !flat) {
         for (int i = 0; i < nsegs; i++) {
             size_t off = 0; bool found = segs[i].n == 0;
             for (int k = 0; k < nbases && !found; k++) {
@@ -1605,9 +1426,8 @@ int msm_core(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, co
     uint32_t gu = nwins;                                          // windows per group
     if (levels > 0) {
         // per entry: dense_a 48 + prefix 24 + descriptors 4, plus the level-0 records (dense_b reuses them: level 0 is their
-        // last reader), 96 or 128 B (rec_words), with 8 B for the item partials and per-bucket arrays;
-        // or dense_b 24 + the 4-byte index
-        size_t per_win = set_cap * (size_t)(records ? 84 + 4 * rec_words : 104) + 1;
+        // last reader), 96 or 128 B (rec_words), with 8 B for the item partials and per-bucket arrays
+        size_t per_win = set_cap * (size_t)(84 + 4 * rec_words) + 1;
         size_t fit = budget / per_win;
         if (fit < 1) fit = 1;
         if (fit < gu) {
@@ -1625,33 +1445,27 @@ int msm_core(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, co
     const uint32_t TBg = gw * plan.nbuckets;                      // buckets of the largest group
     size_t entries_g = set_cap * (size_t)gu;                      // most entries a group can hold
     if (entries_g > max_entries) entries_g = max_entries;
-    if (records && entries_g >= 0x7fffffffull) return (int)cudaErrorInvalidValue;      // record positions carry the sign in bit 31
-    // small problems take the shuffle-based latency path (see k_bucket_reduce_warp)
-    bool warp_reduce = plan.nbuckets <= 1024u;
-    // (measured: the shuffle reduction wins at every size it applies to; eight lanes per item win only while the whole problem
-    // is a few CTAs — up to 2^10 points, equal at 2^12, and from 2^14 they lose to the butterfly's extra additions)
+    if (levels > 0 && entries_g >= 0x7fffffffull) return (int)cudaErrorInvalidValue;      // record positions carry the sign in bit 31
+    // small problems take the quad-lane latency path (k_bucket_reduce_quad, k_window_combine_quad)
+    const bool warp_reduce = plan.nbuckets <= 1024u;
+    // (measured: eight lanes per item win only while the whole problem is a few CTAs — up to 2^10 points, equal at 2^12, and
+    // from 2^14 they lose to the butterfly's extra additions)
     bool acc_g8 = levels == 0 && max_entries <= 100000;
     // round 2 (quad.cuh): four lanes per point operation.  One warp per work item (k_bucket_accumulate_q8) while the whole
     // problem is a few thousand buckets — every lane of the warp executes every multiplication, so it costs 3× the
     // multiplier time of the one-thread kernel and only pays while the GPU is mostly idle; the item holds up to 1/16 of a
     // bucket set, so a bucket has ≤ 17 item partials, k_bucket_reduce_quad adds them itself and the 32:1 folds are skipped.
-    int quad_path = 1;
-    if (const char* e = getenv("SNARKVM_B200_MSM_QUAD")) quad_path = atoi(e);
     // (measured with tools/phase_sizes.py: the warp-per-item kernel wins at 2^8 points and loses from 2^10, where the 1400 items
     // no longer fit one wave of 255-register warps)
-    bool acc_q8 = quad_path != 0 && warp_reduce && levels == 0 && (size_t)TB + max_entries / 32 <= 1100;
-    if (const char* e = getenv("SNARKVM_B200_MSM_WARP_PATH")) { if (atoi(e) == 0) { warp_reduce = false; acc_g8 = false; acc_q8 = false; } }
-    bool quad_tail_large = true;                                  // quad-lane combine levels after the per-chunk reduction of large bucket sets
-    // (measured with tools/phase_sizes.py: faster at 2^20, 2^22 and 2^24; at 2^19 — 4096 buckets per window, 256 chunks — the
-    // shorter old chain wins)
-    if (plan.nbuckets < 16384u) quad_tail_large = false;
-    if (const char* e = getenv("SNARKVM_B200_MSM_QUAD_TAIL")) quad_tail_large = atoi(e) != 0;
-    // scan-free 32:1 folds of the hot buckets (a device-side list of those with more than 32 item partials)
-    const bool quad_fold = quad_path != 0 && warp_reduce && levels == 0;
-    // large bucket sets: the same list-driven folds, down to ONE partial per bucket (a lone thread adds what is left of a bucket in
+    const bool acc_q8 = warp_reduce && levels == 0 && (size_t)TB + max_entries / 32 <= 1100;
+    // Large bucket sets: quad-lane combine levels after the per-chunk reduction (measured with tools/phase_sizes.py: faster at
+    // 2^20, 2^22 and 2^24; at 2^19 — 4096 buckets per window, 256 chunks — the shorter old chain wins), and the hot buckets
+    // folded by the list-driven quad kernel down to ONE partial per bucket (a lone thread adds what is left of a bucket in
     // k_bucket_reduce, so nothing may be left), instead of two scan + copy passes over every bucket
-    const bool large_hot = quad_path != 0 && quad_tail_large && !warp_reduce;
-    const uint32_t hot_keep = large_hot ? 1u : 32u;
+    const bool quad_tail_large = plan.nbuckets >= 16384u;
+    // scan-free 32:1 folds of the hot buckets (a device-side list of those with more than 32 item partials)
+    const bool quad_fold = warp_reduce && levels == 0;
+    const uint32_t hot_keep = quad_tail_large ? 1u : 32u;
     if (acc_q8) acc_g8 = false;
     uint32_t item_cap = plan.cap;                                  // points per work item of the XYZZ accumulation
     if (acc_g8) {                                                  // eight lanes per item: 8 × (4 … 16) points
@@ -1676,21 +1490,12 @@ int msm_core(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, co
     const size_t hot_max = max_items / 2 + 1;                         // buckets with more than `hot_keep` (1 or 32) item partials
     const size_t dense_cap_a = entries_g / 2 + TBg + 1, dense_cap_b = entries_g / 4 + 2 * (size_t)TBg + 1;
 
-    size_t pair_waves = 0;                       // 0 = fewest whole waves with T ≤ 1024 outputs per lane
-    if (const char* e = getenv("SNARKVM_B200_MSM_PAIR_WAVES")) { long v = atol(e); if (v >= 1) pair_waves = (size_t)v; }
-    bool pair_v1 = false;                        // A/B switch: the round-1 thread-contiguous pair level
-    if (const char* e = getenv("SNARKVM_B200_MSM_PAIR_V1")) pair_v1 = atoi(e) != 0;
-    int pair_minb = 4;                           // resident CTAs per SM the pair kernel is built for (4 × 128 regs or 3 × 168 regs)
-    if (const char* e = getenv("SNARKVM_B200_MSM_PAIR_MINB")) { int v = atoi(e); if (v == 3 || v == 4) pair_minb = v; }
     int sm_count = 0;
     {
         static std::once_flag smem_once[64];
         int dev = 0; cudaGetDevice(&dev);
         std::call_once(smem_once[dev & 63], [] {
-            cudaFuncSetAttribute(k_pair_level2<true, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, PAIR2_SMEM);
-            cudaFuncSetAttribute(k_pair_level2<false, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, PAIR2_SMEM);
-            cudaFuncSetAttribute(k_pair_level2<true, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, PAIR2_SMEM);
-            cudaFuncSetAttribute(k_pair_level2<false, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, PAIR2_SMEM);
+            cudaFuncSetAttribute(k_pair_level2<false, PAIR_MIN_BLOCKS>, cudaFuncAttributeMaxDynamicSharedMemorySize, PAIR2_SMEM);
         });
         const cudaError_t e = cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev);
         if (e != cudaSuccess) return (int)e;
@@ -1708,7 +1513,7 @@ int msm_core(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, co
     // ---- one scratch block, carved up ----
     uint32_t *hist, *bucket_start, *cursors, *items, *item_start, *items2, *sorted, *partial, *partial2, *red_a, *red_b;
     uint32_t *off_a = nullptr, *off_b = nullptr, *dense_a = nullptr, *dense_b = nullptr, *prefix = nullptr, *dense_bases = nullptr, *sm_slots = nullptr;
-    uint32_t *dense0 = nullptr, *cnt_tmp = nullptr, *hot_dev = nullptr, *pair_cnt = nullptr, *pair_off = nullptr, *out_pos = nullptr;
+    uint32_t *dense0 = nullptr, *cnt_tmp = nullptr, *hot_dev = nullptr, *pair_cnt = nullptr, *pair_off = nullptr;
     uint2* desc = nullptr;
     uint8_t* cub_tmp;
     Arena ar;
@@ -1719,26 +1524,25 @@ int msm_core(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, co
         items = a.take<uint32_t>((size_t)TBg + 1);
         item_start = a.take<uint32_t>((size_t)TBg + 1);
         items2 = a.take<uint32_t>((size_t)TBg + 1);
-        sorted = records ? nullptr : a.take<uint32_t>(max_entries);
+        sorted = levels > 0 ? nullptr : a.take<uint32_t>(max_entries);
         cnt_tmp = a.take<uint32_t>((size_t)TBg + 1);
         partial = a.take<uint32_t>(max_items * XYZZ_WORDS);
-        partial2 = a.take<uint32_t>(((quad_fold || large_hot) ? max_items : (size_t)TBg + max_items / 32 + 2) * XYZZ_WORDS);      // quad folds keep the item layout
+        partial2 = a.take<uint32_t>(((quad_fold || quad_tail_large) ? max_items : (size_t)TBg + max_items / 32 + 2) * XYZZ_WORDS);      // quad folds keep the item layout
         hot_dev = a.take<uint32_t>(hot_max + 2);
         red_a = a.take<uint32_t>((size_t)gw * (2 * chunks_per_set > 2 * ((plan.nbuckets + 7u) / 8u) ? 2 * chunks_per_set : 2 * ((plan.nbuckets + 7u) / 8u)) * XYZZ_WORDS);
         red_b = a.take<uint32_t>((size_t)gw * (chunks_per_set / tree + 1 > 2 * ((plan.nbuckets + 63u) / 64u) + 2 ? chunks_per_set / tree + 1 : 2 * ((plan.nbuckets + 63u) / 64u) + 2) * XYZZ_WORDS);
         cub_tmp = a.take<uint8_t>(cub_bytes);
-        if (!flat && !records) dense_bases = a.take<uint32_t>(total_bases * (size_t)BASE_WORDS);
-        if (records) dense0 = a.take<uint32_t>(entries_g * (size_t)rec_words);
+        if (!flat && levels == 0) dense_bases = a.take<uint32_t>(total_bases * (size_t)BASE_WORDS);
         if (levels > 0) {
+            dense0 = a.take<uint32_t>(entries_g * (size_t)rec_words);
             off_a = a.take<uint32_t>((size_t)TBg + 1);
             off_b = a.take<uint32_t>((size_t)TBg + 1);
             dense_a = a.take<uint32_t>(dense_cap_a * DENSE_WORDS);
             // level 1 writes its outputs (96-byte points) over the level-0 records: only level 0 reads them, and the next
             // group's scatter runs after this group's accumulation in stream order
-            if (levels > 1) dense_b = records && dense_cap_b * DENSE_WORDS <= entries_g * (size_t)rec_words ? dense0 : a.take<uint32_t>(dense_cap_b * DENSE_WORDS);
+            if (levels > 1) dense_b = dense_cap_b * DENSE_WORDS <= entries_g * (size_t)rec_words ? dense0 : a.take<uint32_t>(dense_cap_b * DENSE_WORDS);
             prefix = a.take<uint32_t>(dense_cap_a * 12);
             desc = a.take<uint2>(dense_cap_a);
-            if (!records) out_pos = a.take<uint32_t>(dense_cap_a);
             pair_cnt = a.take<uint32_t>((size_t)TBg + 1);
             pair_off = a.take<uint32_t>((size_t)TBg + 1);
             sm_slots = a.take<uint32_t>(256);
@@ -1754,12 +1558,12 @@ int msm_core(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, co
 
     CUDA_TRY(cudaMemsetAsync(hist, 0, (size_t)(TB + 1) * 4, stream));
     if (sm_slots) CUDA_TRY(cudaMemsetAsync(sm_slots, 0, 256 * 4, stream));
-    if (quad_fold) CUDA_TRY(cudaMemsetAsync(hot_dev, 0, 4, stream));     // (large_hot: reset per window group below)
+    if (quad_fold) CUDA_TRY(cudaMemsetAsync(hot_dev, 0, 4, stream));     // (quad_tail_large: reset per window group below)
     {
         // ---- bucket sort of all jobs and windows: histogram → offsets → scatter ----
         {
             ProfScope sort_scope(PROF_MSM_SORT, stream);
-            for (int pass = 0; pass < (records ? 1 : 2); pass++) {
+            for (int pass = 0; pass < (levels > 0 ? 1 : 2); pass++) {
                 for (int i = 0; i < nsegs; i++) {
                     const MsmSegment& sg = segs[i];
                     if (sg.n == 0) continue;
@@ -1784,7 +1588,7 @@ int msm_core(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, co
             }
         }
         const uint32_t* gather_src = flat ? table : dense_bases;
-        if (!flat && !records) {
+        if (!flat && levels == 0) {
             ProfScope acc_scope(PROF_MSM_ACCUMULATE, stream);
             size_t at = 0;
             for (int i = 0; i < nbases; i++) {
@@ -1803,14 +1607,14 @@ int msm_core(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, co
             const SetOffsets so = set_offsets(plan, flat, w0);
             size_t entries = set_cap * (size_t)un;                                                // bound on the group's entries
             if (entries > max_entries) entries = max_entries;
-            if (large_hot) CUDA_TRY(cudaMemsetAsync(hot_dev, 0, 4, stream));
+            if (quad_tail_large) CUDA_TRY(cudaMemsetAsync(hot_dev, 0, 4, stream));
             size_t items_bound = 1;                                                                // ≥ item count of any single bucket
             size_t items_launched = 1;                                                             // ≥ total item count of the group
             const uint32_t* final_partial = nullptr;
             const uint32_t* final_start = nullptr;
             if (levels == 0) {
                 const uint32_t cap = (acc_g8 || acc_q8 || small_cap) ? item_cap : plan.cap;
-                k_items_per_bucket<<<(tb + 256) / 256, 256, 0, stream>>>(hist + (size_t)w0 * plan.nbuckets, items, tb, cap, (quad_fold || large_hot) ? hot_dev : nullptr, (uint32_t)hot_max, hot_keep);
+                k_items_per_bucket<<<(tb + 256) / 256, 256, 0, stream>>>(hist + (size_t)w0 * plan.nbuckets, items, tb, cap, (quad_fold || quad_tail_large) ? hot_dev : nullptr, (uint32_t)hot_max, hot_keep);
                 CUDA_TRY(cub::DeviceScan::ExclusiveSum(cub_tmp, cub_bytes, items, item_start, (int)(tb + 1), stream));
                 count_launch(2);
                 const size_t group_items = (size_t)tb + entries / cap + 1;
@@ -1827,7 +1631,7 @@ int msm_core(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, co
                         gather_src, sorted, bs, item_start, tb, cap, partial);
                 count_launch();
             } else {
-                if (records) {
+                {
                     // this group's records: every segment re-derives its digits and emits the windows that fall into the group
                     ProfScope sort_scope(PROF_MSM_SORT, stream);
                     for (int i = 0; i < nsegs; i++) {
@@ -1862,58 +1666,41 @@ int msm_core(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, co
                 const uint32_t* off_in = bs;
                 uint32_t* off_bufs[2] = {off_a, off_b};
                 uint32_t* dense_bufs[2] = {dense_a, dense_b};
-                const uint32_t* dense_in = records ? dense0 : nullptr;
+                const uint32_t* dense_in = dense0;
                 size_t bound = entries;                                  // upper bound on the level's input count
                 for (int l = 0; l < levels; l++) {
                     uint32_t* off_out = off_bufs[l & 1];
                     uint32_t* dense_out = dense_bufs[l & 1];
                     k_halve_counts<<<(tb + 256) / 256, 256, 0, stream>>>(off_in, cnt_tmp, pair_cnt, tb);
                     CUDA_TRY(cub::DeviceScan::ExclusiveSum(cub_tmp, cub_bytes, cnt_tmp, off_out, (int)(tb + 1), stream));
-                    if (!pair_v1) CUDA_TRY(cub::DeviceScan::ExclusiveSum(cub_tmp, cub_bytes, pair_cnt, pair_off, (int)(tb + 1), stream));
+                    CUDA_TRY(cub::DeviceScan::ExclusiveSum(cub_tmp, cub_bytes, pair_cnt, pair_off, (int)(tb + 1), stream));
                     // pairs: Σ ⌊cnt/2⌋ ≤ Σ cnt/2; all outputs (pairs and single inputs): Σ ⌈cnt/2⌉ ≤ Σ cnt/2 + #buckets
-                    const size_t pair_bound = pair_v1 ? bound / 2 + tb : bound / 2;
+                    const size_t pair_bound = bound / 2;
                     bound = bound / 2 + tb;
                     // Whole waves: 132 SMs × 4 resident CTAs × 128 threads = 67584 lanes run at once on an H100; give every lane
                     // the same number T of pairs and launch an integer number of such waves, so no partial last wave
                     // idles most of the machine (a level is one long-running CTA per slot, not many short ones).
-                    const size_t wave = (size_t)sm_count * (pair_v1 ? 4 : pair_minb) * 128;
+                    const size_t wave = (size_t)sm_count * PAIR_MIN_BLOCKS * PAIR_THREADS;
                     size_t waves = (pair_bound + 1024 * wave - 1) / (1024 * wave);
-                    if (pair_waves) waves = pair_waves;
                     if (waves == 0) waves = 1;
                     size_t T = (pair_bound + waves * wave - 1) / (waves * wave);
                     if (T == 0) T = 1;
                     const size_t nthreads = pair_bound > T ? (pair_bound + T - 1) / T : 1;
                     const unsigned lgrid = (unsigned)((nthreads + 127) / 128);
-                    // level 0 reads absolute positions of `sorted` (off_in = bs); its outputs and all later levels are
-                    // group-relative (the scans start at 0)
-                    if (pair_v1) {
-                        if (l == 0 && !records)
-                            k_pair_level<true><<<lgrid, 128, 0, stream>>>(gather_src, sorted, nullptr, off_in, off_out, tb, (uint32_t)T, prefix, dense_out);
-                        else
-                            k_pair_level<false><<<lgrid, 128, 0, stream>>>(nullptr, nullptr, dense_in, off_in, off_out, tb, (uint32_t)T, prefix, dense_out);
-                    } else {
-                        // one thread per bucket (single inputs) and one warp per 32·DESC_CHUNKS pairs
-                        const size_t desc_warps = (pair_bound + 32 * DESC_CHUNKS - 1) / (32 * DESC_CHUNKS);
-                        const size_t desc_threads = desc_warps * 32 > (size_t)tb ? desc_warps * 32 : (size_t)tb;
-                        const unsigned dgrid = (unsigned)((desc_threads + 255) / 256);
-                        const uint32_t* pair_total = pair_off + tb;
-                        if (l == 0 && !records) {
-                            k_pair_desc<true><<<dgrid, 256, 0, stream>>>(sorted, off_in, off_out, pair_off, tb, desc, out_pos, nullptr, gather_src, BASE_WORDS, dense_out);
-                            if (pair_minb == 3) k_pair_level2<true, 3><<<lgrid, 128, PAIR2_SMEM, stream>>>(gather_src, BASE_WORDS, desc, out_pos, pair_total, (uint32_t)T, prefix, dense_out, sm_slots);
-                            else k_pair_level2<true, 4><<<lgrid, 128, PAIR2_SMEM, stream>>>(gather_src, BASE_WORDS, desc, out_pos, pair_total, (uint32_t)T, prefix, dense_out, sm_slots);
-                        } else {
-                            const uint32_t in_words = l == 0 ? rec_words : (uint32_t)DENSE_WORDS;
-                            k_pair_desc<false><<<dgrid, 256, 0, stream>>>(nullptr, off_in, off_out, pair_off, tb, desc, nullptr, l == 0 ? bs : nullptr, dense_in, in_words, dense_out);
-                            if (pair_minb == 3) k_pair_level2<false, 3><<<lgrid, 128, PAIR2_SMEM, stream>>>(dense_in, in_words, desc, nullptr, pair_total, (uint32_t)T, prefix, dense_out, sm_slots);
-                            else k_pair_level2<false, 4><<<lgrid, 128, PAIR2_SMEM, stream>>>(dense_in, in_words, desc, nullptr, pair_total, (uint32_t)T, prefix, dense_out, sm_slots);
-                        }
-                        count_launch(2);                                 // the pair scan and the descriptors
-                    }
-                    count_launch(3);
+                    // one thread per bucket (single inputs) and one warp per 32·DESC_CHUNKS pairs
+                    const size_t desc_warps = (pair_bound + 32 * DESC_CHUNKS - 1) / (32 * DESC_CHUNKS);
+                    const size_t desc_threads = desc_warps * 32 > (size_t)tb ? desc_warps * 32 : (size_t)tb;
+                    const unsigned dgrid = (unsigned)((desc_threads + 255) / 256);
+                    // level 0 reads the group's records, whose first one sits at the absolute position *bs (off_in = bs); its
+                    // outputs and all later levels are group-relative (the scans start at 0)
+                    const uint32_t in_words = l == 0 ? rec_words : (uint32_t)DENSE_WORDS;
+                    k_pair_desc<false><<<dgrid, 256, 0, stream>>>(off_in, off_out, pair_off, tb, desc, l == 0 ? bs : nullptr, dense_in, in_words, dense_out);
+                    k_pair_level2<false, PAIR_MIN_BLOCKS><<<lgrid, 128, PAIR2_SMEM, stream>>>(dense_in, in_words, desc, pair_off + tb, (uint32_t)T, prefix, dense_out, sm_slots);
+                    count_launch(5);                                     // halve, two scans, descriptors, pair level
                     off_in = off_out;
                     dense_in = dense_out;
                 }
-                k_items_from_offsets<<<(tb + 256) / 256, 256, 0, stream>>>(off_in, items, tb, plan.cap, large_hot ? hot_dev : nullptr, (uint32_t)hot_max, hot_keep);
+                k_items_from_offsets<<<(tb + 256) / 256, 256, 0, stream>>>(off_in, items, tb, plan.cap, quad_tail_large ? hot_dev : nullptr, (uint32_t)hot_max, hot_keep);
                 CUDA_TRY(cub::DeviceScan::ExclusiveSum(cub_tmp, cub_bytes, items, item_start, (int)(tb + 1), stream));
                 const size_t group_items = (size_t)tb + bound / plan.cap + 1;
                 items_bound = ((set_cap >> levels) + 1) / plan.cap + 1;
@@ -1937,7 +1724,7 @@ int msm_core(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, co
                     const uint32_t* t1 = p_in; p_in = p_out; p_out = (uint32_t*)t1;
                 }
                 final_partial = partial; final_start = item_start;
-            } else if (large_hot) {
+            } else if (quad_tail_large) {
                 // buckets with more than one item partial (the hot ones: few) are folded to one by the list-driven quad kernel
                 size_t worst = items_bound;
                 const uint32_t* p_in = partial; uint32_t* p_out = partial2;
@@ -1972,7 +1759,7 @@ int msm_core(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, co
                 final_partial = p_in; final_start = st_in;
             }
             uint32_t* group_sums = d_window_sums + (size_t)w0 * XYZZ_WORDS;
-            if (warp_reduce && quad_path != 0) {
+            if (warp_reduce) {
                 const uint32_t qchunks = (plan.nbuckets + 7u) / 8u;                     // ≤ 128
                 k_bucket_reduce_quad<<<(wn * qchunks * 32u + 127u) / 128u, 128, 0, stream>>>(final_partial, quad_fold ? partial2 : final_partial, final_start,
                                                                                               quad_rounds, plan.nbuckets, qchunks, wn, red_a);
@@ -1989,19 +1776,12 @@ int msm_core(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, co
                 count_launch(2);
                 continue;
             }
-            if (warp_reduce) {
-                const uint32_t wchunks = (plan.nbuckets + 31u) / 32u;
-                k_bucket_reduce_warp<<<(wn * wchunks * 32u + 127u) / 128u, 128, 0, stream>>>(final_partial, final_start, plan.nbuckets, wchunks, wn, red_a);
-                k_window_combine_warp<<<wn, 32, 0, stream>>>(red_a, wchunks, group_sums, so);
-                count_launch(2);
-                continue;
-            }
             const uint32_t nthreads = chunks_per_set * wn;
-            if (quad_path != 0 && quad_tail_large) {
+            if (quad_tail_large) {
                 // one thread per 16-bucket chunk leaves its (weighted sum, sum) pair; the chunk offsets are applied by 8:1 quad-lane
                 // folds (span 16 → 128 → 1024 → …), the last ≤ 64 entries of a set inside one CTA
                 k_bucket_reduce<true><<<(nthreads + 127) / 128, 128, 0, stream>>>(final_partial, final_start, plan.nbuckets, chunk, chunks_per_set, wn, red_a,
-                                                                                    partial2, large_hot ? quad_rounds : 0);
+                                                                                    partial2, quad_rounds);
                 count_launch(1);
                 const uint32_t* ent = red_a;
                 uint32_t* other = red_b;

@@ -3,7 +3,7 @@
 // Replaces the hot loops of the reference's VariableBase::msm
 // (algorithms/src/msm/variable_base/mod.rs:30-49 → batched.rs:366-415):
 //   batched_window  (batched.rs:328-364)  →  k_digits<0/1>                      (signed digits, counting sort by bucket)
-//   batch_add       (batched.rs:175-325)  →  k_pair_level ×(0/2/4)              (Montgomery-trick affine pair levels)
+//   batch_add       (batched.rs:175-325)  →  k_pair_desc + k_pair_level2 ×(0…5) (Montgomery-trick affine pair levels)
 //                                            k_bucket_accumulate(_dense)         (XYZZ sums of what is left, per work item)
 //                                            k_partial_group_sum                 (hot buckets: fold item partials 32:1)
 //   running sum     (batched.rs:356-361)  →  k_bucket_reduce / k_group_sum

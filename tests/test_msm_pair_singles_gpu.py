@@ -2,8 +2,8 @@
 copied to the bucket's last output by k_pair_desc and takes no step of k_pair_level2, whose lanes walk real pairs only and
 write each pair's output at the position its descriptor names.  These cases put odd counts everywhere (counts 1, 2 and 3 side
 by side, every bucket odd through all levels), one hot bucket over a full background, degenerate pairs next to single ∞
-outputs, the 2^24 window layout in one and several groups, the gather path, the precomputed tables and a KZG batch, and check
-every sum against the closed form Σ s_i·k_i·G (and the oracle's MSM where the input is small)."""
+outputs, the 2^24 window layout in one and several groups, ∞ bases in the level-0 records, the precomputed tables and a KZG
+batch, and check every sum against the closed form Σ s_i·k_i·G (and the oracle's MSM where the input is small)."""
 import numpy as np
 import pytest
 
@@ -114,16 +114,16 @@ def test_2p24_layout_groups(oracle_cpu, monkeypatch, scratch_mb):
         assert (got == mc.closed_form(oracle_cpu, b, scal)).all(), kind
 
 
-def test_gather_path(oracle_cpu, monkeypatch):
-    """the index sort + gather at level 0 (SNARKVM_B200_MSM_RECORDS=0): single inputs copied with their sign applied"""
+def test_infinite_bases_in_level0_records(oracle_cpu, monkeypatch):
+    """c = 6, three levels, every 7th base ∞ under counts 1, 2 and 3: ∞ records reach level 0 as single inputs and as either
+    input of a pair, and single ∞ inputs survive the copy to the bucket's last output"""
     set_env(monkeypatch, {"SNARKVM_B200_MSM_C": 6, "SNARKVM_B200_MSM_LEVELS": 3})
-    monkeypatch.setenv("SNARKVM_B200_MSM_RECORDS", "0")
     reps = [1, 2, 3] * 10 + [5]
     scal = repeated_digit_scalars(reps)
     b = plain_bases(scal.shape[0], 74)
     b.infinity(np.arange(0, scal.shape[0], 7))
     _, kern = traced(lambda: check(oracle_cpu, b, scal))
-    check_kernels(kern, must=("k_pair_desc<true>", "k_pair_level2<true, 4>"))
+    check_kernels(kern, must=PAIR_KERNELS)
     n = 20000
     b = adversarial_bases(n, seed=75)
     for f, kind in enumerate(mc.SCALAR_FAMILIES):

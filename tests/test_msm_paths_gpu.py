@@ -205,7 +205,7 @@ def test_path_large_tail_small_groups(oracle_cpu, monkeypatch):
     b = adversarial_bases(20000, seed=30)
     run_case(oracle_cpu, b, mc.SCALAR_FAMILIES, 700,
              must=("k_scatter_records<false, false>", "k_pair_level2<false, 4>", "k_bucket_accumulate_dense", "k_combine_level_quad")
-             + LARGE_TAIL, must_not=("k_combine_level_quadseq", "k_bucket_accumulate", "k_pair_level2<true, 4>"),
+             + LARGE_TAIL, must_not=("k_combine_level_quadseq", "k_bucket_accumulate"),
              counts={"k_window_combine_quad": lambda k: k >= 4})
 
 
@@ -221,7 +221,7 @@ def test_path_pair_levels_many_outputs_per_lane(oracle_cpu, monkeypatch):
     t = np.arange(1000, n, 97)                                  # more torsion rows spread over the array
     b.torsion_points(t[0::3], "t2").torsion_points(t[1::3], "t3").torsion_points(t[2::3], "t3neg")
     must = ("k_scatter_records<false, false>", "k_pair_desc<false>", "k_pair_level2<false, 4>", "k_bucket_accumulate_dense")
-    run_case(oracle_cpu, b, mc.SCALAR_FAMILIES, 800, must=must + QUAD_TAIL, must_not=("k_pair_level2<true, 4>", "k_bucket_accumulate"),
+    run_case(oracle_cpu, b, mc.SCALAR_FAMILIES, 800, must=must + QUAD_TAIL, must_not=("k_bucket_accumulate",),
              counts={"k_pair_level2<false, 4>": 3})
     inf = np.frombuffer(py.projective_bytes_normalised(None), dtype=np.uint64)
     scal = random_canonical_fr(n, seed=801)

@@ -29,7 +29,7 @@ def test_record_stride_window_groups(oracle_cpu, monkeypatch, scratch_gb, groups
         if f == 0:
             got, kern = traced(lambda: device.msm(bases, _dev(scal)))
             check_kernels(kern, must=("k_pair_level2<false, 4>", "k_bucket_accumulate_dense") + LARGE_TAIL,
-                          must_not=("k_bucket_accumulate", "k_pair_level2<true, 4>"),
+                          must_not=("k_bucket_accumulate",),
                           counts={"k_scatter_records<false, false>": groups})
         else:
             got = device.msm(bases, _dev(scal))
