@@ -541,9 +541,28 @@ SNARKVM_API int snarkvm_b200_poseidon_transcripts_resume_device(int field, const
  * (y² ≠ x³ + 1) or NOT_IN_SUBGROUP ([x²]·φ(P) + P ≠ O, x the BLS parameter, φ(x, y) = (PHI·x, y)), the first test that fails.  One
  * launch, one thread per point, no synchronisation. */
 enum {
-    SNARKVM_B200_G1_VALID = 0, SNARKVM_B200_G1_NOT_CANONICAL = 1, SNARKVM_B200_G1_NOT_ON_CURVE = 2, SNARKVM_B200_G1_NOT_IN_SUBGROUP = 3
+    SNARKVM_B200_G1_VALID = 0, SNARKVM_B200_G1_NOT_CANONICAL = 1, SNARKVM_B200_G1_NOT_ON_CURVE = 2, SNARKVM_B200_G1_NOT_IN_SUBGROUP = 3,
+    SNARKVM_B200_G1_BAD_FLAGS = 4
 };
 SNARKVM_API int snarkvm_b200_g1_validate_device(int32_t* d_status, const void* d_points, size_t n, size_t stride, void* stream);
+
+/* G1 points from their byte forms (CanonicalDeserialize of Affine<G1>: curves/src/templates/macros.rs:118-144, SWFlags of
+ * utilities/src/serialize/flags.rs).  d_bytes holds n points of 48 bytes (compressed: x little-endian, bit 7 of the last byte
+ * PositiveY, bit 6 Infinity) or 96 bytes (uncompressed: x, then y with the flags; x carries none), no alignment needed.  d_points
+ * (8-byte aligned, 104-byte stride) receives each point's Affine<G1> image and d_status[i] (device int32, 4-byte aligned) its
+ * status: BAD_FLAGS (both flag bits set, or bit 7 of an uncompressed x), NOT_CANONICAL (a coordinate not below q after the flags
+ * are masked), NOT_ON_CURVE (compressed: x³ + 1 has no square root in Fq), the first that applies; otherwise VALID, and with
+ * `validate` the status of Affine::check as snarkvm_b200_g1_validate_device reports it.  Infinity decodes to Affine::zero()
+ * (0, 1, infinity) whatever the coordinates below q were.  A compressed point's y is the root of x³ + 1 that is the larger of y, −y
+ * (canonical integers) when PositiveY is set, the smaller otherwise.  An uncompressed point is not tested against the curve unless
+ * `validate`.  Bytes that decode to no point leave an all-zero image.  One launch, one thread per point, no synchronisation. */
+SNARKVM_API int snarkvm_b200_g1_deserialize_device(void* d_points, int32_t* d_status, const void* d_bytes, size_t n, int compressed,
+                                                   int validate, void* stream);
+/* G1 points to their byte forms (CanonicalSerialize of Affine<G1>, macros.rs:67-97): d_projective holds n normalised projective
+ * images (X, Y, Z Montgomery Fq, 144 bytes each, 8-byte aligned; Z = one, or Z = 0 for infinity); d_bytes receives 48 bytes per
+ * point (compressed: canonical x, PositiveY iff y > −y; infinity: x = 0 with the Infinity bit) or 96 (uncompressed: canonical x and
+ * y, no sign flag; infinity: x = 0, y = 1 with the Infinity bit).  One launch, one thread per point, no synchronisation. */
+SNARKVM_API int snarkvm_b200_g1_serialize_device(void* d_bytes, const void* d_projective, size_t n, int compressed, void* stream);
 
 #ifdef __cplusplus
 }

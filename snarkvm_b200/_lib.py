@@ -40,6 +40,7 @@ SYMBOLS = (
     "snarkvm_b200_varuna_round4_evals_device", "snarkvm_b200_g2_prepare_device", "snarkvm_b200_pairing_products_device",
     "snarkvm_b200_test_tower_op_device", "snarkvm_b200_poseidon_transcripts_device",
     "snarkvm_b200_poseidon_transcripts_resume_device", "snarkvm_b200_g1_validate_device",
+    "snarkvm_b200_g1_deserialize_device", "snarkvm_b200_g1_serialize_device",
 )
 
 
@@ -188,6 +189,8 @@ def lib():
     L.snarkvm_b200_poseidon_transcripts_resume_device.argtypes = [i32, vp, vp, vp, sz, sz, vp, sz, vp, sz, vp, sz, vp,
                                                                   ctypes.POINTER(ctypes.c_int64), vp]
     L.snarkvm_b200_g1_validate_device.argtypes = [vp, vp, sz, sz, vp]
+    L.snarkvm_b200_g1_deserialize_device.argtypes = [vp, vp, vp, sz, i32, i32, vp]
+    L.snarkvm_b200_g1_serialize_device.argtypes = [vp, vp, sz, i32, vp]
     L.snarkvm_b200_msm_batch_device.argtypes = [vp, vp, sz, vp, vp, sz, vp]
     L.snarkvm_b200_msm_window_sums_plan_device.argtypes = [vp, vp, sz, vp, sz, vp, sz, vp]
     L.snarkvm_b200_kzg_commit_batch_hiding_device.argtypes = [vp, vp, sz, vp, vp, vp, vp, vp, sz, vp]

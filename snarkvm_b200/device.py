@@ -165,7 +165,8 @@ def pairing_products(g1: torch.Tensor, g2_index: torch.Tensor, prepared: torch.T
     return (gt, is_one.bool(), mv) if miller else (gt, is_one.bool())
 
 
-G1_VALID, G1_NOT_CANONICAL, G1_NOT_ON_CURVE, G1_NOT_IN_SUBGROUP = 0, 1, 2, 3
+G1_VALID, G1_NOT_CANONICAL, G1_NOT_ON_CURVE, G1_NOT_IN_SUBGROUP, G1_BAD_FLAGS = 0, 1, 2, 3, 4
+G1_COMPRESSED_BYTES, G1_UNCOMPRESSED_BYTES = 48, 96
 
 
 def g1_validate(points: torch.Tensor, stride: int = AFFINE_STRIDE) -> torch.Tensor:
@@ -177,6 +178,40 @@ def g1_validate(points: torch.Tensor, stride: int = AFFINE_STRIDE) -> torch.Tens
         with torch.cuda.device(points.device):
             _lib.check(_lib.lib().snarkvm_b200_g1_validate_device(status.data_ptr(), _check(points, "points"), n, stride, _stream()))
     return status
+
+
+def g1_deserialize(bytes_u8: torch.Tensor, compressed: bool = True, validate: bool = True):
+    """G1 points from their byte forms (snarkvm_b200_g1_deserialize_device): `bytes_u8` a uint8 CUDA tensor of n × 48 compressed
+    or n × 96 uncompressed bytes → (Affine<G1> images uint8 [n, 104], int32 status [n]), both in HBM.  Status G1_BAD_FLAGS (both
+    flag bits set, or bit 7 of an uncompressed x), G1_NOT_CANONICAL (a coordinate ≥ q), G1_NOT_ON_CURVE (compressed: x³ + 1 has no
+    square root), else G1_VALID or, with `validate`, g1_validate's status.  Bytes that decode to no point leave an all-zero image."""
+    size = G1_COMPRESSED_BYTES if compressed else G1_UNCOMPRESSED_BYTES
+    if bytes_u8.dtype != torch.uint8 or _nbytes(bytes_u8) % size:
+        raise ValueError(f"g1_deserialize takes uint8 bytes, {size} per point")
+    n = _nbytes(bytes_u8) // size
+    images = torch.empty((n, AFFINE_STRIDE), dtype=torch.uint8, device=bytes_u8.device)
+    status = torch.empty(n, dtype=torch.int32, device=bytes_u8.device)
+    if n:
+        with torch.cuda.device(bytes_u8.device):
+            _lib.check(_lib.lib().snarkvm_b200_g1_deserialize_device(images.data_ptr(), status.data_ptr(), _check(bytes_u8, "bytes_u8"),
+                                                                     n, int(bool(compressed)), int(bool(validate)), _stream()))
+    return images, status
+
+
+def g1_serialize(projective: torch.Tensor, compressed: bool = True) -> torch.Tensor:
+    """G1 points to their byte forms (snarkvm_b200_g1_serialize_device): `projective` a CUDA tensor of n normalised projective
+    images (X, Y, Z Montgomery Fq, 144 bytes each; Z = one, or zero for infinity) → uint8 [n, 48] compressed or [n, 96]
+    uncompressed, in HBM"""
+    if _nbytes(projective) % 144:
+        raise ValueError("g1_serialize takes 144-byte normalised projective images")
+    n = _nbytes(projective) // 144
+    size = G1_COMPRESSED_BYTES if compressed else G1_UNCOMPRESSED_BYTES
+    out = torch.empty((n, size), dtype=torch.uint8, device=projective.device)
+    if n:
+        with torch.cuda.device(projective.device):
+            _lib.check(_lib.lib().snarkvm_b200_g1_serialize_device(out.data_ptr(), _check(projective, "projective"), n,
+                                                                   int(bool(compressed)), _stream()))
+    return out
 
 
 POSEIDON_ABSORB, POSEIDON_SQUEEZE, POSEIDON_SQUEEZE_NONNATIVE, POSEIDON_SQUEEZE_SHORT_NONNATIVE = 0, 1, 2, 3

@@ -384,6 +384,21 @@ class CircuitVerifyingKey:
     circuit_commitments: np.ndarray
     id: bytes | None = None
 
+    def to_bytes(self, compress: bool = True, device_="cuda") -> bytes:
+        """the bytes of CanonicalSerialize (compressed: ToBytes), every point through one device.g1_serialize call"""
+        return _to_bytes_many(_verifying_key_parts, [self], compress, device_)[0]
+
+    @staticmethod
+    def read(blob, offset: int = 0, compress: bool = True, validate: bool = True, device_="cuda"):
+        """the CircuitVerifyingKey whose bytes start at `offset` of `blob` → (CircuitVerifyingKey, the offset after it); errors as verifying_keys_from_bytes"""
+        objs, ends = _from_bytes_many(_walk_verifying_key, [blob], [offset], compress, validate, device_)
+        return objs[0], ends[0]
+
+    @staticmethod
+    def from_bytes(blob, compress: bool = True, validate: bool = True, device_="cuda") -> "CircuitVerifyingKey":
+        """the CircuitVerifyingKey at the start of `blob` (FromBytes when compressed); trailing bytes are ignored"""
+        return CircuitVerifyingKey.read(blob, 0, compress, validate, device_)[0]
+
 
 @dataclass
 class CircuitProvingKey:
@@ -432,6 +447,21 @@ class Certificate:
     """snark/varuna/data_structures/certificate.rs: the BatchLCProof of prove_vk, one non-hiding KZG proof `w` (normalised projective
     uint64[18]) at the one query point"""
     w: np.ndarray
+
+    def to_bytes(self, compress: bool = True, device_="cuda") -> bytes:
+        """the bytes of CanonicalSerialize (compressed: ToBytes), every point through one device.g1_serialize call"""
+        return _to_bytes_many(_certificate_parts, [self], compress, device_)[0]
+
+    @staticmethod
+    def read(blob, offset: int = 0, compress: bool = True, validate: bool = True, device_="cuda"):
+        """the Certificate whose bytes start at `offset` of `blob` → (Certificate, the offset after it); errors as certificates_from_bytes"""
+        objs, ends = _from_bytes_many(_walk_certificate, [blob], [offset], compress, validate, device_)
+        return objs[0], ends[0]
+
+    @staticmethod
+    def from_bytes(blob, compress: bool = True, validate: bool = True, device_="cuda") -> "Certificate":
+        """the Certificate at the start of `blob` (FromBytes when compressed); trailing bytes are ignored"""
+        return Certificate.read(blob, 0, compress, validate, device_)[0]
 
 
 def _certificate_point(challenges) -> tuple:
@@ -1431,6 +1461,21 @@ class Proof:
                 or [len(s) for s in self.third_sums] != list(self.batch_sizes) or len(self.fourth_sums) != K):
             raise ValueError("InvalidBatchSize: the proof's lists do not match its batch sizes")
 
+    def to_bytes(self, compress: bool = True, device_="cuda") -> bytes:
+        """the bytes of CanonicalSerialize (compressed: ToBytes), every point through one device.g1_serialize call"""
+        return _to_bytes_many(_proof_parts, [self], compress, device_)[0]
+
+    @staticmethod
+    def read(blob, offset: int = 0, compress: bool = True, validate: bool = True, device_="cuda"):
+        """the Proof whose bytes start at `offset` of `blob` → (Proof, the offset after it); errors as proofs_from_bytes"""
+        objs, ends = _from_bytes_many(_walk_proof, [blob], [offset], compress, validate, device_)
+        return objs[0], ends[0]
+
+    @staticmethod
+    def from_bytes(blob, compress: bool = True, validate: bool = True, device_="cuda") -> "Proof":
+        """the Proof at the start of `blob` (FromBytes when compressed); trailing bytes are ignored"""
+        return Proof.read(blob, 0, compress, validate, device_)[0]
+
 
 def _union_committer_key(cks: list):
     """CommitterUnionKey::union (sonic_pc/data_structures.rs) of committer keys trimmed from one SRS: the longest powers, every
@@ -1610,10 +1655,7 @@ def _fr_value(v, what: str) -> int:
 
 def _outside_image(comm, what: str) -> np.ndarray:
     """a normalised projective image (X, Y, one) or (·, ·, zero) from the caller → its Affine image"""
-    limbs = np.ascontiguousarray(comm, dtype=np.uint64).reshape(-1)
-    if limbs.size != 18 or not (not limbs[12:].any() or (limbs[12:] == _FQ_ONE).all()):
-        raise ValueError(f"{what} is not a normalised projective image")
-    return _affine(limbs)
+    return _affine(_normalised(comm, what))
 
 
 class _ProofView:
@@ -1944,3 +1986,232 @@ def verify_batch_many(verifier: UniversalVerifier, batch: list, zk: bool = False
 def verify_batch(verifier: UniversalVerifier, keys_to_inputs: list, proof: Proof, zk: bool = False) -> bool:
     """VarunaSNARK::verify_batch (varuna.rs:625-933) of one proof: verify_batch_many with one entry"""
     return verify_batch_many(verifier, [(keys_to_inputs, proof)], zk)[0]
+
+
+# ---- byte forms: CanonicalSerialize / CanonicalDeserialize of Proof (data_structures/proof.rs:305-368), CircuitVerifyingKey
+# (circuit_verifying_key.rs, derived) and Certificate (certificate.rs, derived), in the compressed (ToBytes) or uncompressed mode ----
+
+_G1_BYTES_STATUS = {**_G1_STATUS, device.G1_BAD_FLAGS: "malformed flag bits"}
+
+
+def _g1_size(compress: bool) -> int:
+    return device.G1_COMPRESSED_BYTES if compress else device.G1_UNCOMPRESSED_BYTES
+
+
+class _Walk:
+    """one blob's host walk from `offset`: bounds-checked reads in the reference's field order; every G1 point's bytes are appended
+    to the shared `points` list ((bytes, field)) and stand for their index there until the one device call decodes them all"""
+
+    def __init__(self, blob, offset: int, compress: bool, points: list):
+        self.b, self.o, self.psize, self.points = bytes(blob), int(offset), _g1_size(compress), points
+        if not 0 <= self.o <= len(self.b):
+            raise ValueError(f"offset {offset} is outside the blob")
+
+    def need(self, n: int, field: str) -> None:
+        if n > len(self.b) - self.o:
+            raise ValueError(f"{field}: {len(self.b) - self.o} bytes left, at least {n} needed")
+
+    def take(self, n: int, field: str) -> bytes:
+        self.need(n, field)
+        self.o += n
+        return self.b[self.o - n: self.o]
+
+    def u64(self, field: str) -> int:
+        return struct.unpack("<Q", self.take(8, field))[0]
+
+    def tag(self, field: str) -> bool:
+        """an Option's tag (bool::read_le): 0 or 1"""
+        t = self.take(1, field)[0]
+        if t > 1:
+            raise ValueError(f"{field}: option tag {t} is neither 0 nor 1")
+        return t == 1
+
+    def fr(self, field: str) -> int:
+        v = int.from_bytes(self.take(32, field), "little")
+        if v >= R_MOD:
+            raise ValueError(f"{field}: not below r")
+        return v
+
+    def point(self, field: str) -> int:
+        self.points.append((self.take(self.psize, field), field))
+        return len(self.points) - 1
+
+    def batch_lc_proof(self, field: str) -> list:
+        """BatchLCProof: a u64 count of KZGProof (w, Option<Fr> random_v) → [(point index, Montgomery random_v or None)]"""
+        n = self.u64(f"{field} length")
+        self.need(n * (self.psize + 1), f"{field} of {n} proofs")
+        out = []
+        for p in range(n):
+            w = self.point(f"{field}[{p}].w")
+            v = self.fr(f"{field}[{p}].random_v") if self.tag(f"{field}[{p}].random_v tag") else None
+            out.append((w, None if v is None else _fr_int_to_mont(v)))
+        return out
+
+
+def _walk_proof(w: _Walk):
+    """proof.rs:344-368 → a function of the decoded points that builds the Proof.  Every count is checked against the bytes left
+    before anything of its size is read, so a blob claiming 2^40 instances costs nothing."""
+    P = w.psize
+    K = w.u64("batch_sizes length")
+    w.need(8 * K, f"batch_sizes of {K} circuits")
+    sizes = [w.u64(f"batch_sizes[{i}]") for i in range(K)]
+    total = sum(sizes)
+    # at least: every commitment without the mask, the mask tag, every Fr, the pc_proof length
+    w.need(P * (total + 4 + 3 * K) + 1 + 32 * (1 + 6 * K + 3 * total) + 8, f"the body of batch sizes {sizes}")
+    wit = [w.point(f"witness_commitments[{j}]") for j in range(total)]
+    mask = w.point("mask_poly") if w.tag("mask_poly tag") else None
+    h_0, g_1, h_1 = (w.point(n) for n in ("h_0", "g_1", "h_1"))
+    g_abc = [[w.point(f"g_{m}_commitments[{i}]") for i in range(K)] for m in "abc"]
+    h_2 = w.point("h_2")
+    g_1_eval = w.fr("evaluations.g_1_eval")
+    evals = [[w.fr(f"evaluations.g_{m}_evals[{i}]") for i in range(K)] for m in "abc"]
+    third = [[[w.fr(f"third_sums[{i}][{j}]") for _ in range(3)] for j in range(b)] for i, b in enumerate(sizes)]
+    fourth = [[w.fr(f"fourth_sums[{i}]") for _ in range(3)] for i in range(K)]
+    pc = w.batch_lc_proof("pc_proof")
+
+    def build(pts):
+        comms = Commitments([pts[j] for j in wit], None if mask is None else pts[mask], pts[h_0], pts[g_1], pts[h_1],
+                            *[[pts[j] for j in g] for g in g_abc], pts[h_2])
+        return Proof(sizes, comms, Evaluations(g_1_eval, *evals), third, fourth, [(pts[j], v) for j, v in pc])
+    return build
+
+
+def _walk_verifying_key(w: _Walk):
+    """CircuitInfo (six u64), the commitments as a Vec (u64 length, which must be 12), the 32-byte circuit id"""
+    info = CircuitInfo(*[w.u64(f"circuit_info.{f}") for f in CircuitInfo.__dataclass_fields__])
+    n = w.u64("circuit_commitments length")
+    if n != len(INDEX_POLYNOMIAL_NAMES):
+        raise ValueError(f"circuit_commitments: {n} commitments, not {len(INDEX_POLYNOMIAL_NAMES)}")
+    comms = [w.point(f"circuit_commitments[{name}]") for name in INDEX_POLYNOMIAL_NAMES]
+    cid = w.take(32, "id")
+    return lambda pts: CircuitVerifyingKey(info, np.stack([pts[j] for j in comms]), cid)
+
+
+def _walk_certificate(w: _Walk):
+    """the BatchLCProof of prove_vk: exactly one non-hiding KZG proof"""
+    pc = w.batch_lc_proof("pc_proof")
+    if len(pc) != 1 or pc[0][1] is not None:
+        raise ValueError("pc_proof: a certificate holds exactly one non-hiding proof")
+    return lambda pts: Certificate(pts[pc[0][0]])
+
+
+def _from_bytes_many(walk, blobs, offsets, compress: bool, validate: bool, device_):
+    """walk every blob on the host, then decode every point of every blob in one device call → (objects, end offsets).
+    ValueError names the lowest blob at fault and its field.  A blob that fails the walk is reported before any device call,
+    unless a blob below it holds points, which are then decoded to find whether one of them fails first."""
+    points, builds, ends, starts, fail = [], [], [], [], None
+    for k, blob in enumerate(blobs):
+        starts.append(len(points))
+        try:
+            w = _Walk(blob, offsets[k], compress, points)
+            builds.append(walk(w))
+            ends.append(w.o)
+        except ValueError as e:
+            fail = (k, str(e))
+            del points[starts[-1]:]
+            break
+    pts = []
+    if points:
+        raw = torch.from_numpy(np.frombuffer(b"".join(b for b, _f in points), dtype=np.uint8).copy()).to(torch.device(device_))
+        images, status = device.g1_deserialize(raw, compress, validate)
+        images, status = images.cpu().numpy(), status.cpu().numpy()
+        bad = np.nonzero(status)[0]
+        if bad.size:
+            i = int(bad[0])
+            k = int(np.searchsorted(starts, i, side="right")) - 1
+            raise ValueError(f"blob {k}: {points[i][1]}: {_G1_BYTES_STATUS[int(status[i])]}")
+        limbs = np.zeros((len(points), 18), dtype=np.uint64)
+        limbs[:, :12] = images[:, :96].copy().view(np.uint64)
+        inf = images[:, 96] != 0
+        limbs[~inf, 12:] = _FQ_ONE
+        limbs[inf, :12] = 0
+        limbs[inf, 6:12] = _FQ_ONE                                        # (0, one, 0)
+        pts = list(limbs)
+    if fail is not None:
+        raise ValueError(f"blob {fail[0]}: {fail[1]}")
+    return [b(pts) for b in builds], ends
+
+
+def _normalised(comm, what: str) -> np.ndarray:
+    """a normalised projective image (X, Y, one) or (·, ·, zero) from the caller → its uint64[18] limbs; ValueError if not"""
+    limbs = np.ascontiguousarray(comm, dtype=np.uint64).reshape(-1)
+    if limbs.size != 18 or not (not limbs[12:].any() or (limbs[12:] == _FQ_ONE).all()):
+        raise ValueError(f"{what} is not a normalised projective image")
+    return limbs
+
+
+def _fr_bytes(v, what: str) -> bytes:
+    return _fr_value(v, what).to_bytes(32, "little")
+
+
+def _proof_parts(p: Proof) -> list:
+    """proof.rs:305-317: bytes and (point, field) pairs in write order"""
+    p.check_batch_sizes()
+    c, e = p.commitments, p.evaluations
+    parts = [struct.pack(f"<{1 + len(p.batch_sizes)}Q", len(p.batch_sizes), *p.batch_sizes)]
+    parts += [(x, f"witness_commitments[{j}]") for j, x in enumerate(c.witness_commitments)]
+    parts += [b"\x00"] if c.mask_poly is None else [b"\x01", (c.mask_poly, "mask_poly")]
+    parts += [(c.h_0, "h_0"), (c.g_1, "g_1"), (c.h_1, "h_1")]
+    for m in "abc":
+        parts += [(x, f"g_{m}_commitments[{i}]") for i, x in enumerate(getattr(c, f"g_{m}_commitments"))]
+    parts.append((c.h_2, "h_2"))
+    parts.append(_fr_bytes(e.g_1_eval, "evaluations.g_1_eval"))
+    parts += [_fr_bytes(v, "evaluations") for v in list(e.g_a_evals) + list(e.g_b_evals) + list(e.g_c_evals)]
+    parts += [_fr_bytes(v, "third_sums") for sums in p.third_sums for t in sums for v in t]
+    parts += [_fr_bytes(v, "fourth_sums") for t in p.fourth_sums for v in t]
+    return parts + _batch_lc_parts(p.pc_proof)
+
+
+def _batch_lc_parts(pc: list) -> list:
+    parts = [struct.pack("<Q", len(pc))]
+    for q, (w, v) in enumerate(pc):
+        parts.append((w, f"pc_proof[{q}].w"))
+        parts += [b"\x00"] if v is None else [b"\x01", _fr_bytes(_fr_mont_to_int(v), f"pc_proof[{q}].random_v")]
+    return parts
+
+
+def _verifying_key_parts(vk: CircuitVerifyingKey) -> list:
+    comms = np.ascontiguousarray(vk.circuit_commitments, dtype=np.uint64).reshape(-1, 18)
+    if comms.shape[0] != len(INDEX_POLYNOMIAL_NAMES) or vk.id is None or len(vk.id) != 32:
+        raise ValueError("a verifying key's bytes need its twelve commitments and its 32-byte circuit id")
+    return ([vk.circuit_info.to_bytes_le(), struct.pack("<Q", len(comms))]
+            + [(x, f"circuit_commitments[{n}]") for n, x in zip(INDEX_POLYNOMIAL_NAMES, comms)] + [bytes(vk.id)])
+
+
+def _certificate_parts(cert: Certificate) -> list:
+    return _batch_lc_parts([(cert.w, None)])
+
+
+def _to_bytes_many(parts_fn, objs, compress: bool, device_) -> list:
+    """every object's layout on the host, every point of every object through one device.g1_serialize call → bytes per object"""
+    layouts = [parts_fn(o) for o in objs]
+    pts = [_normalised(x, f"object {k}: {what}") for k, parts in enumerate(layouts) for x, what in
+           (q for q in parts if not isinstance(q, bytes))]
+    enc = []
+    if pts:
+        enc = device.g1_serialize(torch.from_numpy(np.stack(pts).view(np.int64)).to(torch.device(device_)), compress).cpu().numpy()
+    it = iter(enc)
+    return [b"".join(q if isinstance(q, bytes) else next(it).tobytes() for q in parts) for parts in layouts]
+
+
+def proofs_to_bytes(proofs: list, compress: bool = True, device_="cuda") -> list:
+    """Proof::serialize_with_mode of every proof (compressed: ToBytes), all points in one device call → [bytes]"""
+    return _to_bytes_many(_proof_parts, proofs, compress, device_)
+
+
+def proofs_from_bytes(blobs: list, compress: bool = True, validate: bool = True, device_="cuda") -> list:
+    """Proof::deserialize_with_mode of every blob (compressed: FromBytes; trailing bytes are ignored): one host walk gathers every
+    G1 point, one device call decodes them (device.g1_deserialize; with `validate` each also passes Affine::check) → [Proof].
+    ValueError names the lowest blob at fault and the field: bytes missing, an Option tag other than 0 or 1, an Fr not below r, a
+    count the bytes left cannot hold, or a point that does not decode (or, with `validate`, fails the check)."""
+    return _from_bytes_many(_walk_proof, blobs, [0] * len(blobs), compress, validate, device_)[0]
+
+
+def verifying_keys_from_bytes(blobs: list, compress: bool = True, validate: bool = True, device_="cuda") -> list:
+    """CircuitVerifyingKey::deserialize_with_mode of every blob, as proofs_from_bytes → [CircuitVerifyingKey]"""
+    return _from_bytes_many(_walk_verifying_key, blobs, [0] * len(blobs), compress, validate, device_)[0]
+
+
+def certificates_from_bytes(blobs: list, compress: bool = True, validate: bool = True, device_="cuda") -> list:
+    """Certificate::deserialize_with_mode of every blob, as proofs_from_bytes → [Certificate]"""
+    return _from_bytes_many(_walk_certificate, blobs, [0] * len(blobs), compress, validate, device_)[0]
