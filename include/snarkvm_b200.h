@@ -546,23 +546,62 @@ enum {
 };
 SNARKVM_API int snarkvm_b200_g1_validate_device(int32_t* d_status, const void* d_points, size_t n, size_t stride, void* stream);
 
+/* The byte forms of a G1 point: `form` of the two entry points below. */
+enum { SNARKVM_B200_G1_FORM_UNCOMPRESSED = 0, SNARKVM_B200_G1_FORM_COMPRESSED = 1, SNARKVM_B200_G1_FORM_TO_BYTES = 2 };
+
 /* G1 points from their byte forms (CanonicalDeserialize of Affine<G1>: curves/src/templates/macros.rs:118-144, SWFlags of
- * utilities/src/serialize/flags.rs).  d_bytes holds n points of 48 bytes (compressed: x little-endian, bit 7 of the last byte
- * PositiveY, bit 6 Infinity) or 96 bytes (uncompressed: x, then y with the flags; x carries none), no alignment needed.  d_points
- * (8-byte aligned, 104-byte stride) receives each point's Affine<G1> image and d_status[i] (device int32, 4-byte aligned) its
- * status: BAD_FLAGS (both flag bits set, or bit 7 of an uncompressed x), NOT_CANONICAL (a coordinate not below q after the flags
- * are masked), NOT_ON_CURVE (compressed: x³ + 1 has no square root in Fq), the first that applies; otherwise VALID, and with
- * `validate` the status of Affine::check as snarkvm_b200_g1_validate_device reports it.  Infinity decodes to Affine::zero()
- * (0, 1, infinity) whatever the coordinates below q were.  A compressed point's y is the root of x³ + 1 that is the larger of y, −y
- * (canonical integers) when PositiveY is set, the smaller otherwise.  An uncompressed point is not tested against the curve unless
- * `validate`.  Bytes that decode to no point leave an all-zero image.  One launch, one thread per point, no synchronisation. */
-SNARKVM_API int snarkvm_b200_g1_deserialize_device(void* d_points, int32_t* d_status, const void* d_bytes, size_t n, int compressed,
+ * utilities/src/serialize/flags.rs; FromBytes of Affine, short_weierstrass_jacobian/affine.rs:302-313).  d_bytes holds n points
+ * of 48 bytes (FORM_COMPRESSED: x little-endian, bit 7 of the last byte PositiveY, bit 6 Infinity), 96 bytes (FORM_UNCOMPRESSED: x,
+ * then y with the flags; x carries none) or 97 bytes (FORM_TO_BYTES: canonical x, canonical y, an infinity byte), no alignment
+ * needed.  d_points (8-byte aligned, 104-byte stride) receives each point's Affine<G1> image and d_status[i] (device int32, 4-byte
+ * aligned) its status: BAD_FLAGS (both flag bits set, or bit 7 of an uncompressed x; ToBytes: an infinity byte other than 0 or 1,
+ * or y = 1 with the infinity byte disagreeing with x = 0), NOT_CANONICAL (a coordinate not below q after the flags are masked),
+ * NOT_ON_CURVE (compressed: x³ + 1 has no square root in Fq), the first that applies; otherwise VALID, and with `validate` the
+ * status of Affine::check as snarkvm_b200_g1_validate_device reports it.  A compressed or uncompressed infinity decodes to
+ * Affine::zero() (0, 1, infinity) whatever the coordinates below q were; a ToBytes point keeps the x and y it was read with, so it
+ * writes back to the same bytes.  A compressed point's y is the root of x³ + 1 that is the larger of y, −y (canonical integers)
+ * when PositiveY is set, the smaller otherwise.  An uncompressed or ToBytes point is not tested against the curve unless
+ * `validate`.  Bytes that decode to no point leave an all-zero image.  Another form returns cudaErrorInvalidValue.  One launch,
+ * one thread per point, no synchronisation. */
+SNARKVM_API int snarkvm_b200_g1_deserialize_device(void* d_points, int32_t* d_status, const void* d_bytes, size_t n, int form,
                                                    int validate, void* stream);
-/* G1 points to their byte forms (CanonicalSerialize of Affine<G1>, macros.rs:67-97): d_projective holds n normalised projective
- * images (X, Y, Z Montgomery Fq, 144 bytes each, 8-byte aligned; Z = one, or Z = 0 for infinity); d_bytes receives 48 bytes per
- * point (compressed: canonical x, PositiveY iff y > −y; infinity: x = 0 with the Infinity bit) or 96 (uncompressed: canonical x and
- * y, no sign flag; infinity: x = 0, y = 1 with the Infinity bit).  One launch, one thread per point, no synchronisation. */
-SNARKVM_API int snarkvm_b200_g1_serialize_device(void* d_bytes, const void* d_projective, size_t n, int compressed, void* stream);
+/* G1 points to their byte forms (CanonicalSerialize of Affine<G1>, macros.rs:67-97; ToBytes of Affine, affine.rs:293-300).  For
+ * FORM_COMPRESSED and FORM_UNCOMPRESSED, d_points holds n normalised projective images (X, Y, Z Montgomery Fq, 144 bytes each,
+ * 8-byte aligned; Z = one, or Z = 0 for infinity); d_bytes receives 48 bytes per point (compressed: canonical x, PositiveY iff
+ * y > −y; infinity: x = 0 with the Infinity bit) or 96 (uncompressed: canonical x and y, no sign flag; infinity: x = 0, y = 1 with
+ * the Infinity bit).  For FORM_TO_BYTES, d_points holds n Affine<G1> images (104-byte stride, 8-byte aligned) and d_bytes receives
+ * 97 bytes per point: canonical x and y as the image holds them, then the infinity byte.  One launch, one thread per point, no
+ * synchronisation. */
+SNARKVM_API int snarkvm_b200_g1_serialize_device(void* d_bytes, const void* d_points, size_t n, int form, void* stream);
+
+/* One run of Fr records in a proving key's bytes (CanonicalSerialize of Circuit: snark/varuna/ahp/indexer/circuit.rs:158-237).
+ * stride 32: `count` canonical Fr at d_blob + offset, 32 bytes apart (an Evaluations vector).  stride 40: matrix entries, each a
+ * canonical Fr and a u64 column; with d_row_ptr (int32 [nrows + 1], device) `offset` is the matrix section (its u64 row count) and
+ * entry e of row i sits at offset + 16 + 8·i + 40·e.  d_out (16-byte aligned) receives count Montgomery Fr; for stride 40, d_cols
+ * (4-byte aligned) receives the columns as int32, each of which must be below num_cols (≤ 2^31). */
+typedef struct {
+    uint64_t offset, count;
+    uint32_t stride, reserved;
+    const void* d_row_ptr;
+    uint64_t nrows;
+    void* d_out;
+    void* d_cols;
+    uint64_t num_cols;
+} snarkvm_b200_fr_records_segment_t;
+enum { SNARKVM_B200_FR_RECORD_NOT_CANONICAL = 1, SNARKVM_B200_FR_RECORD_BAD_COLUMN = 2 };
+/* Every record of every segment (HOST table) decoded from d_blob (blob_bytes bytes in HBM, no alignment) in one launch and one
+ * synchronisation.  bad_record (HOST, count entries) receives per segment UINT64_MAX, or (e << 2) | reason for its first bad
+ * record e: NOT_CANONICAL (an Fr not below r; checked first) or BAD_COLUMN (a column ≥ num_cols).  The outputs of a bad record are
+ * unspecified.  A stride other than 32 or 40, a segment whose bytes leave the blob or a misaligned output returns
+ * cudaErrorInvalidValue before any launch. */
+SNARKVM_API int snarkvm_b200_fr_records_decode_device(const void* d_blob, size_t blob_bytes, const snarkvm_b200_fr_records_segment_t* segs,
+                                                      size_t count, uint64_t* bad_record, void* stream);
+/* A HOST function: the row headers of one matrix section (CanonicalSerialize of Vec<Vec<(Fr, u64)>>), after its u64 row count.
+ * `rows` holds `bytes` bytes (HOST); row i is a u64 length and that many 40-byte entries.  row_ptr (HOST, nrows + 1 int32)
+ * receives the CSR row starts.  A row whose header or entries overrun `bytes`, or whose length carries the count past nnz, returns
+ * cudaErrorInvalidValue with *bad_row = i; a total below nnz, with *bad_row = nrows; nnz ≥ 2^31, with *bad_row = −1. */
+SNARKVM_API int snarkvm_b200_matrix_row_walk(const void* rows, size_t bytes, uint64_t nrows, uint64_t nnz, int32_t* row_ptr,
+                                             int64_t* bad_row);
 
 #ifdef __cplusplus
 }

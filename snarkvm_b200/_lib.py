@@ -40,7 +40,8 @@ SYMBOLS = (
     "snarkvm_b200_varuna_round4_evals_device", "snarkvm_b200_g2_prepare_device", "snarkvm_b200_pairing_products_device",
     "snarkvm_b200_test_tower_op_device", "snarkvm_b200_poseidon_transcripts_device",
     "snarkvm_b200_poseidon_transcripts_resume_device", "snarkvm_b200_g1_validate_device",
-    "snarkvm_b200_g1_deserialize_device", "snarkvm_b200_g1_serialize_device",
+    "snarkvm_b200_g1_deserialize_device", "snarkvm_b200_g1_serialize_device", "snarkvm_b200_fr_records_decode_device",
+    "snarkvm_b200_matrix_row_walk",
 )
 
 
@@ -92,6 +93,13 @@ class Round4Segment(ctypes.Structure):
     _fields_ = [("d_row", ctypes.c_void_p), ("d_col", ctypes.c_void_p), ("d_row_col_val", ctypes.c_void_p), ("n", ctypes.c_uint64),
                 ("v_rc_mont", ctypes.c_uint8 * 32), ("rc_mont", ctypes.c_uint8 * 32), ("f_scale_mont", ctypes.c_uint8 * 32),
                 ("d_a", ctypes.c_void_p), ("d_b", ctypes.c_void_p), ("d_f", ctypes.c_void_p)]
+
+
+class FrRecordsSegment(ctypes.Structure):
+    """snarkvm_b200_fr_records_segment_t"""
+    _fields_ = [("offset", ctypes.c_uint64), ("count", ctypes.c_uint64), ("stride", ctypes.c_uint32), ("reserved", ctypes.c_uint32),
+                ("d_row_ptr", ctypes.c_void_p), ("nrows", ctypes.c_uint64), ("d_out", ctypes.c_void_p), ("d_cols", ctypes.c_void_p),
+                ("num_cols", ctypes.c_uint64)]
 
 
 class CudaError(RuntimeError):
@@ -191,6 +199,8 @@ def lib():
     L.snarkvm_b200_g1_validate_device.argtypes = [vp, vp, sz, sz, vp]
     L.snarkvm_b200_g1_deserialize_device.argtypes = [vp, vp, vp, sz, i32, i32, vp]
     L.snarkvm_b200_g1_serialize_device.argtypes = [vp, vp, sz, i32, vp]
+    L.snarkvm_b200_fr_records_decode_device.argtypes = [vp, sz, ctypes.POINTER(FrRecordsSegment), sz, ctypes.POINTER(u64), vp]
+    L.snarkvm_b200_matrix_row_walk.argtypes = [vp, sz, u64, u64, vp, ctypes.POINTER(ctypes.c_int64)]
     L.snarkvm_b200_msm_batch_device.argtypes = [vp, vp, sz, vp, vp, sz, vp]
     L.snarkvm_b200_msm_window_sums_plan_device.argtypes = [vp, vp, sz, vp, sz, vp, sz, vp]
     L.snarkvm_b200_kzg_commit_batch_hiding_device.argtypes = [vp, vp, sz, vp, vp, vp, vp, vp, sz, vp]

@@ -1,15 +1,21 @@
 // G1 points that reach the verifier from outside: validation (Affine::check: curves/src/templates/short_weierstrass_jacobian/
 // affine.rs, is_on_curve and is_in_correct_subgroup_assuming_on_curve of curves/src/bls12_377/g1.rs:98-106) and the byte forms
 // (CanonicalSerialize / CanonicalDeserialize of Affine<G1>, curves/src/templates/macros.rs:67-144, SWFlags of
-// utilities/src/serialize/flags.rs).
+// utilities/src/serialize/flags.rs; ToBytes / FromBytes of Affine, short_weierstrass_jacobian/affine.rs:293-313).  Also the Fr
+// records of a proving key's byte form (matrix entries and evaluations, CanonicalSerialize of Circuit) and its matrix row walk.
 //
 //   k_g1_validate      one thread per point: coordinates below q, y² = x³ + 1, then [x²]·φ(P) + P = O with φ(x, y) = (PHI·x, y)
-//   k_g1_deserialize   one thread per point: 48 compressed or 96 uncompressed bytes → Affine image and status; a compressed point's
-//                      y is the square root of x³ + 1 (Tonelli–Shanks) whose sign the PositiveY flag picks
-//   k_g1_serialize     one thread per point: normalised projective image → the compressed or uncompressed bytes
+//   k_g1_deserialize   one thread per point: 48 compressed, 96 uncompressed or 97 ToBytes bytes → Affine image and status; a
+//                      compressed point's y is the square root of x³ + 1 (Tonelli–Shanks) whose sign the PositiveY flag picks
+//   k_g1_serialize     one thread per point: normalised projective image → the compressed or uncompressed bytes, or Affine image →
+//                      the 97 ToBytes bytes
+//   k_fr_records       one thread per record of every segment: canonical Fr (and column) → Montgomery Fr (and int32 column)
 //
 // The subgroup test is the reference's: x² (x = 0x8508c00000000001, the BLS parameter) is 127 bits, so the chain is 126 doublings
 // and one mixed addition per set bit of x² in XYZZ coordinates, then one mixed addition of P.
+#include <cstring>
+#include <vector>
+
 #include "ec.cuh"
 #include "msm.cuh"
 #include "../../include/snarkvm_b200.h"
@@ -123,14 +129,30 @@ FF_DEV bool fq_above_half(const Fq& a) {
 constexpr uint8_t FLAG_POSITIVE_Y = 0x80, FLAG_INFINITY = 0x40;
 
 __global__ void __launch_bounds__(128) k_g1_deserialize(uint8_t* __restrict__ points, int32_t* __restrict__ status,
-                                                        const uint8_t* __restrict__ bytes, size_t n, int compressed, int validate) {
+                                                        const uint8_t* __restrict__ bytes, size_t n, int form, int validate) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     AffinePoint p;
     p.x = Fq::zero(); p.y = Fq::zero(); p.inf = false;            // the image of bytes that decode to no point
     int32_t s = SNARKVM_B200_G1_VALID;
     bool decoded = false;
-    if (compressed) {
+    if (form == SNARKVM_B200_G1_FORM_TO_BYTES) {
+        // FromBytes for Affine: x, y (Fq::read_le: below q), the infinity flag (bool::read_le: 0 or 1), then the only test the
+        // reference makes, `infinity != x.is_zero() && y.is_one()` refused; Affine::new keeps x and y, infinity included
+        const uint8_t* src = bytes + i * 97;
+        const Fq x = fq_from_bytes(src, 0xFF), y = fq_from_bytes(src + 48, 0xFF);
+        const uint8_t inf = src[96];
+        Fq one_raw = Fq::zero();
+        one_raw.v[0] = 1u;
+        if (!fq_is_canonical(x) || !fq_is_canonical(y)) {
+            s = SNARKVM_B200_G1_NOT_CANONICAL;
+        } else if (inf > 1 || ((inf == 1) != x.is_zero() && y == one_raw)) {
+            s = SNARKVM_B200_G1_BAD_FLAGS;
+        } else {
+            p.x = x.to_mont(); p.y = y.to_mont(); p.inf = inf == 1;
+            decoded = true;
+        }
+    } else if (form == SNARKVM_B200_G1_FORM_COMPRESSED) {
         const uint8_t* src = bytes + i * 48;
         const uint8_t flags = src[47] & 0xC0;
         const Fq x = fq_from_bytes(src, 0x3F);
@@ -179,9 +201,18 @@ __global__ void __launch_bounds__(128) k_g1_deserialize(uint8_t* __restrict__ po
 }
 
 __global__ void __launch_bounds__(128) k_g1_serialize(uint8_t* __restrict__ bytes, const uint8_t* __restrict__ projective, size_t n,
-                                                      int compressed) {
+                                                      int form) {
     const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
+    if (form == SNARKVM_B200_G1_FORM_TO_BYTES) {                  // ToBytes of the Affine image: x, y as held, the infinity byte
+        const AffinePoint a = load_affine(projective, 104, i);
+        uint8_t* dst = bytes + i * 97;
+        fq_to_bytes(dst, a.x.from_mont(), 0);
+        fq_to_bytes(dst + 48, a.y.from_mont(), 0);
+        dst[96] = a.inf ? 1 : 0;
+        return;
+    }
+    const bool compressed = form == SNARKVM_B200_G1_FORM_COMPRESSED;
     const uint8_t* src = projective + i * 144;
     const Fq X = load_fq_u64(src), Y = load_fq_u64(src + 48), Z = load_fq_u64(src + 96);
     Fq x = Fq::zero(), y = Fq::zero();
@@ -201,6 +232,68 @@ __global__ void __launch_bounds__(128) k_g1_serialize(uint8_t* __restrict__ byte
     }
 }
 
+// A run of Fr records in a proving key's bytes.  Thread g takes record g − first of its segment: record e sits at src + stride·e,
+// or — a matrix entry, row_ptr set — at src + 16 + 8·row(e) + 40·e (the u64 row count, then per row a u64 length and the row's
+// entries).  The row is searched in [0, nrows), so a row_ptr that disagrees with the section cannot move a read past the extent
+// the host checked.  The first bad record of a segment wins an atomicMin of (e << 2 | reason).
+struct FrRecordSeg {
+    uint64_t first, src, count;
+    uint32_t stride, nrows;
+    const uint32_t* row_ptr;
+    uint32_t* out;
+    int32_t* cols;
+    uint64_t num_cols;
+};
+constexpr unsigned long long FR_RECORD_NOT_CANONICAL = 1, FR_RECORD_BAD_COLUMN = 2;
+
+FF_DEV bool fr_is_canonical(const Fr& a) {
+    (void)ptx_sub_cc(a.v[0], FrParams::mod(0));
+#pragma unroll
+    for (int k = 1; k < 8; k++) (void)ptx_subc_cc(a.v[k], FrParams::mod(k));
+    return ptx_subc(0u, 0u) != 0u;
+}
+
+__global__ void __launch_bounds__(256) k_fr_records(const FrRecordSeg* __restrict__ segs, uint32_t nsegs, uint64_t total,
+                                                    const uint8_t* __restrict__ blob, unsigned long long* __restrict__ bad) {
+    const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= total) return;
+    uint32_t lo = 0, hi = nsegs;                                  // the last segment whose `first` is ≤ g
+    while (hi - lo > 1) {
+        const uint32_t mid = lo + (hi - lo) / 2;
+        if (segs[mid].first <= g) lo = mid; else hi = mid;
+    }
+    const FrRecordSeg& sg = segs[lo];
+    const uint64_t e = g - sg.first;
+    uint64_t at = sg.src + (uint64_t)sg.stride * e;
+    if (sg.row_ptr) {
+        uint32_t rlo = 0, rhi = sg.nrows;                         // the last row whose start is ≤ e
+        while (rhi - rlo > 1) {
+            const uint32_t mid = rlo + (rhi - rlo) / 2;
+            if (__ldg(sg.row_ptr + mid) <= e) rlo = mid; else rhi = mid;
+        }
+        at = sg.src + 16 + 8 * (uint64_t)rlo + 40 * e;
+    }
+    const uint8_t* p = blob + at;
+    Fr v;
+#pragma unroll
+    for (int k = 0; k < 8; k++)
+        v.v[k] = (uint32_t)p[4 * k] | ((uint32_t)p[4 * k + 1] << 8) | ((uint32_t)p[4 * k + 2] << 16) | ((uint32_t)p[4 * k + 3] << 24);
+    unsigned long long reason = 0;
+    if (!fr_is_canonical(v)) {
+        reason = FR_RECORD_NOT_CANONICAL;
+        v = Fr::zero();
+    }
+    if (sg.cols) {
+        uint64_t c = 0;
+#pragma unroll
+        for (int k = 0; k < 8; k++) c |= (uint64_t)p[32 + k] << (8 * k);
+        if (c >= sg.num_cols && !reason) reason = FR_RECORD_BAD_COLUMN;
+        sg.cols[e] = c < sg.num_cols ? (int32_t)c : 0;
+    }
+    v.to_mont().store(sg.out + 8 * e);
+    if (reason) atomicMin(bad + lo, (e << 2) | reason);
+}
+
 }  // namespace
 }  // namespace b200
 
@@ -216,25 +309,94 @@ extern "C" int snarkvm_b200_g1_validate_device(int32_t* d_status, const void* d_
     return (int)cudaGetLastError();
 }
 
-extern "C" int snarkvm_b200_g1_deserialize_device(void* d_points, int32_t* d_status, const void* d_bytes, size_t n, int compressed,
+extern "C" int snarkvm_b200_g1_deserialize_device(void* d_points, int32_t* d_status, const void* d_bytes, size_t n, int form,
                                                   int validate, void* stream) {
     using namespace b200;
     if (n == 0) return 0;
-    if (!d_points || !d_status || !d_bytes || ((uintptr_t)d_points & 7) || ((uintptr_t)d_status & 3) || n > ((size_t)1 << 31))
+    if (!d_points || !d_status || !d_bytes || ((uintptr_t)d_points & 7) || ((uintptr_t)d_status & 3) || n > ((size_t)1 << 31) ||
+        form < SNARKVM_B200_G1_FORM_UNCOMPRESSED || form > SNARKVM_B200_G1_FORM_TO_BYTES)
         return (int)cudaErrorInvalidValue;
     const unsigned blocks = (unsigned)((n + 127) / 128);
-    k_g1_deserialize<<<blocks, 128, 0, (cudaStream_t)stream>>>((uint8_t*)d_points, d_status, (const uint8_t*)d_bytes, n,
-                                                               compressed ? 1 : 0, validate ? 1 : 0);
+    k_g1_deserialize<<<blocks, 128, 0, (cudaStream_t)stream>>>((uint8_t*)d_points, d_status, (const uint8_t*)d_bytes, n, form,
+                                                               validate ? 1 : 0);
     count_launch();
     return (int)cudaGetLastError();
 }
 
-extern "C" int snarkvm_b200_g1_serialize_device(void* d_bytes, const void* d_projective, size_t n, int compressed, void* stream) {
+extern "C" int snarkvm_b200_g1_serialize_device(void* d_bytes, const void* d_points, size_t n, int form, void* stream) {
     using namespace b200;
     if (n == 0) return 0;
-    if (!d_bytes || !d_projective || ((uintptr_t)d_projective & 7) || n > ((size_t)1 << 31)) return (int)cudaErrorInvalidValue;
+    if (!d_bytes || !d_points || ((uintptr_t)d_points & 7) || n > ((size_t)1 << 31) || form < SNARKVM_B200_G1_FORM_UNCOMPRESSED ||
+        form > SNARKVM_B200_G1_FORM_TO_BYTES)
+        return (int)cudaErrorInvalidValue;
     const unsigned blocks = (unsigned)((n + 127) / 128);
-    k_g1_serialize<<<blocks, 128, 0, (cudaStream_t)stream>>>((uint8_t*)d_bytes, (const uint8_t*)d_projective, n, compressed ? 1 : 0);
+    k_g1_serialize<<<blocks, 128, 0, (cudaStream_t)stream>>>((uint8_t*)d_bytes, (const uint8_t*)d_points, n, form);
     count_launch();
     return (int)cudaGetLastError();
+}
+
+extern "C" int snarkvm_b200_fr_records_decode_device(const void* d_blob, size_t blob_bytes, const snarkvm_b200_fr_records_segment_t* segs,
+                                                     size_t count, uint64_t* bad_record, void* stream) {
+    using namespace b200;
+    if (count == 0) return 0;
+    if (!d_blob || !segs || !bad_record || count >= ((size_t)1 << 31)) return (int)cudaErrorInvalidValue;
+    std::vector<FrRecordSeg> table(count);
+    uint64_t total = 0;
+    for (size_t i = 0; i < count; i++) {
+        const snarkvm_b200_fr_records_segment_t& s = segs[i];
+        FrRecordSeg& t = table[i];
+        const bool matrix = s.d_row_ptr != nullptr;
+        if ((s.stride != 32 && s.stride != 40) || (s.count && !s.d_out) || ((uintptr_t)s.d_out & 15) || s.count >= ((uint64_t)1 << 32))
+            return (int)cudaErrorInvalidValue;
+        if ((s.stride == 40) != (s.d_cols != nullptr) || (matrix && (s.stride != 40 || s.nrows == 0 || s.nrows >= ((uint64_t)1 << 32))) ||
+            ((uintptr_t)s.d_cols & 3) || (s.d_cols && s.num_cols > ((uint64_t)1 << 31)))
+            return (int)cudaErrorInvalidValue;
+        // the extent every read of the segment stays inside
+        const uint64_t extent = matrix ? 8 + 8 * s.nrows + 40 * s.count : (uint64_t)s.stride * s.count;
+        if (s.offset > blob_bytes || extent > blob_bytes - s.offset) return (int)cudaErrorInvalidValue;
+        t = FrRecordSeg{total, s.offset, s.count, s.stride, (uint32_t)s.nrows, (const uint32_t*)s.d_row_ptr, (uint32_t*)s.d_out,
+                        (int32_t*)s.d_cols, s.num_cols};
+        total += s.count;
+    }
+    cudaStream_t st = (cudaStream_t)stream;
+    const size_t nbad = (count * sizeof(unsigned long long) + 255) & ~(size_t)255;
+    uint8_t* scratch = nullptr;
+    cudaError_t e = pool_alloc(&scratch, nbad + count * sizeof(FrRecordSeg), st);
+    if (e != cudaSuccess) return (int)e;
+    unsigned long long* d_bad = (unsigned long long*)scratch;
+    FrRecordSeg* d_table = (FrRecordSeg*)(scratch + nbad);
+    int rc = (int)cudaMemsetAsync(d_bad, 0xFF, count * sizeof(unsigned long long), st);
+    if (rc == 0) rc = (int)cudaMemcpyAsync(d_table, table.data(), count * sizeof(FrRecordSeg), cudaMemcpyHostToDevice, st);
+    if (rc == 0 && total) {
+        k_fr_records<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(d_table, (uint32_t)count, total, (const uint8_t*)d_blob, d_bad);
+        count_launch();
+        rc = (int)cudaGetLastError();
+    }
+    if (rc == 0) rc = (int)cudaMemcpyAsync(bad_record, d_bad, count * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st);
+    cudaFreeAsync(scratch, st);
+    if (rc == 0) rc = (int)cudaStreamSynchronize(st);
+    return rc;
+}
+
+// The row headers of one matrix section, walked on the host: a chain of lengths, each locating the next.  Bounds-checked against
+// the bytes the caller holds, so a length cannot carry the walk past them.
+extern "C" int snarkvm_b200_matrix_row_walk(const void* rows, size_t bytes, uint64_t nrows, uint64_t nnz, int32_t* row_ptr,
+                                            int64_t* bad_row) {
+    if (bad_row) *bad_row = -1;
+    if (!row_ptr || (nrows && !rows) || nnz >= ((uint64_t)1 << 31)) return (int)cudaErrorInvalidValue;
+    const uint8_t* p = (const uint8_t*)rows;
+    uint64_t at = 0, total = 0;
+    row_ptr[0] = 0;
+    for (uint64_t i = 0; i < nrows; i++) {
+        uint64_t len = 0;
+        if (bytes - at < 8) { if (bad_row) *bad_row = (int64_t)i; return (int)cudaErrorInvalidValue; }
+        std::memcpy(&len, p + at, 8);
+        at += 8;
+        if (len > (bytes - at) / 40 || len > nnz - total) { if (bad_row) *bad_row = (int64_t)i; return (int)cudaErrorInvalidValue; }
+        at += 40 * len;
+        total += len;
+        row_ptr[i + 1] = (int32_t)total;
+    }
+    if (total != nnz) { if (bad_row) *bad_row = (int64_t)nrows; return (int)cudaErrorInvalidValue; }
+    return 0;
 }

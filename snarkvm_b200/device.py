@@ -166,7 +166,17 @@ def pairing_products(g1: torch.Tensor, g2_index: torch.Tensor, prepared: torch.T
 
 
 G1_VALID, G1_NOT_CANONICAL, G1_NOT_ON_CURVE, G1_NOT_IN_SUBGROUP, G1_BAD_FLAGS = 0, 1, 2, 3, 4
-G1_COMPRESSED_BYTES, G1_UNCOMPRESSED_BYTES = 48, 96
+G1_COMPRESSED_BYTES, G1_UNCOMPRESSED_BYTES, G1_TO_BYTES_BYTES = 48, 96, 97
+# the byte forms of a G1 point (SNARKVM_B200_G1_FORM_*): False / True name the first two, as `compressed` flags
+G1_UNCOMPRESSED, G1_COMPRESSED, G1_TO_BYTES = 0, 1, 2
+_G1_FORM_BYTES = {G1_UNCOMPRESSED: G1_UNCOMPRESSED_BYTES, G1_COMPRESSED: G1_COMPRESSED_BYTES, G1_TO_BYTES: G1_TO_BYTES_BYTES}
+
+
+def _g1_form(compressed) -> int:
+    form = int(compressed)
+    if form not in _G1_FORM_BYTES:
+        raise ValueError(f"unknown G1 byte form {compressed!r}")
+    return form
 
 
 def g1_validate(points: torch.Tensor, stride: int = AFFINE_STRIDE) -> torch.Tensor:
@@ -180,12 +190,15 @@ def g1_validate(points: torch.Tensor, stride: int = AFFINE_STRIDE) -> torch.Tens
     return status
 
 
-def g1_deserialize(bytes_u8: torch.Tensor, compressed: bool = True, validate: bool = True):
-    """G1 points from their byte forms (snarkvm_b200_g1_deserialize_device): `bytes_u8` a uint8 CUDA tensor of n × 48 compressed
-    or n × 96 uncompressed bytes → (Affine<G1> images uint8 [n, 104], int32 status [n]), both in HBM.  Status G1_BAD_FLAGS (both
-    flag bits set, or bit 7 of an uncompressed x), G1_NOT_CANONICAL (a coordinate ≥ q), G1_NOT_ON_CURVE (compressed: x³ + 1 has no
-    square root), else G1_VALID or, with `validate`, g1_validate's status.  Bytes that decode to no point leave an all-zero image."""
-    size = G1_COMPRESSED_BYTES if compressed else G1_UNCOMPRESSED_BYTES
+def g1_deserialize(bytes_u8: torch.Tensor, compressed=True, validate: bool = True):
+    """G1 points from their byte forms (snarkvm_b200_g1_deserialize_device): `bytes_u8` a uint8 CUDA tensor of n × 48 compressed,
+    n × 96 uncompressed or (compressed = G1_TO_BYTES) n × 97 ToBytes bytes → (Affine<G1> images uint8 [n, 104], int32 status [n]),
+    both in HBM.  Status G1_BAD_FLAGS (both flag bits set, or bit 7 of an uncompressed x; ToBytes: an infinity byte above 1, or
+    y = 1 with the infinity byte disagreeing with x = 0), G1_NOT_CANONICAL (a coordinate ≥ q), G1_NOT_ON_CURVE (compressed: x³ + 1
+    has no square root), else G1_VALID or, with `validate`, g1_validate's status.  Bytes that decode to no point leave an all-zero
+    image; a ToBytes infinity keeps the coordinates it was read with."""
+    form = _g1_form(compressed)
+    size = _G1_FORM_BYTES[form]
     if bytes_u8.dtype != torch.uint8 or _nbytes(bytes_u8) % size:
         raise ValueError(f"g1_deserialize takes uint8 bytes, {size} per point")
     n = _nbytes(bytes_u8) // size
@@ -194,24 +207,79 @@ def g1_deserialize(bytes_u8: torch.Tensor, compressed: bool = True, validate: bo
     if n:
         with torch.cuda.device(bytes_u8.device):
             _lib.check(_lib.lib().snarkvm_b200_g1_deserialize_device(images.data_ptr(), status.data_ptr(), _check(bytes_u8, "bytes_u8"),
-                                                                     n, int(bool(compressed)), int(bool(validate)), _stream()))
+                                                                     n, form, int(bool(validate)), _stream()))
     return images, status
 
 
-def g1_serialize(projective: torch.Tensor, compressed: bool = True) -> torch.Tensor:
+def g1_serialize(projective: torch.Tensor, compressed=True) -> torch.Tensor:
     """G1 points to their byte forms (snarkvm_b200_g1_serialize_device): `projective` a CUDA tensor of n normalised projective
     images (X, Y, Z Montgomery Fq, 144 bytes each; Z = one, or zero for infinity) → uint8 [n, 48] compressed or [n, 96]
-    uncompressed, in HBM"""
-    if _nbytes(projective) % 144:
-        raise ValueError("g1_serialize takes 144-byte normalised projective images")
-    n = _nbytes(projective) // 144
-    size = G1_COMPRESSED_BYTES if compressed else G1_UNCOMPRESSED_BYTES
+    uncompressed, in HBM.  With compressed = G1_TO_BYTES, `projective` holds Affine<G1> images (104 bytes each) instead → uint8
+    [n, 97], their ToBytes form."""
+    form = _g1_form(compressed)
+    image = AFFINE_STRIDE if form == G1_TO_BYTES else 144
+    if _nbytes(projective) % image:
+        raise ValueError(f"g1_serialize takes {image}-byte images in this form")
+    n = _nbytes(projective) // image
+    size = _G1_FORM_BYTES[form]
     out = torch.empty((n, size), dtype=torch.uint8, device=projective.device)
     if n:
         with torch.cuda.device(projective.device):
             _lib.check(_lib.lib().snarkvm_b200_g1_serialize_device(out.data_ptr(), _check(projective, "projective"), n,
-                                                                   int(bool(compressed)), _stream()))
+                                                                   form, _stream()))
     return out
+
+
+FR_RECORD_NOT_CANONICAL, FR_RECORD_BAD_COLUMN = 1, 2
+
+
+def fr_records_decode(blob: torch.Tensor, segments: list) -> list:
+    """Fr records of a byte blob in HBM (snarkvm_b200_fr_records_decode_device), every segment in one launch and one
+    synchronisation.  A segment is (offset, count, stride, out, cols, num_cols, row_ptr): `count` canonical Fr 32 bytes apart
+    (stride 32) or Fr-and-u64-column entries (stride 40), written to `out` ([count, 4] int64 CUDA tensor, Montgomery) and, for
+    stride 40, the columns to `cols` (int32 [count]), each checked below num_cols.  With `row_ptr` (int32 [nrows + 1] CUDA tensor)
+    the segment is a matrix section at `offset` whose entry e of row i sits at offset + 16 + 8·i + 40·e.  → per segment None, or
+    (index, FR_RECORD_NOT_CANONICAL or FR_RECORD_BAD_COLUMN) of its first bad record."""
+    if blob.dtype != torch.uint8:
+        raise TypeError("blob must be a uint8 tensor")
+    if not segments:
+        return []
+    segs = (_lib.FrRecordsSegment * len(segments))()
+    for k, (offset, count, stride, out, cols, num_cols, row_ptr) in enumerate(segments):
+        if _nbytes(out) != 32 * count or (cols is not None and (cols.dtype != torch.int32 or cols.numel() != count)):
+            raise ValueError(f"segment {k}: one 32-byte output and one int32 column per record")
+        s = segs[k]
+        s.offset, s.count, s.stride = offset, count, stride
+        s.d_out = _check(out, "out") if count else None
+        s.d_cols = _check(cols, "cols") if cols is not None and count else None
+        s.num_cols = num_cols
+        if row_ptr is not None:
+            if row_ptr.dtype != torch.int32:
+                raise TypeError("row_ptr must be an int32 tensor")
+            s.d_row_ptr, s.nrows = _check(row_ptr, "row_ptr"), row_ptr.numel() - 1
+    bad = (ctypes.c_uint64 * len(segments))()
+    with torch.cuda.device(blob.device):
+        _lib.check(_lib.lib().snarkvm_b200_fr_records_decode_device(_check(blob, "blob"), _nbytes(blob), segs, len(segments), bad,
+                                                                    _stream()))
+    return [None if v == 2**64 - 1 else (v >> 2, v & 3) for v in bad]
+
+
+def matrix_row_walk(blob, offset: int, nrows: int, nnz: int):
+    """the row headers of one matrix section of a HOST buffer (snarkvm_b200_matrix_row_walk): its rows start at byte `offset` of
+    `blob` (anything with the buffer protocol; no copy) → (int32 row_ptr [nrows + 1] as a numpy array, None), or (None, the first
+    row that overruns the buffer or carries the count past nnz; nrows when the rows hold fewer than nnz entries)"""
+    buf = np.frombuffer(blob, dtype=np.uint8)
+    if not 0 <= offset <= buf.size:
+        raise ValueError("offset outside the buffer")
+    if nnz >= 2**31:
+        return None, -1
+    row_ptr = np.empty(nrows + 1, dtype=np.int32)
+    bad = ctypes.c_int64(-1)
+    code = _lib.lib().snarkvm_b200_matrix_row_walk(buf.ctypes.data + offset if nrows else None, buf.size - offset, nrows, nnz,
+                                                   row_ptr.ctypes.data, ctypes.byref(bad))
+    if code != 0:
+        return None, bad.value
+    return row_ptr, None
 
 
 POSEIDON_ABSORB, POSEIDON_SQUEEZE, POSEIDON_SQUEEZE_NONNATIVE, POSEIDON_SQUEEZE_SHORT_NONNATIVE = 0, 1, 2, 3

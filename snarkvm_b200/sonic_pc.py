@@ -20,6 +20,10 @@ consumed in the reference's squeeze order.
 """
 from __future__ import annotations
 
+import hashlib
+import struct
+import warnings
+from concurrent.futures import ThreadPoolExecutor
 from dataclasses import dataclass, field
 
 import numpy as np
@@ -87,7 +91,7 @@ class CommitterKey:
     shifted_powers_of_beta_g: torch.Tensor | None = None             # pp.powers[max_degree − highest bound …]
     shifted_powers_of_beta_times_gamma_g: dict | None = None         # bound → gamma powers of that shift
     enforced_degree_bounds: list | None = None
-    max_degree: int = 0
+    max_degree: int | None = 0        # the SRS's degree; None for a key read from bytes, whose byte form does not carry it
 
     @classmethod
     def trim(cls, pp_powers_of_beta_g: torch.Tensor, pp_powers_of_beta_times_gamma_g: torch.Tensor, supported_degree: int,
@@ -133,13 +137,43 @@ class CommitterKey:
             raise ValueError(f"UnsupportedLagrangeBasisSize({size})")
         return self.lagrange_bases_at_beta_g[size], self.powers_of_beta_times_gamma_g
 
+    def to_bytes(self) -> bytes:
+        """ToBytes (data_structures.rs:186-265): every point in its 97-byte form through one device.g1_serialize call, then the
+        SHA-256 of the point sections"""
+        return committer_keys_to_bytes([self])[0]
+
+    @staticmethod
+    def read(blob, offset: int = 0, validate: bool = True, device_="cuda"):
+        """FromBytes (data_structures.rs:65-184) of the key whose bytes start at `offset` of `blob` → (CommitterKey, the offset after
+        it).  The host walks the headers only (no copy of `blob`); the key's bytes go to the device once and every point is decoded
+        there by one device.g1_deserialize call (with `validate`, each also passes Affine::check).  ValueError names the field and
+        the element: bytes missing, a bool other than 0 or 1, a coordinate not below q, an infinity byte the reference refuses, a
+        SHA-256 that differs from the points', and — stricter than the reference — the keys of the Lagrange bases or of the shifted
+        γ powers not strictly increasing (ToBytes writes a BTreeMap in order) and, with `validate`, a point off the curve or outside
+        the subgroup.  max_degree is None: the byte form does not carry the SRS's degree."""
+        mv = memoryview(blob).cast("B")
+        r = ByteReader(mv, offset, "committer key")
+        layout = walk_committer_key(r)
+        with ThreadPoolExecutor(1) as pool:
+            digest = pool.submit(layout.sha256, mv)
+            d_blob = upload(mv[offset: r.o], torch.empty(r.o - offset, dtype=torch.uint8, device=torch.device(device_)))
+            runs = [(o - offset, n) for o, n in layout.runs()]
+            images, status = device.g1_deserialize(gather_records(d_blob, runs, POINT_BYTES), device.G1_TO_BYTES, validate)
+            bad = first_bad_point(status, layout.fields(), POINT_BYTES)
+            if bad is not None:
+                raise ValueError(f"committer key: {bad[1]}")
+            if digest.result() != bytes(mv[layout.hash_offset: layout.hash_offset + 32]):
+                raise ValueError("committer key: hash: the SHA-256 of the points differs")
+        return layout.build(images), r.o
+
 
 def _check_degrees_and_bounds(ck: CommitterKey, p: LabeledPolynomial) -> None:
     """kzg10/mod.rs check_degrees_and_bounds: a bounded polynomial needs degree ≤ bound ≤ max_degree and an enforced bound"""
     if p.degree_bound is not None:
         if ck.enforced_degree_bounds is None or p.degree_bound not in ck.enforced_degree_bounds:
             raise ValueError(f"UnsupportedDegreeBound({p.degree_bound})")
-        if p.polynomial.shape[0] - 1 > p.degree_bound or p.degree_bound > ck.max_degree:
+        # a key read from bytes has no max_degree: its enforced bounds, all within its SRS, stand for it
+        if p.polynomial.shape[0] - 1 > p.degree_bound or (ck.max_degree is not None and p.degree_bound > ck.max_degree):
             raise ValueError(f"IncorrectDegreeBound for {p.label}")
 
 
@@ -304,3 +338,228 @@ def synthetic_srs(max_degree: int, beta: int, gamma: int, dev="cuda"):
     commitment can be checked in the scalar field: commit(p, r) = (p(β) + γ·r(β))·G.  Built on the device from the generator by
     one fixed-base pass (device.generate_powers)."""
     return device.generate_powers(max_degree + 1, beta, 1, dev), device.generate_powers(max_degree + 2, beta, gamma, dev)
+
+
+# ---- byte form: ToBytes / FromBytes of CommitterKey (data_structures.rs:65-265) ----
+POINT_BYTES = device.G1_TO_BYTES_BYTES
+_G1_STATUS = {device.G1_NOT_CANONICAL: "a coordinate not below q", device.G1_NOT_ON_CURVE: "not on the curve",
+              device.G1_NOT_IN_SUBGROUP: "not in the prime-order subgroup", device.G1_BAD_FLAGS: "an infinity byte the reference refuses"}
+
+
+class ByteReader:
+    """bounds-checked little-endian header reads from `offset` of a memoryview; every failure is a ValueError naming `name` and
+    the field"""
+
+    def __init__(self, mv: memoryview, offset: int, name: str):
+        self.mv, self.o, self.name = mv, int(offset), name
+        if not 0 <= self.o <= len(mv):
+            raise ValueError(f"{name}: offset {offset} is outside the blob")
+
+    def fail(self, field: str, what: str) -> ValueError:
+        return ValueError(f"{self.name}: {field}: {what}")
+
+    def need(self, n: int, field: str) -> None:
+        if n > len(self.mv) - self.o:
+            raise self.fail(field, f"{len(self.mv) - self.o} bytes left, at least {n} needed")
+
+    def take(self, n: int, field: str) -> memoryview:
+        self.need(n, field)
+        self.o += n
+        return self.mv[self.o - n: self.o]
+
+    def u32(self, field: str) -> int:
+        return struct.unpack("<I", self.take(4, field))[0]
+
+    def u64(self, field: str) -> int:
+        return struct.unpack("<Q", self.take(8, field))[0]
+
+    def tag(self, field: str) -> bool:
+        """bool::read_le, also an Option's tag: 0 or 1"""
+        t = self.take(1, field)[0]
+        if t > 1:
+            raise self.fail(field, f"{t} is neither 0 nor 1")
+        return t == 1
+
+
+def upload(mv: memoryview, out: torch.Tensor) -> torch.Tensor:
+    """one copy of host bytes into the uint8 device tensor `out` of their length, without a host copy first → out"""
+    if len(mv):
+        with warnings.catch_warnings():
+            warnings.simplefilter("ignore")                  # a read-only buffer is only read here
+            out.copy_(torch.from_numpy(np.frombuffer(mv, dtype=np.uint8)))
+    return out
+
+
+def gather_records(d_blob: torch.Tensor, runs: list, size: int) -> torch.Tensor:
+    """the `size`-byte records of every run (byte offset in d_blob, count), concatenated in run order by one gather → uint8
+    [records · size] on d_blob's device"""
+    counts = np.array([n for _o, n in runs], dtype=np.int64)
+    total = int(counts.sum()) if runs else 0
+    if total == 0:
+        return torch.empty(0, dtype=torch.uint8, device=d_blob.device)
+    starts = np.array([o for o, _n in runs], dtype=np.int64)
+    first = np.cumsum(counts) - counts
+    offsets = np.repeat(starts - size * first, counts) + size * np.arange(total, dtype=np.int64)
+    windows = d_blob.as_strided((d_blob.numel() - size + 1, size), (1, 1))     # row j: the `size` bytes from j
+    return windows.index_select(0, torch.from_numpy(offsets).to(d_blob.device)).reshape(-1)
+
+
+def first_bad_point(status: torch.Tensor, runs: list, size: int):
+    """the first point whose status is not G1_VALID → (its index, "field[element]: reason", its byte offset), or None; `runs`
+    places the points: [(first index, count, field, byte offset of the run)], `size` bytes per point"""
+    bad = torch.nonzero(status).flatten()[:1].cpu().tolist()
+    if not bad:
+        return None
+    i = bad[0]
+    for first, n, fld, at in runs:
+        if first <= i < first + n:
+            return i, f"{fld}[{i - first}]: {_G1_STATUS[int(status[i])]}", at + size * (i - first)
+    raise AssertionError("a point outside every run")
+
+
+@dataclass
+class CommitterKeyLayout:
+    """where one committer key's sections sit in its blob: point runs as (byte offset, count), the bound keys and the hash"""
+    powers: tuple
+    lagrange: list                 # [(size, offset)]
+    gamma: tuple
+    shifted: tuple | None
+    shifted_gamma: list | None     # [(bound, offset, count)]
+    bounds: list | None
+    hash_offset: int
+
+    def runs(self) -> list:
+        """every point run in blob order"""
+        out = [self.powers] + [(o, n) for n, o in self.lagrange] + [self.gamma]
+        out += [self.shifted] if self.shifted is not None else []
+        return out + [(o, n) for _b, o, n in self.shifted_gamma or []]
+
+    def fields(self, first: int = 0) -> list:
+        """[(first point index, count, field, byte offset)] of the runs, points numbered from `first`"""
+        names = (["powers_of_beta_g"] + [f"lagrange_bases_at_beta_g[{n}]" for n, _o in self.lagrange] + ["powers_of_beta_times_gamma_g"]
+                 + (["shifted_powers_of_beta_g"] if self.shifted is not None else [])
+                 + [f"shifted_powers_of_beta_times_gamma_g[{b}]" for b, _o, _n in self.shifted_gamma or []])
+        out = []
+        for name, (o, n) in zip(names, self.runs()):
+            out.append((first, n, name, o))
+            first += n
+        return out
+
+    def sha256(self, mv: memoryview) -> bytes:
+        """the hash FromBytes recomputes (data_structures.rs:152-177): the bytes of every point section but the Lagrange bases, as
+        read (every accepted encoding writes back to itself)"""
+        h = hashlib.sha256()
+        for o, n in [self.powers, self.gamma] + ([self.shifted] if self.shifted is not None else []) + \
+                [(o, n) for _b, o, n in self.shifted_gamma or []]:
+            h.update(mv[o: o + POINT_BYTES * n])
+        return h.digest()
+
+    def build(self, images: torch.Tensor, first: int = 0) -> CommitterKey:
+        """the CommitterKey whose points are images[first:], decoded in runs() order (views, no copy)"""
+        views = []
+        for _o, n in self.runs():
+            views.append(images[first: first + n])
+            first += n
+        it = iter(views)
+        powers = next(it)
+        lagrange = {size: next(it) for size, _o in self.lagrange}
+        gamma = next(it)
+        shifted = next(it) if self.shifted is not None else None
+        shifted_gamma = None if self.shifted_gamma is None else {b: next(it) for b, _o, _n in self.shifted_gamma}
+        return CommitterKey(powers, gamma, lagrange, shifted, shifted_gamma, None if self.bounds is None else list(self.bounds), None)
+
+
+def walk_committer_key(r: ByteReader) -> CommitterKeyLayout:
+    """the headers of ToBytes for CommitterKey from r's offset: u32 counts, bool tags, u32 keys and bounds; every count is checked
+    against the bytes left before anything of its size exists, and the points are only located"""
+    def run(field: str) -> tuple:
+        n = r.u32(f"{field} length")
+        r.need(POINT_BYTES * n, f"{field} of {n} points")
+        r.o += POINT_BYTES * n
+        return r.o - POINT_BYTES * n, n
+
+    def increasing(keys: list, field: str) -> None:
+        for i in range(1, len(keys)):
+            if keys[i] <= keys[i - 1]:
+                raise r.fail(f"{field}[{i}]", f"key {keys[i]} does not follow {keys[i - 1]}")
+
+    powers = run("powers_of_beta_g")
+    nl = r.u32("lagrange_bases_at_beta_g length")
+    r.need(4 * nl, f"lagrange_bases_at_beta_g of {nl} bases")
+    lagrange = []
+    for i in range(nl):
+        size = r.u32(f"lagrange_bases_at_beta_g[{i}] size")
+        r.need(POINT_BYTES * size, f"lagrange_bases_at_beta_g[{i}] of {size} points")
+        lagrange.append((size, r.o))
+        r.o += POINT_BYTES * size
+    increasing([n for n, _o in lagrange], "lagrange_bases_at_beta_g")
+    gamma = run("powers_of_beta_times_gamma_g")
+    shifted = run("shifted_powers_of_beta_g") if r.tag("shifted_powers_of_beta_g tag") else None
+    shifted_gamma = None
+    if r.tag("shifted_powers_of_beta_times_gamma_g tag"):
+        nb = r.u32("shifted_powers_of_beta_times_gamma_g length")
+        r.need(8 * nb, f"shifted_powers_of_beta_times_gamma_g of {nb} entries")
+        shifted_gamma = []
+        for i in range(nb):
+            b = r.u32(f"shifted_powers_of_beta_times_gamma_g[{i}] key")
+            o, n = run(f"shifted_powers_of_beta_times_gamma_g[{i}]")
+            shifted_gamma.append((b, o, n))
+        increasing([b for b, _o, _n in shifted_gamma], "shifted_powers_of_beta_times_gamma_g")
+    bounds = None
+    if r.tag("enforced_degree_bounds tag"):
+        nb = r.u32("enforced_degree_bounds length")
+        r.need(4 * nb, f"enforced_degree_bounds of {nb} bounds")
+        bounds = list(struct.unpack(f"<{nb}I", r.take(4 * nb, "enforced_degree_bounds")))
+    hash_offset = r.o
+    r.take(32, "hash")
+    return CommitterKeyLayout(powers, lagrange, gamma, shifted, shifted_gamma, bounds, hash_offset)
+
+
+def _committer_key_parts(ck: CommitterKey) -> list:
+    """ToBytes of one key in write order: bytes, and point tensors ([n, 104] Affine images) with whether the hash covers them"""
+    parts = [struct.pack("<I", ck.powers_of_beta_g.shape[0]), (ck.powers_of_beta_g, True),
+             struct.pack("<I", len(ck.lagrange_bases_at_beta_g))]
+    for size in sorted(ck.lagrange_bases_at_beta_g):
+        parts += [struct.pack("<I", size), (ck.lagrange_bases_at_beta_g[size], False)]
+    parts += [struct.pack("<I", ck.powers_of_beta_times_gamma_g.shape[0]), (ck.powers_of_beta_times_gamma_g, True)]
+    if ck.shifted_powers_of_beta_g is None:
+        parts.append(b"\x00")
+    else:
+        parts += [b"\x01", struct.pack("<I", ck.shifted_powers_of_beta_g.shape[0]), (ck.shifted_powers_of_beta_g, True)]
+    if ck.shifted_powers_of_beta_times_gamma_g is None:
+        parts.append(b"\x00")
+    else:
+        parts += [b"\x01", struct.pack("<I", len(ck.shifted_powers_of_beta_times_gamma_g))]
+        for b in sorted(ck.shifted_powers_of_beta_times_gamma_g):
+            v = ck.shifted_powers_of_beta_times_gamma_g[b]
+            parts += [struct.pack("<II", b, v.shape[0]), (v, True)]
+    if ck.enforced_degree_bounds is None:
+        parts.append(b"\x00")
+    else:
+        parts += [b"\x01", struct.pack(f"<I{len(ck.enforced_degree_bounds)}I", len(ck.enforced_degree_bounds), *ck.enforced_degree_bounds)]
+    return parts
+
+
+def committer_keys_to_bytes(cks: list) -> list:
+    """ToBytes of every key, all points of all keys through one device.g1_serialize call (the 97-byte form) → [bytes]"""
+    layouts = [_committer_key_parts(ck) for ck in cks]
+    tensors = [t for parts in layouts for t, _h in (q for q in parts if not isinstance(q, bytes))]
+    enc = np.zeros(0, dtype=np.uint8)
+    if tensors and sum(t.shape[0] for t in tensors):
+        flat = torch.cat([t.reshape(-1, STRIDE) for t in tensors])
+        enc = device.g1_serialize(flat.contiguous(), device.G1_TO_BYTES).cpu().numpy().reshape(-1)
+    out, at = [], 0
+    for parts in layouts:
+        chunks, h = [], hashlib.sha256()
+        for q in parts:
+            if isinstance(q, bytes):
+                chunks.append(q)
+                continue
+            t, hashed = q
+            b = enc[at: at + POINT_BYTES * t.shape[0]].tobytes()
+            at += POINT_BYTES * t.shape[0]
+            chunks.append(b)
+            if hashed:
+                h.update(b)
+        out.append(b"".join(chunks) + h.digest())
+    return out

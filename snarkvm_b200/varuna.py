@@ -407,6 +407,22 @@ class CircuitProvingKey:
     circuit: Circuit
     committer_key: object
 
+    def to_bytes(self) -> bytes:
+        """ToBytes (circuit_proving_key.rs:42-49): proving_keys_to_bytes of this key"""
+        return proving_keys_to_bytes([self])[0]
+
+    @staticmethod
+    def read(blob, offset: int = 0, validate: bool = True, device_="cuda"):
+        """the CircuitProvingKey whose bytes start at `offset` of `blob` → (CircuitProvingKey, the offset after it); errors as
+        proving_keys_from_bytes.  A snarkVM `.prover` file is a version byte (1) and then this layout: read it at offset 1."""
+        pks, ends = _proving_keys_from_bytes([blob], [offset], validate, device_)
+        return pks[0], ends[0]
+
+    @staticmethod
+    def from_bytes(blob, validate: bool = True, device_="cuda") -> "CircuitProvingKey":
+        """the CircuitProvingKey at the start of `blob`; trailing bytes are ignored"""
+        return CircuitProvingKey.read(blob, 0, validate, device_)[0]
+
 
 def batch_circuit_setup(circuits: list, pp_powers_of_beta_g: torch.Tensor, pp_powers_of_beta_times_gamma_g: torch.Tensor, zk: bool = False,
                         with_id: bool = False) -> list:
@@ -1483,8 +1499,17 @@ def _union_committer_key(cks: list):
     from .sonic_pc import CommitterKey
     if len(cks) == 1:
         return cks[0]
-    if len({ck.max_degree for ck in cks}) != 1:
-        raise ValueError("the committer keys come from different universal parameters")
+    if all(ck.max_degree is not None for ck in cks):
+        if len({ck.max_degree for ck in cks}) != 1:
+            raise ValueError("the committer keys come from different universal parameters")
+    else:
+        # a key read from bytes does not carry its SRS's degree, but every key trimmed from one SRS ends its shifted powers on
+        # the SRS's last power
+        lasts = [ck.shifted_powers_of_beta_g[-1] for ck in cks if ck.shifted_powers_of_beta_g is not None and
+                 ck.shifted_powers_of_beta_g.shape[0]]
+        if len(lasts) != len(cks) or not all(torch.equal(lasts[0], t) for t in lasts[1:]):
+            raise ValueError("the committer keys come from different universal parameters")
+    max_degree = next((ck.max_degree for ck in cks if ck.max_degree is not None), None)
     longest = max(cks, key=lambda ck: ck.powers_of_beta_g.shape[0])
     bounds = sorted({b for ck in cks for b in (ck.enforced_degree_bounds or [])})
     shifted, gamma = None, {}
@@ -1494,7 +1519,7 @@ def _union_committer_key(cks: list):
             if ck.enforced_degree_bounds[-1] == bounds[-1]:
                 shifted = ck.shifted_powers_of_beta_g
     return CommitterKey(longest.powers_of_beta_g, longest.powers_of_beta_times_gamma_g, {}, shifted, gamma or None, bounds or None,
-                        longest.max_degree)
+                        max_degree)
 
 
 def _nonzero_vanishing(domain: EvaluationDomain, x: int, name: str):
@@ -2120,13 +2145,7 @@ def _from_bytes_many(walk, blobs, offsets, compress: bool, validate: bool, devic
             i = int(bad[0])
             k = int(np.searchsorted(starts, i, side="right")) - 1
             raise ValueError(f"blob {k}: {points[i][1]}: {_G1_BYTES_STATUS[int(status[i])]}")
-        limbs = np.zeros((len(points), 18), dtype=np.uint64)
-        limbs[:, :12] = images[:, :96].copy().view(np.uint64)
-        inf = images[:, 96] != 0
-        limbs[~inf, 12:] = _FQ_ONE
-        limbs[inf, :12] = 0
-        limbs[inf, 6:12] = _FQ_ONE                                        # (0, one, 0)
-        pts = list(limbs)
+        pts = list(_projective_limbs(images))
     if fail is not None:
         raise ValueError(f"blob {fail[0]}: {fail[1]}")
     return [b(pts) for b in builds], ends
@@ -2215,3 +2234,285 @@ def verifying_keys_from_bytes(blobs: list, compress: bool = True, validate: bool
 def certificates_from_bytes(blobs: list, compress: bool = True, validate: bool = True, device_="cuda") -> list:
     """Certificate::deserialize_with_mode of every blob, as proofs_from_bytes → [Certificate]"""
     return _from_bytes_many(_walk_certificate, blobs, [0] * len(blobs), compress, validate, device_)[0]
+
+
+# ---- byte form of CircuitProvingKey: ToBytes / FromBytes (circuit_proving_key.rs:42-57) = the verifying key (CanonicalSerialize,
+# compressed), the Circuit (CanonicalSerialize, compressed: ahp/indexer/circuit.rs:158-237) and the CommitterKey (ToBytes,
+# sonic_pc/data_structures.rs:65-265) ----
+
+_FR_TWO_ADIC_ROOT = 8065159656716812877374967518403273466521432693661810619979959746626482506078   # fr.rs:110: FrParameters
+_FR_GENERATOR = 22                                                                                   # fr.rs:126: GENERATOR
+_DOMAIN_FIELDS = (("size", 0, 8), ("log_size_of_group", 8, 4), ("size_as_field_element", 12, 32), ("size_inv", 44, 32),
+                  ("group_gen", 76, 32), ("group_gen_inv", 108, 32), ("generator_inv", 140, 32))
+_DOMAIN_BYTES = 172
+_VK_BYTES = 48 + 8 + 12 * device.G1_COMPRESSED_BYTES + 32
+
+
+def _domain_bytes(size: int) -> bytes:
+    """CanonicalSerialize of EvaluationDomain::new(size) for a power of two (fft/domain.rs:82-147): u64 size, u32 log size, then
+    size, 1/size, the subgroup's generator ω (TWO_ADIC_ROOT_OF_UNITY squared down to order `size`), 1/ω and 1/GENERATOR as Fr"""
+    cached = _DOMAIN_CACHE.get(size)
+    if cached is None:
+        lg = size.bit_length() - 1
+        w = pow(_FR_TWO_ADIC_ROOT, 1 << (47 - lg), R_MOD)
+        vals = (size % R_MOD, pow(size, -1, R_MOD), w, pow(w, -1, R_MOD), pow(_FR_GENERATOR, -1, R_MOD))
+        cached = _DOMAIN_CACHE[size] = struct.pack("<QI", size, lg) + b"".join(v.to_bytes(32, "little") for v in vals)
+    return cached
+
+
+_DOMAIN_CACHE: dict = {}
+
+
+@dataclass
+class _KeyLayout:
+    """where one proving key's sections sit in its blob (byte offsets), from the host walk"""
+    info: CircuitInfo
+    vk_points: int                 # the twelve compressed commitments
+    vk_id: bytes
+    id_span: tuple                 # (start, end): CircuitInfo and the three matrices, the bytes of the circuit id
+    matrices: list                 # per matrix (offset of its u64 row count, host row_ptr int32)
+    evals: list                    # per matrix {"row", "col", "row_col_val": offset of the first value}
+    domains: list                  # per matrix K
+    ck: object                     # sonic_pc.CommitterKeyLayout
+
+
+def _walk_proving_key(r) -> _KeyLayout:
+    """the headers of one proving key from r's offset, checking each count against the bytes left before anything of its size
+    exists; the bulk sections are only located (a matrix's rows by the library's row walk)"""
+    from .sonic_pc import walk_committer_key
+    fields = CircuitInfo.__dataclass_fields__
+    info = CircuitInfo(*[r.u64(f"circuit_verifying_key.circuit_info.{f}") for f in fields])
+    n = r.u64("circuit_verifying_key.circuit_commitments length")
+    if n != len(INDEX_POLYNOMIAL_NAMES):
+        raise r.fail("circuit_verifying_key.circuit_commitments", f"{n} commitments, not {len(INDEX_POLYNOMIAL_NAMES)}")
+    vk_points = r.o
+    r.take(len(INDEX_POLYNOMIAL_NAMES) * device.G1_COMPRESSED_BYTES, "circuit_verifying_key.circuit_commitments")
+    vk_id = bytes(r.take(32, "circuit_verifying_key.id"))
+    start = r.o
+    cinfo = CircuitInfo(*[r.u64(f"circuit.index_info.{f}") for f in fields])
+    if cinfo != info:
+        raise r.fail("circuit_verifying_key.circuit_info", "differs from the circuit's index_info")
+    # the domains Circuit's read builds (circuit.rs:196-214) and those Circuit._shape needs
+    counts = (info.num_constraints, info.num_public_and_private_variables, info.num_public_inputs, info.num_non_zero_a,
+              info.num_non_zero_b, info.num_non_zero_c)
+    doms = [EvaluationDomain.new(c) for c in counts]
+    for f, d in zip(("num_constraints", "num_public_and_private_variables", "num_public_inputs", "num_non_zero_a",
+                     "num_non_zero_b", "num_non_zero_c"), doms):
+        if d is None:
+            raise r.fail(f"circuit.index_info.{f}", "no evaluation domain holds this many elements")
+    if info.num_public_inputs & (info.num_public_inputs - 1) or doms[1].size <= doms[2].size:
+        raise r.fail("circuit.index_info", "public inputs not padded to a power of two below the variable domain")
+    matrices = []
+    for m, nnz in zip("abc", counts[3:]):
+        at = r.o
+        nrows = r.u64(f"circuit.{m} length")
+        if nrows != info.num_constraints:
+            raise r.fail(f"circuit.{m}", f"{nrows} rows, not num_constraints = {info.num_constraints}")
+        r.need(8 * nrows + 40 * nnz, f"circuit.{m} of {nrows} rows and {nnz} entries")
+        row_ptr, bad = device.matrix_row_walk(r.mv, r.o, nrows, nnz)
+        if row_ptr is None:
+            what = f"circuit.{m}[{bad}]" if 0 <= bad < nrows else f"circuit.{m}"
+            raise r.fail(what, f"the row lengths overrun the matrix or disagree with num_non_zero_{m} = {nnz}")
+        r.o += 8 * nrows + 40 * nnz
+        matrices.append((at, row_ptr))
+    id_span = (start, r.o)
+    evals, ks = [], [d.size for d in doms[3:]]
+    for m, K in zip("abc", ks):
+        e = {}
+        for name in ("row", "col", "row_col", "row_col_val"):
+            fld = f"circuit.{m}_arith.{name}"
+            if name == "row_col":
+                if r.tag(f"{fld} tag"):
+                    raise r.fail(fld, "present; a proving key holds it pruned (prune_row_col_evals)")
+                continue
+            n = r.u64(f"{fld} length")
+            if n != K:
+                raise r.fail(fld, f"{n} evaluations, not |K| = {K}")
+            r.need(32 * K + _DOMAIN_BYTES, f"{fld} of {K} evaluations and its domain")
+            e[name] = r.o
+            r.o += 32 * K
+            got, want = r.take(_DOMAIN_BYTES, f"{fld}.domain"), _domain_bytes(K)
+            if got != want:
+                f, _o, _n = next(x for x in _DOMAIN_FIELDS if got[x[1]: x[1] + x[2]] != want[x[1]: x[1] + x[2]])
+                raise r.fail(f"{fld}.domain.{f}", f"differs from EvaluationDomain::new({K})")
+        evals.append(e)
+    return _KeyLayout(info, vk_points, vk_id, id_span, matrices, evals, ks, walk_committer_key(r))
+
+
+def _blake2s(mv: memoryview, span: tuple) -> bytes:
+    return hashlib.blake2s(mv[span[0]: span[1]], digest_size=32).digest()
+
+
+def _proving_keys_from_bytes(blobs: list, offsets: list, validate: bool, device_):
+    """proving_keys_from_bytes at per-blob offsets → (keys, end offsets)"""
+    from .sonic_pc import POINT_BYTES, ByteReader, first_bad_point, gather_records, upload
+    if not blobs:
+        return [], []
+    mvs = [memoryview(b).cast("B") for b in blobs]
+    layouts, ends = [], []
+    for k, (mv, off) in enumerate(zip(mvs, offsets)):
+        r = ByteReader(mv, off, f"blob {k}")
+        layouts.append(_walk_proving_key(r))
+        ends.append(r.o)
+    dev = torch.device(device_)
+    pool = ThreadPoolExecutor(min(ID_HASH_THREADS, 2 * len(blobs)))
+    try:
+        # host: SHA-256 and Blake2s of the bytes as read, while the device decodes
+        shas = [pool.submit(L.ck.sha256, mv) for L, mv in zip(layouts, mvs)]
+        ids = [pool.submit(_blake2s, mv, L.id_span) for L, mv in zip(layouts, mvs)]
+        # device: each blob's key once into one buffer; every row_ptr in one upload
+        base = np.cumsum([0] + [e - o for o, e in zip(offsets, ends)]).tolist()
+        d_blob = torch.empty(base[-1], dtype=torch.uint8, device=dev)
+        for k, (mv, off) in enumerate(zip(mvs, offsets)):
+            upload(mv[off: ends[k]], d_blob[base[k]: base[k + 1]])
+        row_ptrs = torch.from_numpy(np.concatenate([rp for L in layouts for _o, rp in L.matrices])).to(dev)
+        nnzs = [n for L in layouts for n in (L.info.num_non_zero_a, L.info.num_non_zero_b, L.info.num_non_zero_c)]
+        vals = torch.empty((sum(nnzs), 4), dtype=torch.int64, device=dev)
+        cols = torch.empty(sum(nnzs), dtype=torch.int32, device=dev)
+        evals = torch.empty((3 * sum(sum(L.domains) for L in layouts), 4), dtype=torch.int64, device=dev)
+        # every point of the call: the verifying keys' compressed commitments, then the committer keys' ToBytes points
+        shift = [b - o for b, o in zip(base, offsets)]
+        vk_raw = gather_records(d_blob, [(L.vk_points + shift[k], 12) for k, L in enumerate(layouts)], device.G1_COMPRESSED_BYTES)
+        vk_images, vk_status = device.g1_deserialize(vk_raw, device.G1_COMPRESSED, validate)
+        ck_runs, ck_first = [], []
+        for k, L in enumerate(layouts):
+            ck_first.append(sum(n for _o, n in ck_runs))
+            ck_runs += [(o + shift[k], n) for o, n in L.ck.runs()]
+        ck_images, ck_status = device.g1_deserialize(gather_records(d_blob, ck_runs, POINT_BYTES), device.G1_TO_BYTES, validate)
+        # every Fr record of the call in one launch; its synchronisation also ends the point decodes
+        segments, owners, mats, arith = [], [], [], []
+        at_rp = at_nnz = at_ev = 0
+        for k, L in enumerate(layouts):
+            for j, (m, (o, rp)) in enumerate(zip("abc", L.matrices)):
+                nnz = nnzs[3 * k + j]
+                views = (row_ptrs[at_rp: at_rp + rp.size], cols[at_nnz: at_nnz + nnz], vals[at_nnz: at_nnz + nnz])
+                segments.append((o + shift[k], nnz, 40, views[2], views[1], L.info.num_public_and_private_variables, views[0]))
+                owners.append((k, o, f"circuit.{m}", rp))
+                mats.append(views)
+                at_rp += rp.size
+                at_nnz += nnz
+            for m, e, K in zip("abc", L.evals, L.domains):
+                trio = []
+                for name in ("row", "col", "row_col_val"):
+                    out = evals[at_ev: at_ev + K]
+                    at_ev += K
+                    segments.append((e[name] + shift[k], K, 32, out, None, 0, None))
+                    owners.append((k, e[name], f"circuit.{m}_arith.{name}", None))
+                    trio.append(out)
+                arith.append(trio)
+        bad = device.fr_records_decode(d_blob, segments)
+        # the first fault of the lowest blob at fault, in byte order; a hash is checked after every element
+        faults = []
+        for (k, o, fld, rp), b in zip(owners, bad):
+            if b is not None:
+                e, why = b
+                if rp is not None:                                     # a matrix entry: name its row
+                    row = int(np.searchsorted(rp, e, side="right")) - 1
+                    fld, at = f"{fld}[{row}][{e - rp[row]}]", o + 16 + 8 * row + 40 * e
+                else:
+                    fld, at = f"{fld}[{e}]", o + 32 * e
+                what = "not below r" if why == device.FR_RECORD_NOT_CANONICAL else \
+                    "column not below num_public_and_private_variables"
+                faults.append((k, 0, at, f"{fld}: {what}"))
+        bad_vk = first_bad_point(vk_status, [(12 * k, 12, "circuit_verifying_key.circuit_commitments", L.vk_points)
+                                             for k, L in enumerate(layouts)], device.G1_COMPRESSED_BYTES)
+        if bad_vk is not None:
+            faults.append((bad_vk[0] // 12, 0, bad_vk[2], bad_vk[1]))
+        bad_ck = first_bad_point(ck_status, [(f, n, f"committer_key.{fld}", o) for k, L in enumerate(layouts)
+                                             for f, n, fld, o in L.ck.fields(ck_first[k])], POINT_BYTES)
+        if bad_ck is not None:
+            faults.append((int(np.searchsorted(ck_first, bad_ck[0], side="right")) - 1, 0, bad_ck[2], bad_ck[1]))
+        for k, L in enumerate(layouts):
+            if shas[k].result() != bytes(mvs[k][L.ck.hash_offset: L.ck.hash_offset + 32]):
+                faults.append((k, 1, L.ck.hash_offset, "committer_key.hash: the SHA-256 of the points differs"))
+            if ids[k].result() != L.vk_id:
+                faults.append((k, 1, L.vk_points, "circuit_verifying_key.id: differs from the circuit's id"))
+        if faults:
+            k, _rank, _at, what = min(faults)
+            raise ValueError(f"blob {k}: {what}")
+    finally:
+        pool.shutdown(wait=True)
+    vk_limbs = _projective_limbs(vk_images.cpu().numpy())
+    out = []
+    for k, L in enumerate(layouts):
+        c = Circuit.__new__(Circuit)
+        c._shape(*[Matrix.from_device(*mats[3 * k + j]) for j in range(3)], L.info.num_public_inputs,
+                 L.info.num_public_and_private_variables)
+        c.ariths = [MatrixEvals(*arith[3 * k + j], K) for j, K in enumerate(c.non_zero_domains)]
+        c._id = L.vk_id
+        vk = CircuitVerifyingKey(L.info, vk_limbs[12 * k: 12 * k + 12].copy(), L.vk_id)
+        out.append(CircuitProvingKey(vk, c, L.ck.build(ck_images, ck_first[k])))
+    return out, ends
+
+
+def proving_keys_from_bytes(blobs: list, validate: bool = True, device_="cuda") -> list:
+    """CircuitProvingKey::read_le (circuit_proving_key.rs:51-57) of every blob (trailing bytes are ignored) → [CircuitProvingKey].
+
+    The host walks the headers only — counts, tags, CircuitInfo, domains, the matrices' row lengths (a bounds-checked walk in the
+    library) — and checks every count against the bytes left before anything of that size exists; a header fault of any blob is
+    reported before any device call.  Each key's bytes then go to the device once, and a fixed number of launches decodes every
+    key of the call: one for the Fr records (matrix values and columns, evaluations), one per point form (the verifying keys'
+    compressed commitments, the committer keys' 97-byte points; with `validate` each point also passes Affine::check).  One
+    synchronisation precedes the reports.  The SHA-256 of each committer key's points and the Blake2s circuit id are computed from
+    the bytes as read, on host threads, while the device decodes.  The loaded Circuit holds the decoded CSR arrays and
+    evaluations; its id is the one computed here, and no matrix_evals pass runs.  Its committer key's max_degree is None.
+
+    ValueError names the blob, the field and the element: everything the reference refuses (bytes missing, a tag or bool other
+    than 0 or 1, an Fr not below r, a coordinate not below q, an infinity byte the reference refuses, a SHA-256 mismatch), and,
+    stricter than the reference, because this prover would otherwise diverge from it silently:
+      a column not below num_public_and_private_variables (an out-of-range read in the prover's mat-vecs and transposes);
+      a matrix whose row count or entry count differs from CircuitInfo;
+      an evaluation vector whose length is not |K|, or whose EvaluationDomain differs from EvaluationDomain::new(|K|);
+      a row_col evaluation vector present (setup always prunes it);
+      a CircuitInfo without the domains the prover needs (public inputs padded to a power of two below the variable domain);
+      a verifying key whose circuit_info or id differs from the circuit's;
+      committer-key map keys not strictly increasing;
+      with `validate`, a point off the curve or outside the subgroup.
+    Body faults name the lowest blob at fault and its first fault in byte order, hashes after elements."""
+    return _proving_keys_from_bytes(blobs, [0] * len(blobs), validate, device_)[0]
+
+
+def _projective_limbs(images: np.ndarray) -> np.ndarray:
+    """Affine<G1> images [n, 104] → normalised projective limbs uint64[n, 18]"""
+    limbs = np.zeros((images.shape[0], 18), dtype=np.uint64)
+    limbs[:, :12] = images[:, :96].copy().view(np.uint64)
+    inf = images[:, 96] != 0
+    limbs[~inf, 12:] = _FQ_ONE
+    limbs[inf, :12] = 0
+    limbs[inf, 6:12] = _FQ_ONE                                        # (0, one, 0)
+    return limbs
+
+
+def proving_keys_to_bytes(pks: list) -> list:
+    """CircuitProvingKey::write_le (circuit_proving_key.rs:42-49) of every key → [bytes]: the verifying key compressed (its id
+    the circuit's), the circuit (CircuitInfo; A, B, C through csr_serialize; per matrix row, col, row_col = None and row_col_val
+    through fr_from_mont, each with its domain), the committer key's ToBytes.  Every matrix of the call shares one launch, the
+    evaluations one, and the points of each form one."""
+    from .sonic_pc import committer_keys_to_bytes
+    if not pks:
+        return []
+    circuits = [pk.circuit for pk in pks]
+    buf, offs = device.csr_serialize_batch([(m.row_ptr, m.cols, m.vals) for c in circuits for m in (c.a, c.b, c.c)])
+    mats = buf.cpu().numpy()
+    for k, c in enumerate(circuits):
+        if c._id is None:
+            c._id = hashlib.blake2s(c.info.to_bytes_le() + mats[offs[3 * k]: offs[3 * k + 3]].tobytes(), digest_size=32).digest()
+    ev = device.fr_from_mont(torch.cat([t for c in circuits for a in c.ariths for t in (a.row, a.col, a.row_col_val)]))
+    ev = ev.cpu().numpy().view(np.uint8).reshape(-1)
+    vks = [CircuitVerifyingKey(pk.circuit_verifying_key.circuit_info, pk.circuit_verifying_key.circuit_commitments, pk.circuit.id())
+           for pk in pks]
+    vk_bytes = _to_bytes_many(_verifying_key_parts, vks, True, circuits[0].a.row_ptr.device)
+    ck_bytes = committer_keys_to_bytes([pk.committer_key for pk in pks])
+    out, at = [], 0
+    for k, c in enumerate(circuits):
+        parts = [vk_bytes[k], c.info.to_bytes_le(), mats[offs[3 * k]: offs[3 * k + 3]].tobytes()]
+        for a in c.ariths:
+            K = a.domain.size
+            head = struct.pack("<Q", K)
+            for j in range(3):
+                if j == 2:
+                    parts.append(b"\x00")                                     # row_col: pruned
+                parts += [head, ev[at: at + 32 * K].tobytes(), _domain_bytes(K)]
+                at += 32 * K
+        out.append(b"".join(parts) + ck_bytes[k])
+    return out
