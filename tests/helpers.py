@@ -38,6 +38,22 @@ def random_fr_mont(n: int, seed: int) -> np.ndarray:
     return random_canonical_fr(n, seed)
 
 
+NEAR_R = np.array([py.to_limbs(py.R_MOD - 1, 4), py.to_limbs(py.R_MOD - 2, 4)], dtype=np.uint64)
+
+
+def put_near_r(x):
+    """The first and last min(4, n) rows of x ← r − 1, r − 2, r − 2, r − 1: the largest canonical limbs, which uniform draws
+    never reach, at even and odd indices.  x: uint64 [n, 4] array or int64 [n, 4] tensor, modified in place → x."""
+    k = min(4, x.shape[0])
+    v = NEAR_R[[0, 1, 1, 0][:k]]
+    if not isinstance(x, np.ndarray):
+        import torch
+        v = torch.from_numpy(v.view(np.int64)).to(x.device)
+    x[:k] = v
+    x[x.shape[0] - k:] = v
+    return x
+
+
 def fr_ints_to_mont_array(vals) -> np.ndarray:
     return np.array([py.to_limbs(py.fr_to_mont(v), 4) for v in vals], dtype=np.uint64).reshape(-1, 4)
 

@@ -4,7 +4,7 @@ Restates test_fft_correctness_cuda (algorithms/src/fft/domain.rs:1140-1218: size
 import numpy as np
 import pytest
 
-from helpers import random_fr_mont
+from helpers import put_near_r, random_fr_mont
 
 pytestmark = pytest.mark.gpu
 
@@ -33,15 +33,16 @@ def test_ntt_host_ffi_vs_oracle(oracle_cpu, lg):
         assert (got == want).all(), (lg, d, t)
 
 
-@pytest.mark.parametrize("lg", [20, 21, 22])
+@pytest.mark.parametrize("lg", [20, 21, 22, 25])
 def test_ntt_host_ffi_pipelined_vs_oracle(oracle_cpu, lg, monkeypatch):
     """snarkvm_ntt from 2^20 elements: the host buffer is uploaded / downloaded by column ranges under the first and last pass
     (ntt_host_pipelined) — pageable numpy memory (staged through the pinned ring row by row) and pinned memory (2-D DMA straight
-    from the caller's buffer), all four transforms; the plain path (switch off) must agree"""
+    from the caller's buffer), all four transforms; the plain path (switch off) must agree.  2^25 is a four-pass plan: two
+    middle passes between the column ranges, and 32 ranges for the 1 GiB pageable buffer."""
     import torch
     from snarkvm_b200 import cuda
     n = 1 << lg
-    x = random_fr_mont(n, seed=300 + lg)
+    x = put_near_r(random_fr_mont(n, seed=300 + lg))
     pinned = torch.empty((n, 4), dtype=torch.int64).pin_memory()
     for d, t in MODES:
         want = oracle_cpu.ntt(x, d, t)
@@ -186,15 +187,15 @@ def test_ntt_input_output_orders(oracle_cpu, lg):
         assert (got == want[perm]).all()
 
 
-@pytest.mark.parametrize("lg", [22, 23, 24])
+@pytest.mark.parametrize("lg", [22, 23, 24, 25])
 def test_ntt_large_sizes_vs_oracle(oracle_cpu, lg):
-    """BASELINE config 3 (and the sizes between, whose pass splits differ: 8+7+7, 8+8+7, 8+8+8): all four
-    (direction, type) modes against the oracle's fft_in_place, element by element."""
+    """BASELINE config 3 (and the sizes between, whose pass splits differ: 8+7+7, 8+8+7, 8+8+8) and the smallest four-pass
+    plan, 7+6+6+6: all four (direction, type) modes against the oracle's fft_in_place, element by element."""
     import torch
     from snarkvm_b200 import device
     from snarkvm_b200.cuda import NTTDirection, NTTType
     n = 1 << lg
-    x = random_fr_mont(n, seed=2200 + lg)
+    x = put_near_r(random_fr_mont(n, seed=2200 + lg))
     dx = _dev(x)
     scratch = torch.empty_like(dx)
     for d, t in MODES:
