@@ -58,12 +58,6 @@ int prof_collect(int kind, double* total_ms, uint64_t* count) {
     return rc;
 }
 
-#define CUDA_TRY(x)                                   \
-    do {                                              \
-        cudaError_t e_ = (x);                         \
-        if (e_ != cudaSuccess) { rc = (int)e_; goto done; } \
-    } while (0)
-
 static int ceil_log2(size_t x) { int l = 0; size_t v = x > 1 ? x - 1 : 0; while (v) { l++; v >>= 1; } return l; }
 // log2 rounded to the NEAREST integer (in the log domain): the plans below were swept at powers of two, and a size just above one
 // — a 2^20-coefficient polynomial plus four blinding terms — belongs to that power's plan, not to the next one's.
@@ -127,7 +121,6 @@ MsmPlan msm_make_plan(size_t npoints, bool mixed) {
     size_t total = npoints * (size_t)p.nwin;
     size_t cap = total / 300000 + 1;
     if (cap < 16) cap = 16;
-    if (const char* e = getenv("SNARKVM_B200_MSM_CAP")) { long v = atol(e); if (v >= 1) cap = (size_t)v; }
     p.cap = (uint32_t)cap;
     // Batched-affine pair levels before the XYZZ accumulation pay off only when every level still fills the
     // GPU (tools/ab_pair.py sweep with the record-scatter sort): 5 levels from 2^23, 4 at 2^21–2^22, 3 at 2^20, 2 at 2^19
@@ -155,7 +148,6 @@ MsmPlan msm_make_plan_batch(size_t max_n, size_t total_n) {
         if (levels > p.levels) p.levels = levels;
         size_t cap = total_n * (size_t)p.nwin / 300000 + 1;
         if (cap < 16) cap = 16;
-        if (const char* e = getenv("SNARKVM_B200_MSM_CAP")) { long v = atol(e); if (v >= 1) cap = (size_t)v; }
         p.cap = (uint32_t)cap;
     }
     return p;
@@ -1346,15 +1338,338 @@ int msm_set_scratch_limit(size_t bytes) {
     return 0;
 }
 
-struct Arena {
-    uint8_t* base = nullptr;
-    size_t off = 0;
-    template <class T> T* take(size_t count) {
-        T* p = base ? (T*)(base + off) : nullptr;
-        off += (count * sizeof(T) + 255) & ~(size_t)255;
-        return p;
-    }
+// How msm_core runs a call after its bucket sort.  msm_path() is the one place that decides it; every later phase switches on one
+// of these fields.
+struct MsmPath {
+    enum Acc { ACC_DENSE, ACC_THREAD, ACC_G8, ACC_Q8 } acc;         // XYZZ sums of the records the pair levels leave, or of
+                                                                    // gathered points: one thread, 8 lanes or a warp per item
+    uint32_t item_cap;                                              // points per work item of the XYZZ accumulation
+    enum Fold { FOLD_SCAN, FOLD_HOT32, FOLD_HOT1 } fold;            // scan 32:1, or the hot list keeping 32 or 1 partials
+    enum Tail { TAIL_QUAD_SMALL, TAIL_QUAD_LARGE, TAIL_CLASSIC } tail;
+    uint32_t hot_keep() const { return fold == FOLD_HOT1 ? 1u : 32u; }
 };
+
+static MsmPath msm_path(const MsmPlan& plan, uint32_t total_buckets, size_t max_entries, size_t set_cap) {
+    MsmPath p;
+    const bool gather = plan.levels == 0;
+    // Small problems take the quad-lane latency path (k_bucket_reduce_quad, k_window_combine_quad).  Large bucket sets: quad-lane
+    // combine levels after the per-chunk reduction (measured with tools/phase_sizes.py: faster at 2^20, 2^22 and 2^24; at 2^19 —
+    // 4096 buckets per window, 256 chunks — the shorter classic chain wins).
+    p.tail = plan.nbuckets <= 1024u ? MsmPath::TAIL_QUAD_SMALL : plan.nbuckets >= 16384u ? MsmPath::TAIL_QUAD_LARGE : MsmPath::TAIL_CLASSIC;
+    // The small-set quad reduction adds up to 32 partials per bucket itself; without pair levels the buckets with more are folded
+    // 32:1 per round, scan-free, from a device-side list of them.  The large-set tail folds its hot buckets the same way down to
+    // ONE partial per bucket (a lone thread adds what is left of a bucket in k_bucket_reduce, so nothing may be left), instead of
+    // two scan + copy passes over every bucket.  Everything else takes the scan folds: the classic tail, and pair levels with
+    // ≤ 1024 buckets per set, whose folds are followed by the small-set quad tail.
+    p.fold = p.tail == MsmPath::TAIL_QUAD_SMALL && gather ? MsmPath::FOLD_HOT32
+           : p.tail == MsmPath::TAIL_QUAD_LARGE         ? MsmPath::FOLD_HOT1
+                                                        : MsmPath::FOLD_SCAN;
+    p.item_cap = plan.cap;
+    if (!gather) {
+        p.acc = MsmPath::ACC_DENSE;
+    } else if (p.tail == MsmPath::TAIL_QUAD_SMALL && (size_t)total_buckets + max_entries / 32 <= 1100) {
+        // round 2 (quad.cuh): four lanes per point operation.  One warp per work item (k_bucket_accumulate_q8) while the whole
+        // problem is a few thousand buckets — every lane of the warp executes every multiplication, so it costs 3× the
+        // multiplier time of the one-thread kernel and only pays while the GPU is mostly idle; the item holds up to 1/16 of a
+        // bucket set, so a bucket has ≤ 17 item partials, k_bucket_reduce_quad adds them itself and the 32:1 folds are skipped.
+        // (measured with tools/phase_sizes.py: the warp-per-item kernel wins at 2^8 points and loses from 2^10, where the 1400
+        // items no longer fit one wave of 255-register warps)
+        p.acc = MsmPath::ACC_Q8;
+        const size_t cap16 = ((set_cap + 15) / 16 + 7) & ~(size_t)7;
+        p.item_cap = (uint32_t)(cap16 < 32 ? 32 : cap16);
+    } else if (max_entries <= 100000) {
+        // (measured: eight lanes per item win only while the whole problem is a few CTAs — up to 2^10 points, equal at 2^12, and
+        // from 2^14 they lose to the butterfly's extra additions)
+        p.acc = MsmPath::ACC_G8;
+        p.item_cap = 8 * 4;                                       // eight lanes per item, four points each
+    } else {
+        p.acc = MsmPath::ACC_THREAD;
+        // latency-bound sizes (2^12 … 2^15 points): 4 … 8 dependent mixed additions per thread instead of 16; the extra item
+        // partials of a bucket cost the quad reduction 4 multiplication steps each (swept with tools/phase_sizes.py: 4 wins at
+        // 2^12, 8 at 2^13 … 2^15)
+        if (p.fold == MsmPath::FOLD_HOT32 && max_entries <= 900000) p.item_cap = max_entries <= 150000 ? 4 : 8;
+    }
+    return p;
+}
+
+// One msm_core call: what its phases read, and its scratch as msm_core lays it out
+struct MsmCall {
+    MsmPlan plan;
+    MsmPath path;
+    bool flat;
+    const uint32_t* table;
+    size_t flat_n;                        // table mode: the table's points per window, else 0
+    uint32_t sets_per_job, wins_per_job, rec_words;
+    uint32_t chunk, chunks_per_set;       // buckets per thread of the per-chunk reduction, and such chunks per bucket set
+    size_t set_cap, hot_max;
+    int sm_count;
+    cudaStream_t stream;
+    uint8_t* cub_tmp;
+    size_t cub_bytes;
+    uint32_t *hist, *bucket_start, *cursors, *items, *item_start, *items2, *sorted, *cnt_tmp, *partial, *partial2, *hot_dev, *red_a, *red_b;
+    uint32_t *dense_bases, *dense0, *off_a, *off_b, *dense_a, *dense_b, *prefix, *pair_cnt, *pair_off, *sm_slots;
+    uint2* desc;
+};
+struct MsmGroup {                         // windows [u0, u0 + un) of the call, i.e. its bucket sets [w0, w0 + wn)
+    uint32_t u0, un, w0, wn, tb;
+    const uint32_t* bs;                   // tb + 1 absolute offsets into `sorted` (gather) or the level-0 records
+    size_t entries;                       // bound on the group's entries
+    size_t items_bound, items_launched;   // from the accumulation: ≥ the item count of any single bucket, of the whole group
+    const uint32_t *partial, *start;      // from the folds: the item partials and their per-bucket offsets the tail reads
+    int quad_rounds;
+};
+
+// the pair levels' dynamic shared memory limit (set once per device), and the current device's SM count
+static int msm_device_setup(int* sm_count) {
+    static std::once_flag smem_once[64];
+    int dev = 0; cudaGetDevice(&dev);
+    std::call_once(smem_once[dev & 63], [] {
+        cudaFuncSetAttribute(k_pair_level2<false, PAIR_MIN_BLOCKS>, cudaFuncAttributeMaxDynamicSharedMemorySize, PAIR2_SMEM);
+    });
+    return (int)cudaDeviceGetAttribute(sm_count, cudaDevAttrMultiProcessorCount, dev);
+}
+// msm_core's scans: one launch each, over a `uint32_t*` input (CUB instantiates its scan kernels per input type, and these are
+// the ones msm_core runs; msm_exclusive_scan's take `const uint32_t*` and count two)
+static int scan_counted_once(void* tmp, size_t tmp_bytes, const uint32_t* in, uint32_t* out, size_t count, cudaStream_t stream) {
+    count_launch();
+    return (int)cub::DeviceScan::ExclusiveSum(tmp, tmp_bytes, const_cast<uint32_t*>(in), out, (int)count, stream);
+}
+static void launch_digits(bool scatter, const MsmPlan& plan, const MsmSegment& sg, size_t flat_n, uint32_t slot_base, uint32_t* counters,
+                          uint32_t* sorted, uint32_t* d_flags, cudaStream_t stream) {
+    const auto k = !scatter ? (sg.mont ? k_digits<false, true> : k_digits<false, false>) : (sg.mont ? k_digits<true, true> : k_digits<true, false>);
+    k<<<(unsigned)((sg.n + 255) / 256), 256, 0, stream>>>((const uint32_t*)sg.d_scalars, sg.n, plan.c, plan.c_top, plan.nwin, plan.nbuckets,
+                                                          counters, sorted, flat_n, slot_base, sg.base0, d_flags);
+    count_launch();
+}
+// Bucket sort of all jobs and windows: histogram of every segment's digits into `hist` (TB + 1 counters, keyed by (job, bucket
+// set, bucket)), its exclusive scan into `bucket_start` and `cursors`, and, given `sorted`, the scatter of the entries into it.
+// Without `sorted` only the histogram runs (the pair levels' record scatter follows per window group).
+static int msm_bucket_sort(const MsmPlan& plan, const MsmSegment* segs, int nsegs, uint32_t sets_per_job, size_t flat_n, uint32_t TB,
+                           uint32_t* hist, uint32_t* bucket_start, uint32_t* cursors, uint32_t* sorted, void* cub_tmp, size_t cub_bytes,
+                           MsmScan scan, uint32_t* d_flags, cudaStream_t stream) {
+    for (int pass = 0; pass < (sorted ? 2 : 1); pass++) {
+        for (int i = 0; i < nsegs; i++)
+            if (segs[i].n) launch_digits(pass == 1, plan, segs[i], flat_n, segs[i].job * sets_per_job * plan.nbuckets, pass ? cursors : hist,
+                                         pass ? sorted : nullptr, d_flags, stream);
+        if (pass == 0) {
+            int rc = scan(cub_tmp, cub_bytes, hist, bucket_start, (size_t)TB + 1, stream);
+            if (rc == 0) rc = (int)cudaMemcpyAsync(cursors, bucket_start, (size_t)(TB + 1) * 4, cudaMemcpyDeviceToDevice, stream);
+            if (rc) return rc;
+            count_launch();                                       // the cursor copy
+        }
+    }
+    return (int)cudaGetLastError();
+}
+
+// the gather path's points: every base array, back to back as 128-byte records
+static int msm_densify(const MsmBases* bases, int nbases, uint32_t* dense_bases, cudaStream_t stream) {
+    size_t at = 0;
+    for (int i = 0; i < nbases; i++) {
+        if (bases[i].n == 0) continue;
+        k_densify_bases<<<(unsigned)((bases[i].n + 255) / 256), 256, 0, stream>>>((const uint8_t*)bases[i].d_points, bases[i].stride, bases[i].n,
+                                                                                dense_bases + at * BASE_WORDS);
+        count_launch();
+        at += bases[i].n;
+    }
+    return (int)cudaGetLastError();
+}
+
+// Gather path: work items of ≤ item_cap sorted entries per bucket, each summed in XYZZ from the densified bases or the tables.
+// The item count and its scan run outside every profiling scope.
+static int msm_gather_accumulate(const MsmCall& mc, MsmGroup& g) {
+    const uint32_t cap = mc.path.item_cap;
+    k_items_per_bucket<<<(g.tb + 256) / 256, 256, 0, mc.stream>>>(mc.hist + (size_t)g.w0 * mc.plan.nbuckets, mc.items, g.tb, cap,
+                                                                  mc.path.fold != MsmPath::FOLD_SCAN ? mc.hot_dev : nullptr,
+                                                                  (uint32_t)mc.hot_max, mc.path.hot_keep());
+    count_launch();
+    const int rc = scan_counted_once(mc.cub_tmp, mc.cub_bytes, mc.items, mc.item_start, (size_t)g.tb + 1, mc.stream);
+    if (rc) return rc;
+    const size_t group_items = (size_t)g.tb + g.entries / cap + 1;
+    g.items_launched = group_items;
+    // q8: ≤ 17 partials per bucket, summed by k_bucket_reduce_quad without folds
+    g.items_bound = mc.path.acc == MsmPath::ACC_Q8 ? 1 : mc.set_cap / cap + 1;
+    const uint32_t* src = mc.flat ? mc.table : mc.dense_bases;
+    ProfScope acc_scope(PROF_MSM_ACCUMULATE, mc.stream);
+    if (mc.path.acc == MsmPath::ACC_Q8)
+        k_bucket_accumulate_q8<<<(unsigned)((group_items * 32 + 127) / 128), 128, 0, mc.stream>>>(src, mc.sorted, g.bs, mc.item_start, g.tb, cap, mc.partial);
+    else if (mc.path.acc == MsmPath::ACC_G8)
+        k_bucket_accumulate_g8<<<(unsigned)((group_items * ACC_G + 127) / 128), 128, 0, mc.stream>>>(src, mc.sorted, g.bs, mc.item_start, g.tb, cap, mc.partial);
+    else
+        k_bucket_accumulate<<<(unsigned)((group_items + MSM_ACC_THREADS - 1) / MSM_ACC_THREADS), MSM_ACC_THREADS, 0, mc.stream>>>(
+            src, mc.sorted, g.bs, mc.item_start, g.tb, cap, mc.partial);
+    count_launch();
+    return (int)cudaGetLastError();
+}
+
+static void launch_scatter_records(const MsmCall& mc, const MsmSegment& sg, const uint8_t* points, size_t stride, int w_lo, int w_hi, const uint32_t* bs) {
+    const auto k = mc.flat ? (sg.mont ? k_scatter_records<true, true> : k_scatter_records<false, true>)
+                           : (sg.mont ? k_scatter_records<true, false> : k_scatter_records<false, false>);
+    k<<<(unsigned)((sg.n + 255) / 256), 256, 0, mc.stream>>>((const uint32_t*)sg.d_scalars, sg.n, points, stride, mc.table, mc.flat_n, mc.plan.c,
+                                                             mc.plan.c_top, mc.plan.nwin, mc.plan.nbuckets, mc.cursors,
+                                                             sg.job * mc.sets_per_job * mc.plan.nbuckets, w_lo, w_hi, bs, (uint4*)mc.dense0, mc.rec_words);
+    count_launch();
+}
+// Pair-level path: the group's level-0 records, the batched-affine pair levels over them, and the XYZZ sums of what is left.
+// seg_points / seg_stride: where each segment's points start in its base array (nullptr / 0 in table mode).
+static int msm_pair_accumulate(const MsmCall& mc, MsmGroup& g, const MsmSegment* segs, int nsegs, const uint8_t* const* seg_points,
+                               const size_t* seg_stride) {
+    const cudaStream_t stream = mc.stream;
+    const uint32_t tb = g.tb;
+    {
+        // this group's records: every segment re-derives its digits and emits the windows that fall into the group
+        ProfScope sort_scope(PROF_MSM_SORT, stream);
+        for (int i = 0; i < nsegs; i++) {
+            const MsmSegment& sg = segs[i];
+            if (sg.n == 0) continue;
+            // windows of this segment inside the group: its job's windows are [job·wins, (job+1)·wins)
+            const int64_t first = (int64_t)sg.job * mc.wins_per_job;
+            int w_lo, w_hi;
+            if (mc.flat) {                                                                // one set per job: all windows or none
+                if (first < (int64_t)g.u0 || first >= (int64_t)g.u0 + g.un) continue;
+                w_lo = 0; w_hi = mc.plan.nwin;
+            } else {
+                const int64_t lo_w = (int64_t)g.u0 - first, hi_w = (int64_t)g.u0 + g.un - first;
+                w_lo = lo_w < 0 ? 0 : (int)lo_w; w_hi = hi_w > mc.plan.nwin ? mc.plan.nwin : (int)hi_w;
+                if (w_lo >= w_hi) continue;
+            }
+            launch_scatter_records(mc, sg, seg_points[i], seg_stride[i], w_lo, w_hi, g.bs);
+        }
+    }
+    ProfScope acc_scope(PROF_MSM_ACCUMULATE, stream);
+    const uint32_t* off_in = g.bs;
+    uint32_t* off_bufs[2] = {mc.off_a, mc.off_b};
+    uint32_t* dense_bufs[2] = {mc.dense_a, mc.dense_b};
+    const uint32_t* dense_in = mc.dense0;
+    size_t bound = g.entries;                                // upper bound on the level's input count
+    int rc = 0;
+    for (int l = 0; l < mc.plan.levels; l++) {
+        uint32_t* off_out = off_bufs[l & 1];
+        uint32_t* dense_out = dense_bufs[l & 1];
+        k_halve_counts<<<(tb + 256) / 256, 256, 0, stream>>>(off_in, mc.cnt_tmp, mc.pair_cnt, tb);
+        count_launch();
+        if ((rc = scan_counted_once(mc.cub_tmp, mc.cub_bytes, mc.cnt_tmp, off_out, (size_t)tb + 1, stream)) != 0) return rc;
+        if ((rc = scan_counted_once(mc.cub_tmp, mc.cub_bytes, mc.pair_cnt, mc.pair_off, (size_t)tb + 1, stream)) != 0) return rc;
+        // pairs: Σ ⌊cnt/2⌋ ≤ Σ cnt/2; all outputs (pairs and single inputs): Σ ⌈cnt/2⌉ ≤ Σ cnt/2 + #buckets
+        const size_t pair_bound = bound / 2;
+        bound = bound / 2 + tb;
+        // Whole waves: 132 SMs × 4 resident CTAs × 128 threads = 67584 lanes run at once on an H100; give every lane
+        // the same number T of pairs and launch an integer number of such waves, so no partial last wave
+        // idles most of the machine (a level is one long-running CTA per slot, not many short ones).
+        const size_t wave = (size_t)mc.sm_count * PAIR_MIN_BLOCKS * PAIR_THREADS;
+        size_t waves = (pair_bound + 1024 * wave - 1) / (1024 * wave);
+        if (waves == 0) waves = 1;
+        size_t T = (pair_bound + waves * wave - 1) / (waves * wave);
+        if (T == 0) T = 1;
+        const size_t nthreads = pair_bound > T ? (pair_bound + T - 1) / T : 1;
+        const unsigned lgrid = (unsigned)((nthreads + 127) / 128);
+        // one thread per bucket (single inputs) and one warp per 32·DESC_CHUNKS pairs
+        const size_t desc_warps = (pair_bound + 32 * DESC_CHUNKS - 1) / (32 * DESC_CHUNKS);
+        const size_t desc_threads = desc_warps * 32 > (size_t)tb ? desc_warps * 32 : (size_t)tb;
+        const unsigned dgrid = (unsigned)((desc_threads + 255) / 256);
+        // level 0 reads the group's records, whose first one sits at the absolute position *bs (off_in = bs); its
+        // outputs and all later levels are group-relative (the scans start at 0)
+        const uint32_t in_words = l == 0 ? mc.rec_words : (uint32_t)DENSE_WORDS;
+        k_pair_desc<false><<<dgrid, 256, 0, stream>>>(off_in, off_out, mc.pair_off, tb, mc.desc, l == 0 ? g.bs : nullptr, dense_in, in_words, dense_out);
+        k_pair_level2<false, PAIR_MIN_BLOCKS><<<lgrid, 128, PAIR2_SMEM, stream>>>(dense_in, in_words, mc.desc, mc.pair_off + tb, (uint32_t)T, mc.prefix,
+                                                                                 dense_out, mc.sm_slots);
+        count_launch(2);
+        off_in = off_out;
+        dense_in = dense_out;
+    }
+    k_items_from_offsets<<<(tb + 256) / 256, 256, 0, stream>>>(off_in, mc.items, tb, mc.plan.cap,
+                                                               mc.path.fold != MsmPath::FOLD_SCAN ? mc.hot_dev : nullptr, (uint32_t)mc.hot_max,
+                                                               mc.path.hot_keep());
+    count_launch();
+    if ((rc = scan_counted_once(mc.cub_tmp, mc.cub_bytes, mc.items, mc.item_start, (size_t)tb + 1, stream)) != 0) return rc;
+    const size_t group_items = (size_t)tb + bound / mc.plan.cap + 1;
+    g.items_bound = ((mc.set_cap >> mc.plan.levels) + 1) / mc.plan.cap + 1;
+    g.items_launched = group_items;
+    k_bucket_accumulate_dense<<<(unsigned)((group_items + MSM_ACC_THREADS - 1) / MSM_ACC_THREADS), MSM_ACC_THREADS, 0, stream>>>(
+        dense_in, off_in, mc.item_start, tb, mc.plan.cap, mc.partial);
+    count_launch();
+    return (int)cudaGetLastError();
+}
+
+// List-driven quad folds of the hot buckets, 32:1 per round, as many rounds as the worst case needs for no bucket to hold more
+// than `keep` item partials.  The partials stay at their bucket's offset, alternating between partial and partial2 by the round's
+// parity.  Returns the number of rounds.
+static int msm_fold_hot(const MsmCall& mc, size_t worst, uint32_t keep) {
+    int rounds = 0;
+    const uint32_t* p_in = mc.partial;
+    uint32_t* p_out = mc.partial2;
+    while (worst > keep) {
+        k_fold_hot_quad<<<(unsigned)mc.sm_count * 8, 128, 0, mc.stream>>>(p_in, mc.item_start, mc.hot_dev, (uint32_t)mc.hot_max, (uint32_t)rounds, keep, p_out);
+        count_launch();
+        worst = (worst + 31) / 32;
+        rounds++;
+        const uint32_t* t = p_in; p_in = p_out; p_out = (uint32_t*)t;
+    }
+    return rounds;
+}
+static int msm_fold(const MsmCall& mc, MsmGroup& g) {
+    uint32_t *partial = mc.partial, *start = mc.item_start;
+    g.quad_rounds = 0;
+    int rc = 0;
+    if (mc.path.fold != MsmPath::FOLD_SCAN) g.quad_rounds = msm_fold_hot(mc, g.items_bound, mc.path.hot_keep());
+    else rc = msm_scan_fold(k_partial_group_sum, scan_counted_once, &partial, mc.partial2, &start, mc.items2, mc.cnt_tmp, g.tb, g.items_bound,
+                            g.items_launched, mc.cub_tmp, mc.cub_bytes, mc.stream);
+    g.partial = partial;
+    g.start = start;
+    return rc ? rc : (int)cudaGetLastError();
+}
+// bucket reduction and window combine of the group's bucket sets into its window sums
+static int msm_tail(const MsmCall& mc, const MsmGroup& g, uint32_t* group_sums) {
+    const cudaStream_t stream = mc.stream;
+    const uint32_t nbuckets = mc.plan.nbuckets, wn = g.wn, chunks_per_set = mc.chunks_per_set;
+    const SetOffsets so = set_offsets(mc.plan, mc.flat, g.w0);
+    if (mc.path.tail == MsmPath::TAIL_QUAD_SMALL) {
+        const uint32_t qchunks = (nbuckets + 7u) / 8u;                          // ≤ 128
+        k_bucket_reduce_quad<<<(wn * qchunks * 32u + 127u) / 128u, 128, 0, stream>>>(
+            g.partial, mc.path.fold == MsmPath::FOLD_HOT32 ? mc.partial2 : g.partial, g.start, g.quad_rounds, nbuckets, qchunks, wn, mc.red_a);
+        const uint32_t* ent = mc.red_a;
+        uint32_t m = qchunks;
+        int lgw = 3;
+        if (m > 64u) {                                                          // c = 11: 128 entries → 16
+            const uint32_t groups = (m + 7u) / 8u;
+            k_combine_level_quad<<<(wn * groups * 32u + 127u) / 128u, 128, 0, stream>>>(ent, m, wn, lgw, mc.red_b);
+            count_launch();
+            ent = mc.red_b; m = groups; lgw += 3;
+        }
+        k_window_combine_quad<<<wn, 32u * ((m + 7u) / 8u), 0, stream>>>(ent, m, lgw, group_sums, so);
+        count_launch(2);
+        return (int)cudaGetLastError();
+    }
+    const uint32_t nthreads = chunks_per_set * wn;
+    if (mc.path.tail == MsmPath::TAIL_QUAD_LARGE) {
+        // one thread per 16-bucket chunk leaves its (weighted sum, sum) pair; the chunk offsets are applied by 8:1 quad-lane
+        // folds (span 16 → 128 → 1024 → …), the last ≤ 64 entries of a set inside one CTA
+        k_bucket_reduce<true><<<(nthreads + 127) / 128, 128, 0, stream>>>(g.partial, g.start, nbuckets, mc.chunk, chunks_per_set, wn, mc.red_a,
+                                                                            mc.partial2, g.quad_rounds);
+        count_launch(1);
+        const uint32_t* ent = mc.red_a;
+        uint32_t* other = mc.red_b;
+        uint32_t m = chunks_per_set;
+        int lgw = 0;
+        while ((1u << lgw) < mc.chunk) lgw++;
+        while (m > 64u) {
+            const uint32_t groups = (m + 7u) / 8u;
+            if ((size_t)wn * groups >= 2048)                    // many groups: one quad each, sequential
+                k_combine_level_quadseq<<<(unsigned)(((size_t)wn * groups * 4 + 127) / 128), 128, 0, stream>>>(ent, m, wn, lgw, other);
+            else
+                k_combine_level_quad<<<(wn * groups * 32u + 127u) / 128u, 128, 0, stream>>>(ent, m, wn, lgw, other);
+            count_launch();
+            uint32_t* done = other; other = (uint32_t*)ent; ent = done;
+            m = groups; lgw += 3;
+        }
+        k_window_combine_quad<<<wn, 32u * ((m + 7u) / 8u), 0, stream>>>(ent, m, lgw, group_sums, so);
+        count_launch();
+        return (int)cudaGetLastError();
+    }
+    k_bucket_reduce<false><<<(nthreads + 127) / 128, 128, 0, stream>>>(g.partial, g.start, nbuckets, mc.chunk, chunks_per_set, wn, mc.red_a,
+                                                                         nullptr, 0, so);
+    count_launch(1);
+    return msm_tree_sum(k_group_sum, mc.red_a, mc.red_b, chunks_per_set, wn, XYZZ_WORDS, group_sums, stream);
+}
 
 // The general form: `njobs` independent sums (one per committed polynomial), each fed by one or more scalar segments,
 // over ONE set of resident bases.  All jobs go through one digit/sort pass keyed by (job, window, bucket), one set of pair
@@ -1363,16 +1678,14 @@ struct Arena {
 // one bucket set, so the pipeline sees ONE set of n·nwin entries per job and writes a single sum per job.
 int msm_core(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, const MsmBases* bases, int nbases,
              const uint32_t* table, size_t table_n, const MsmSegment* segs, int nsegs, int njobs, cudaStream_t stream) {
-    int rc = 0;
     const bool flat = table != nullptr;
     const uint32_t sets_per_job = flat ? 1u : (uint32_t)plan.nsets;  // bucket sets to reduce per job
     const uint32_t wins_per_job = flat ? 1u : (uint32_t)plan.nwin;   // windows per job, each ≤ one scalar's worth of entries
     if (njobs < 1 || nsegs < 1 || (!flat && nbases < 1)) return (int)cudaErrorInvalidValue;
     if (plan.nsets < plan.nwin || plan.nwin < 1 || (flat && plan.nsets != plan.nwin)) return (int)cudaErrorInvalidValue;
-    const uint64_t nsets64 = (uint64_t)njobs * sets_per_job;
-    const uint64_t TB64 = nsets64 * plan.nbuckets;
+    const uint64_t TB64 = (uint64_t)njobs * sets_per_job * plan.nbuckets;
     if (TB64 >= (1ull << 31)) return (int)cudaErrorInvalidValue;
-    const uint32_t nsets = (uint32_t)nsets64, TB = (uint32_t)TB64;
+    const uint32_t TB = (uint32_t)TB64;
     size_t total_scalars = 0, total_bases = 0;
     std::vector<size_t> job_n((size_t)njobs, 0);
     for (int i = 0; i < nbases; i++) {
@@ -1419,7 +1732,8 @@ int msm_core(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, co
     // windows at a time.  Fewer groups mean fewer, larger pair-level launches (H100 SXM, 700 W: 116 ms of kernels in one group against 121 ms
     // in two).  A window holds at most one entry per scalar whatever the number of its sets.
     size_t budget = 0;
-    if ((rc = scratch_group_budget(&budget)) != 0) return rc;
+    int rc = scratch_group_budget(&budget);
+    if (rc) return rc;
     if (const char* e = getenv("SNARKVM_B200_MSM_SCRATCH_GB")) { long v = atol(e); if (v >= 1) budget = (size_t)v << 30; }
     if (const char* e = getenv("SNARKVM_B200_MSM_SCRATCH_MB")) { long v = atol(e); if (v >= 1) budget = (size_t)v << 20; }      // tests: force many groups
     const uint32_t nwins = (uint32_t)njobs * wins_per_job;
@@ -1446,108 +1760,64 @@ int msm_core(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, co
     size_t entries_g = set_cap * (size_t)gu;                      // most entries a group can hold
     if (entries_g > max_entries) entries_g = max_entries;
     if (levels > 0 && entries_g >= 0x7fffffffull) return (int)cudaErrorInvalidValue;      // record positions carry the sign in bit 31
-    // small problems take the quad-lane latency path (k_bucket_reduce_quad, k_window_combine_quad)
-    const bool warp_reduce = plan.nbuckets <= 1024u;
-    // (measured: eight lanes per item win only while the whole problem is a few CTAs — up to 2^10 points, equal at 2^12, and
-    // from 2^14 they lose to the butterfly's extra additions)
-    bool acc_g8 = levels == 0 && max_entries <= 100000;
-    // round 2 (quad.cuh): four lanes per point operation.  One warp per work item (k_bucket_accumulate_q8) while the whole
-    // problem is a few thousand buckets — every lane of the warp executes every multiplication, so it costs 3× the
-    // multiplier time of the one-thread kernel and only pays while the GPU is mostly idle; the item holds up to 1/16 of a
-    // bucket set, so a bucket has ≤ 17 item partials, k_bucket_reduce_quad adds them itself and the 32:1 folds are skipped.
-    // (measured with tools/phase_sizes.py: the warp-per-item kernel wins at 2^8 points and loses from 2^10, where the 1400 items
-    // no longer fit one wave of 255-register warps)
-    const bool acc_q8 = warp_reduce && levels == 0 && (size_t)TB + max_entries / 32 <= 1100;
-    // Large bucket sets: quad-lane combine levels after the per-chunk reduction (measured with tools/phase_sizes.py: faster at
-    // 2^20, 2^22 and 2^24; at 2^19 — 4096 buckets per window, 256 chunks — the shorter old chain wins), and the hot buckets
-    // folded by the list-driven quad kernel down to ONE partial per bucket (a lone thread adds what is left of a bucket in
-    // k_bucket_reduce, so nothing may be left), instead of two scan + copy passes over every bucket
-    const bool quad_tail_large = plan.nbuckets >= 16384u;
-    // scan-free 32:1 folds of the hot buckets (a device-side list of those with more than 32 item partials)
-    const bool quad_fold = warp_reduce && levels == 0;
-    const uint32_t hot_keep = quad_tail_large ? 1u : 32u;
-    if (acc_q8) acc_g8 = false;
-    uint32_t item_cap = plan.cap;                                  // points per work item of the XYZZ accumulation
-    if (acc_g8) {                                                  // eight lanes per item: 8 × (4 … 16) points
-        size_t per_lane = max_entries / 300000 + 1;
-        if (per_lane < 4) per_lane = 4;
-        if (per_lane > 16) per_lane = 16;
-        item_cap = (uint32_t)per_lane * 8u;
-        if (const char* e = getenv("SNARKVM_B200_MSM_CAP")) { long v = atol(e); if (v >= 1) item_cap = (uint32_t)v; }
-    }
-    if (acc_q8) {
-        size_t cap16 = ((set_cap + 15) / 16 + 7) & ~(size_t)7;
-        item_cap = (uint32_t)(cap16 < 32 ? 32 : cap16);
-    } else if (quad_fold && !acc_g8 && max_entries <= 900000) {
-        // latency-bound sizes (2^12 … 2^15 points): 4 … 8 dependent mixed additions per thread instead of 16; the extra item
-        // partials of a bucket cost the quad reduction 4 multiplication steps each (swept with tools/phase_sizes.py: 4 wins at
-        // 2^12, 8 at 2^13 … 2^15)
-        item_cap = max_entries <= 150000 ? 4 : 8;
-        if (const char* e = getenv("SNARKVM_B200_MSM_CAP")) { long v = atol(e); if (v >= 1) item_cap = (uint32_t)v; }
-    }
-    const bool small_cap = quad_fold && !acc_g8 && !acc_q8 && item_cap != plan.cap;
-    const size_t max_items = (size_t)TBg + entries_g / (item_cap < plan.cap ? item_cap : plan.cap) + 1;
-    const size_t hot_max = max_items / 2 + 1;                         // buckets with more than `hot_keep` (1 or 32) item partials
-    const size_t dense_cap_a = entries_g / 2 + TBg + 1, dense_cap_b = entries_g / 4 + 2 * (size_t)TBg + 1;
 
-    int sm_count = 0;
-    {
-        static std::once_flag smem_once[64];
-        int dev = 0; cudaGetDevice(&dev);
-        std::call_once(smem_once[dev & 63], [] {
-            cudaFuncSetAttribute(k_pair_level2<false, PAIR_MIN_BLOCKS>, cudaFuncAttributeMaxDynamicSharedMemorySize, PAIR2_SMEM);
-        });
-        const cudaError_t e = cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev);
-        if (e != cudaSuccess) return (int)e;
-    }
+    MsmCall mc = {};
+    mc.plan = plan;
+    mc.path = msm_path(plan, TB, max_entries, set_cap);
+    mc.flat = flat;
+    mc.table = table;
+    mc.flat_n = flat ? table_n : 0;
+    mc.sets_per_job = sets_per_job;
+    mc.wins_per_job = wins_per_job;
+    mc.rec_words = rec_words;
+    mc.set_cap = set_cap;
+    mc.stream = stream;
+    const size_t max_items = (size_t)TBg + entries_g / (mc.path.item_cap < plan.cap ? mc.path.item_cap : plan.cap) + 1;
+    mc.hot_max = max_items / 2 + 1;                               // buckets with more than hot_keep() (1 or 32) item partials
+    const size_t dense_cap_a = entries_g / 2 + TBg + 1, dense_cap_b = entries_g / 4 + 2 * (size_t)TBg + 1;
+    if ((rc = msm_device_setup(&mc.sm_count)) != 0) return rc;
     // The reduction tail is a chain of dependent point additions per thread (latency-bound for a lone warp): short chunks
     // and a narrow (8:1) tree keep that chain short — what matters at 2^16–2^20 points, where the tail is 20–50 % of the call.
-    const uint32_t chunk = plan.nbuckets < 16u ? plan.nbuckets : 16u;
-    const uint32_t tree = 8;
-    const uint32_t chunks_per_set = plan.nbuckets / chunk;
+    mc.chunk = plan.nbuckets < 16u ? plan.nbuckets : 16u;
+    mc.chunks_per_set = plan.nbuckets / mc.chunk;
+    const uint32_t tree = MSM_TREE_FANIN, chunks_per_set = mc.chunks_per_set;
 
-    size_t cub_bytes = 0;
-    if (cub::DeviceScan::ExclusiveSum(nullptr, cub_bytes, (uint32_t*)nullptr, (uint32_t*)nullptr, (int)(TB + 1), stream) != cudaSuccess) return (int)cudaErrorUnknown;
-    if (cub_bytes < 16) cub_bytes = 16;
+    if (cub::DeviceScan::ExclusiveSum(nullptr, mc.cub_bytes, (uint32_t*)nullptr, (uint32_t*)nullptr, (int)(TB + 1), stream) != cudaSuccess) return (int)cudaErrorUnknown;
+    if (mc.cub_bytes < 16) mc.cub_bytes = 16;
 
     // ---- one scratch block, carved up ----
-    uint32_t *hist, *bucket_start, *cursors, *items, *item_start, *items2, *sorted, *partial, *partial2, *red_a, *red_b;
-    uint32_t *off_a = nullptr, *off_b = nullptr, *dense_a = nullptr, *dense_b = nullptr, *prefix = nullptr, *dense_bases = nullptr, *sm_slots = nullptr;
-    uint32_t *dense0 = nullptr, *cnt_tmp = nullptr, *hot_dev = nullptr, *pair_cnt = nullptr, *pair_off = nullptr;
-    uint2* desc = nullptr;
-    uint8_t* cub_tmp;
-    Arena ar;
     auto layout = [&](Arena& a) {
-        hist = a.take<uint32_t>((size_t)TB + 1);
-        bucket_start = a.take<uint32_t>((size_t)TB + 1);
-        cursors = a.take<uint32_t>((size_t)TB + 1);
-        items = a.take<uint32_t>((size_t)TBg + 1);
-        item_start = a.take<uint32_t>((size_t)TBg + 1);
-        items2 = a.take<uint32_t>((size_t)TBg + 1);
-        sorted = levels > 0 ? nullptr : a.take<uint32_t>(max_entries);
-        cnt_tmp = a.take<uint32_t>((size_t)TBg + 1);
-        partial = a.take<uint32_t>(max_items * XYZZ_WORDS);
-        partial2 = a.take<uint32_t>(((quad_fold || quad_tail_large) ? max_items : (size_t)TBg + max_items / 32 + 2) * XYZZ_WORDS);      // quad folds keep the item layout
-        hot_dev = a.take<uint32_t>(hot_max + 2);
-        red_a = a.take<uint32_t>((size_t)gw * (2 * chunks_per_set > 2 * ((plan.nbuckets + 7u) / 8u) ? 2 * chunks_per_set : 2 * ((plan.nbuckets + 7u) / 8u)) * XYZZ_WORDS);
-        red_b = a.take<uint32_t>((size_t)gw * (chunks_per_set / tree + 1 > 2 * ((plan.nbuckets + 63u) / 64u) + 2 ? chunks_per_set / tree + 1 : 2 * ((plan.nbuckets + 63u) / 64u) + 2) * XYZZ_WORDS);
-        cub_tmp = a.take<uint8_t>(cub_bytes);
-        if (!flat && levels == 0) dense_bases = a.take<uint32_t>(total_bases * (size_t)BASE_WORDS);
+        mc.hist = a.take<uint32_t>((size_t)TB + 1);
+        mc.bucket_start = a.take<uint32_t>((size_t)TB + 1);
+        mc.cursors = a.take<uint32_t>((size_t)TB + 1);
+        mc.items = a.take<uint32_t>((size_t)TBg + 1);
+        mc.item_start = a.take<uint32_t>((size_t)TBg + 1);
+        mc.items2 = a.take<uint32_t>((size_t)TBg + 1);
+        mc.sorted = levels > 0 ? nullptr : a.take<uint32_t>(max_entries);
+        mc.cnt_tmp = a.take<uint32_t>((size_t)TBg + 1);
+        mc.partial = a.take<uint32_t>(max_items * XYZZ_WORDS);
+        mc.partial2 = a.take<uint32_t>((mc.path.fold != MsmPath::FOLD_SCAN ? max_items : (size_t)TBg + max_items / 32 + 2) * XYZZ_WORDS);      // quad folds keep the item layout
+        mc.hot_dev = a.take<uint32_t>(mc.hot_max + 2);
+        mc.red_a = a.take<uint32_t>((size_t)gw * (2 * chunks_per_set > 2 * ((plan.nbuckets + 7u) / 8u) ? 2 * chunks_per_set : 2 * ((plan.nbuckets + 7u) / 8u)) * XYZZ_WORDS);
+        mc.red_b = a.take<uint32_t>((size_t)gw * (chunks_per_set / tree + 1 > 2 * ((plan.nbuckets + 63u) / 64u) + 2 ? chunks_per_set / tree + 1 : 2 * ((plan.nbuckets + 63u) / 64u) + 2) * XYZZ_WORDS);
+        mc.cub_tmp = a.take<uint8_t>(mc.cub_bytes);
+        if (!flat && levels == 0) mc.dense_bases = a.take<uint32_t>(total_bases * (size_t)BASE_WORDS);
         if (levels > 0) {
-            dense0 = a.take<uint32_t>(entries_g * (size_t)rec_words);
-            off_a = a.take<uint32_t>((size_t)TBg + 1);
-            off_b = a.take<uint32_t>((size_t)TBg + 1);
-            dense_a = a.take<uint32_t>(dense_cap_a * DENSE_WORDS);
+            mc.dense0 = a.take<uint32_t>(entries_g * (size_t)rec_words);
+            mc.off_a = a.take<uint32_t>((size_t)TBg + 1);
+            mc.off_b = a.take<uint32_t>((size_t)TBg + 1);
+            mc.dense_a = a.take<uint32_t>(dense_cap_a * DENSE_WORDS);
             // level 1 writes its outputs (96-byte points) over the level-0 records: only level 0 reads them, and the next
             // group's scatter runs after this group's accumulation in stream order
-            if (levels > 1) dense_b = dense_cap_b * DENSE_WORDS <= entries_g * (size_t)rec_words ? dense0 : a.take<uint32_t>(dense_cap_b * DENSE_WORDS);
-            prefix = a.take<uint32_t>(dense_cap_a * 12);
-            desc = a.take<uint2>(dense_cap_a);
-            pair_cnt = a.take<uint32_t>((size_t)TBg + 1);
-            pair_off = a.take<uint32_t>((size_t)TBg + 1);
-            sm_slots = a.take<uint32_t>(256);
+            if (levels > 1) mc.dense_b = dense_cap_b * DENSE_WORDS <= entries_g * (size_t)rec_words ? mc.dense0 : a.take<uint32_t>(dense_cap_b * DENSE_WORDS);
+            mc.prefix = a.take<uint32_t>(dense_cap_a * 12);
+            mc.desc = a.take<uint2>(dense_cap_a);
+            mc.pair_cnt = a.take<uint32_t>((size_t)TBg + 1);
+            mc.pair_off = a.take<uint32_t>((size_t)TBg + 1);
+            mc.sm_slots = a.take<uint32_t>(256);
         }
     };
+    Arena ar;
     layout(ar);
     const size_t scratch_bytes = ar.off;
     void* block = nullptr;
@@ -1556,274 +1826,36 @@ int msm_core(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, co
     ar.base = (uint8_t*)block; ar.off = 0;
     layout(ar);
 
-    CUDA_TRY(cudaMemsetAsync(hist, 0, (size_t)(TB + 1) * 4, stream));
-    if (sm_slots) CUDA_TRY(cudaMemsetAsync(sm_slots, 0, 256 * 4, stream));
-    if (quad_fold) CUDA_TRY(cudaMemsetAsync(hot_dev, 0, 4, stream));     // (quad_tail_large: reset per window group below)
-    {
-        // ---- bucket sort of all jobs and windows: histogram → offsets → scatter ----
-        {
-            ProfScope sort_scope(PROF_MSM_SORT, stream);
-            for (int pass = 0; pass < (levels > 0 ? 1 : 2); pass++) {
-                for (int i = 0; i < nsegs; i++) {
-                    const MsmSegment& sg = segs[i];
-                    if (sg.n == 0) continue;
-                    const unsigned grid = (unsigned)((sg.n + 255) / 256);
-                    const uint32_t slot_base = sg.job * sets_per_job * plan.nbuckets;
-                    const uint32_t* sc = (const uint32_t*)sg.d_scalars;
-                    const size_t fl = flat ? table_n : 0;
-                    if (pass == 0) {
-                        if (sg.mont) k_digits<false, true><<<grid, 256, 0, stream>>>(sc, sg.n, plan.c, plan.c_top, plan.nwin, plan.nbuckets, hist, nullptr, fl, slot_base, sg.base0, d_flags);
-                        else k_digits<false, false><<<grid, 256, 0, stream>>>(sc, sg.n, plan.c, plan.c_top, plan.nwin, plan.nbuckets, hist, nullptr, fl, slot_base, sg.base0, d_flags);
-                    } else {
-                        if (sg.mont) k_digits<true, true><<<grid, 256, 0, stream>>>(sc, sg.n, plan.c, plan.c_top, plan.nwin, plan.nbuckets, cursors, sorted, fl, slot_base, sg.base0, d_flags);
-                        else k_digits<true, false><<<grid, 256, 0, stream>>>(sc, sg.n, plan.c, plan.c_top, plan.nwin, plan.nbuckets, cursors, sorted, fl, slot_base, sg.base0, d_flags);
-                    }
-                    count_launch();
-                }
-                if (pass == 0) {
-                    CUDA_TRY(cub::DeviceScan::ExclusiveSum(cub_tmp, cub_bytes, hist, bucket_start, (int)(TB + 1), stream));
-                    CUDA_TRY(cudaMemcpyAsync(cursors, bucket_start, (size_t)(TB + 1) * 4, cudaMemcpyDeviceToDevice, stream));
-                    count_launch(2);
-                }
-            }
-        }
-        const uint32_t* gather_src = flat ? table : dense_bases;
-        if (!flat && levels == 0) {
-            ProfScope acc_scope(PROF_MSM_ACCUMULATE, stream);
-            size_t at = 0;
-            for (int i = 0; i < nbases; i++) {
-                if (bases[i].n == 0) continue;
-                k_densify_bases<<<(unsigned)((bases[i].n + 255) / 256), 256, 0, stream>>>((const uint8_t*)bases[i].d_points, bases[i].stride, bases[i].n,
-                                                                                        dense_bases + at * BASE_WORDS);
-                count_launch();
-                at += bases[i].n;
-            }
-        }
-        for (uint32_t u0 = 0; u0 < nwins; u0 += gu) {
-            const uint32_t un = nwins - u0 < gu ? nwins - u0 : gu;                                // windows in this group
-            const uint32_t w0 = set_of(u0), wn = set_of(u0 + un) - w0;                            // its bucket sets
-            const uint32_t tb = wn * plan.nbuckets;
-            const uint32_t* bs = bucket_start + (size_t)w0 * plan.nbuckets;                       // tb + 1 absolute offsets into `sorted`
-            const SetOffsets so = set_offsets(plan, flat, w0);
-            size_t entries = set_cap * (size_t)un;                                                // bound on the group's entries
-            if (entries > max_entries) entries = max_entries;
-            if (quad_tail_large) CUDA_TRY(cudaMemsetAsync(hot_dev, 0, 4, stream));
-            size_t items_bound = 1;                                                                // ≥ item count of any single bucket
-            size_t items_launched = 1;                                                             // ≥ total item count of the group
-            const uint32_t* final_partial = nullptr;
-            const uint32_t* final_start = nullptr;
-            if (levels == 0) {
-                const uint32_t cap = (acc_g8 || acc_q8 || small_cap) ? item_cap : plan.cap;
-                k_items_per_bucket<<<(tb + 256) / 256, 256, 0, stream>>>(hist + (size_t)w0 * plan.nbuckets, items, tb, cap, (quad_fold || quad_tail_large) ? hot_dev : nullptr, (uint32_t)hot_max, hot_keep);
-                CUDA_TRY(cub::DeviceScan::ExclusiveSum(cub_tmp, cub_bytes, items, item_start, (int)(tb + 1), stream));
-                count_launch(2);
-                const size_t group_items = (size_t)tb + entries / cap + 1;
-                items_bound = set_cap / cap + 1;
-                items_launched = group_items;
-                ProfScope acc_scope(PROF_MSM_ACCUMULATE, stream);
-                if (acc_q8) {
-                    k_bucket_accumulate_q8<<<(unsigned)((group_items * 32 + 127) / 128), 128, 0, stream>>>(gather_src, sorted, bs, item_start, tb, cap, partial);
-                    items_bound = 1;                           // ≤ 17 partials per bucket: summed by k_bucket_reduce_quad, no folds
-                } else if (acc_g8)
-                    k_bucket_accumulate_g8<<<(unsigned)((group_items * ACC_G + 127) / 128), 128, 0, stream>>>(gather_src, sorted, bs, item_start, tb, cap, partial);
-                else
-                    k_bucket_accumulate<<<(unsigned)((group_items + MSM_ACC_THREADS - 1) / MSM_ACC_THREADS), MSM_ACC_THREADS, 0, stream>>>(
-                        gather_src, sorted, bs, item_start, tb, cap, partial);
-                count_launch();
-            } else {
-                {
-                    // this group's records: every segment re-derives its digits and emits the windows that fall into the group
-                    ProfScope sort_scope(PROF_MSM_SORT, stream);
-                    for (int i = 0; i < nsegs; i++) {
-                        const MsmSegment& sg = segs[i];
-                        if (sg.n == 0) continue;
-                        // windows of this segment inside the group: its job's windows are [job·wins, (job+1)·wins)
-                        const int64_t first = (int64_t)sg.job * wins_per_job;
-                        int w_lo, w_hi;
-                        if (flat) {                                                                   // one set per job: all windows or none
-                            if (first < (int64_t)u0 || first >= (int64_t)u0 + un) continue;
-                            w_lo = 0; w_hi = plan.nwin;
-                        } else {
-                            const int64_t lo_w = (int64_t)u0 - first, hi_w = (int64_t)u0 + un - first;
-                            w_lo = lo_w < 0 ? 0 : (int)lo_w; w_hi = hi_w > plan.nwin ? plan.nwin : (int)hi_w;
-                            if (w_lo >= w_hi) continue;
-                        }
-                        const unsigned grid = (unsigned)((sg.n + 255) / 256);
-                        const uint32_t slot_base = sg.job * sets_per_job * plan.nbuckets;
-                        const uint32_t* sc = (const uint32_t*)sg.d_scalars;
-                        const int ct = plan.c_top, nw = plan.nwin;
-                        if (flat) {
-                            if (sg.mont) k_scatter_records<true, true><<<grid, 256, 0, stream>>>(sc, sg.n, nullptr, 0, table, table_n, plan.c, ct, nw, plan.nbuckets, cursors, slot_base, w_lo, w_hi, bs, (uint4*)dense0, rec_words);
-                            else k_scatter_records<false, true><<<grid, 256, 0, stream>>>(sc, sg.n, nullptr, 0, table, table_n, plan.c, ct, nw, plan.nbuckets, cursors, slot_base, w_lo, w_hi, bs, (uint4*)dense0, rec_words);
-                        } else {
-                            if (sg.mont) k_scatter_records<true, false><<<grid, 256, 0, stream>>>(sc, sg.n, seg_points[i], seg_stride[i], nullptr, 0, plan.c, ct, nw, plan.nbuckets, cursors, slot_base, w_lo, w_hi, bs, (uint4*)dense0, rec_words);
-                            else k_scatter_records<false, false><<<grid, 256, 0, stream>>>(sc, sg.n, seg_points[i], seg_stride[i], nullptr, 0, plan.c, ct, nw, plan.nbuckets, cursors, slot_base, w_lo, w_hi, bs, (uint4*)dense0, rec_words);
-                        }
-                        count_launch();
-                    }
-                }
-                ProfScope acc_scope(PROF_MSM_ACCUMULATE, stream);
-                const uint32_t* off_in = bs;
-                uint32_t* off_bufs[2] = {off_a, off_b};
-                uint32_t* dense_bufs[2] = {dense_a, dense_b};
-                const uint32_t* dense_in = dense0;
-                size_t bound = entries;                                  // upper bound on the level's input count
-                for (int l = 0; l < levels; l++) {
-                    uint32_t* off_out = off_bufs[l & 1];
-                    uint32_t* dense_out = dense_bufs[l & 1];
-                    k_halve_counts<<<(tb + 256) / 256, 256, 0, stream>>>(off_in, cnt_tmp, pair_cnt, tb);
-                    CUDA_TRY(cub::DeviceScan::ExclusiveSum(cub_tmp, cub_bytes, cnt_tmp, off_out, (int)(tb + 1), stream));
-                    CUDA_TRY(cub::DeviceScan::ExclusiveSum(cub_tmp, cub_bytes, pair_cnt, pair_off, (int)(tb + 1), stream));
-                    // pairs: Σ ⌊cnt/2⌋ ≤ Σ cnt/2; all outputs (pairs and single inputs): Σ ⌈cnt/2⌉ ≤ Σ cnt/2 + #buckets
-                    const size_t pair_bound = bound / 2;
-                    bound = bound / 2 + tb;
-                    // Whole waves: 132 SMs × 4 resident CTAs × 128 threads = 67584 lanes run at once on an H100; give every lane
-                    // the same number T of pairs and launch an integer number of such waves, so no partial last wave
-                    // idles most of the machine (a level is one long-running CTA per slot, not many short ones).
-                    const size_t wave = (size_t)sm_count * PAIR_MIN_BLOCKS * PAIR_THREADS;
-                    size_t waves = (pair_bound + 1024 * wave - 1) / (1024 * wave);
-                    if (waves == 0) waves = 1;
-                    size_t T = (pair_bound + waves * wave - 1) / (waves * wave);
-                    if (T == 0) T = 1;
-                    const size_t nthreads = pair_bound > T ? (pair_bound + T - 1) / T : 1;
-                    const unsigned lgrid = (unsigned)((nthreads + 127) / 128);
-                    // one thread per bucket (single inputs) and one warp per 32·DESC_CHUNKS pairs
-                    const size_t desc_warps = (pair_bound + 32 * DESC_CHUNKS - 1) / (32 * DESC_CHUNKS);
-                    const size_t desc_threads = desc_warps * 32 > (size_t)tb ? desc_warps * 32 : (size_t)tb;
-                    const unsigned dgrid = (unsigned)((desc_threads + 255) / 256);
-                    // level 0 reads the group's records, whose first one sits at the absolute position *bs (off_in = bs); its
-                    // outputs and all later levels are group-relative (the scans start at 0)
-                    const uint32_t in_words = l == 0 ? rec_words : (uint32_t)DENSE_WORDS;
-                    k_pair_desc<false><<<dgrid, 256, 0, stream>>>(off_in, off_out, pair_off, tb, desc, l == 0 ? bs : nullptr, dense_in, in_words, dense_out);
-                    k_pair_level2<false, PAIR_MIN_BLOCKS><<<lgrid, 128, PAIR2_SMEM, stream>>>(dense_in, in_words, desc, pair_off + tb, (uint32_t)T, prefix, dense_out, sm_slots);
-                    count_launch(5);                                     // halve, two scans, descriptors, pair level
-                    off_in = off_out;
-                    dense_in = dense_out;
-                }
-                k_items_from_offsets<<<(tb + 256) / 256, 256, 0, stream>>>(off_in, items, tb, plan.cap, quad_tail_large ? hot_dev : nullptr, (uint32_t)hot_max, hot_keep);
-                CUDA_TRY(cub::DeviceScan::ExclusiveSum(cub_tmp, cub_bytes, items, item_start, (int)(tb + 1), stream));
-                const size_t group_items = (size_t)tb + bound / plan.cap + 1;
-                items_bound = ((set_cap >> levels) + 1) / plan.cap + 1;
-                items_launched = group_items;
-                k_bucket_accumulate_dense<<<(unsigned)((group_items + MSM_ACC_THREADS - 1) / MSM_ACC_THREADS), MSM_ACC_THREADS, 0, stream>>>(
-                    dense_in, off_in, item_start, tb, plan.cap, partial);
-                count_launch(3);
-            }
-            ProfScope red_scope(PROF_MSM_REDUCE, stream);
-            int quad_rounds = 0;
-            if (quad_fold) {
-                // the quad reduction adds up to 32 partials per bucket itself; buckets with more are folded 32:1 per round from the
-                // device's hot list, as many rounds as the worst case needs
-                size_t worst = acc_q8 ? 1 : items_bound;
-                const uint32_t* p_in = partial; uint32_t* p_out = partial2;
-                while (worst > 32) {
-                    k_fold_hot_quad<<<(unsigned)sm_count * 8, 128, 0, stream>>>(p_in, item_start, hot_dev, (uint32_t)hot_max, (uint32_t)quad_rounds, 32u, p_out);
-                    count_launch();
-                    worst = (worst + 31) / 32;
-                    quad_rounds++;
-                    const uint32_t* t1 = p_in; p_in = p_out; p_out = (uint32_t*)t1;
-                }
-                final_partial = partial; final_start = item_start;
-            } else if (quad_tail_large) {
-                // buckets with more than one item partial (the hot ones: few) are folded to one by the list-driven quad kernel
-                size_t worst = items_bound;
-                const uint32_t* p_in = partial; uint32_t* p_out = partial2;
-                while (worst > 1) {
-                    k_fold_hot_quad<<<(unsigned)sm_count * 8, 128, 0, stream>>>(p_in, item_start, hot_dev, (uint32_t)hot_max, (uint32_t)quad_rounds, 1u, p_out);
-                    count_launch();
-                    worst = (worst + 31) / 32;
-                    quad_rounds++;
-                    const uint32_t* t1 = p_in; p_in = p_out; p_out = (uint32_t*)t1;
-                }
-                final_partial = partial; final_start = item_start;
-            } else {
-                // fold item partials 32:1 until no bucket can hold more than one (worst case: all entries in one bucket).
-                // `worst` (≥ the item count of any single bucket) only decides when to stop; the launch covers
-                // Σ_b ceil(items_b / 32) ≤ #buckets + total/32 outputs, where `total_bound` bounds the items of ALL buckets
-                // (a few hot buckets over a full background need far more outputs than tb + worst/32).
-                size_t worst = items_bound;
-                size_t total_bound = items_launched;
-                uint32_t* p_in = partial; uint32_t* p_out = partial2;
-                uint32_t* st_in = item_start; uint32_t* st_out = items2;
-                while (worst > 1) {
-                    k_group_counts<<<(tb + 256) / 256, 256, 0, stream>>>(st_in, cnt_tmp, tb);
-                    CUDA_TRY(cub::DeviceScan::ExclusiveSum(cub_tmp, cub_bytes, cnt_tmp, st_out, (int)(tb + 1), stream));
-                    const size_t out_bound = (size_t)tb + total_bound / 32 + 1;
-                    total_bound = out_bound;
-                    k_partial_group_sum<<<(unsigned)((out_bound + 127) / 128), 128, 0, stream>>>(p_in, st_in, st_out, tb, p_out);
-                    count_launch(3);
-                    worst = (worst + 31) / 32;
-                    uint32_t* t1 = p_in; p_in = p_out; p_out = t1;
-                    uint32_t* t2 = st_in; st_in = st_out; st_out = t2;
-                }
-                final_partial = p_in; final_start = st_in;
-            }
-            uint32_t* group_sums = d_window_sums + (size_t)w0 * XYZZ_WORDS;
-            if (warp_reduce) {
-                const uint32_t qchunks = (plan.nbuckets + 7u) / 8u;                     // ≤ 128
-                k_bucket_reduce_quad<<<(wn * qchunks * 32u + 127u) / 128u, 128, 0, stream>>>(final_partial, quad_fold ? partial2 : final_partial, final_start,
-                                                                                              quad_rounds, plan.nbuckets, qchunks, wn, red_a);
-                const uint32_t* ent = red_a;
-                uint32_t m = qchunks;
-                int lgw = 3;
-                if (m > 64u) {                                                          // c = 11: 128 entries → 16
-                    const uint32_t groups = (m + 7u) / 8u;
-                    k_combine_level_quad<<<(wn * groups * 32u + 127u) / 128u, 128, 0, stream>>>(ent, m, wn, lgw, red_b);
-                    count_launch();
-                    ent = red_b; m = groups; lgw += 3;
-                }
-                k_window_combine_quad<<<wn, 32u * ((m + 7u) / 8u), 0, stream>>>(ent, m, lgw, group_sums, so);
-                count_launch(2);
-                continue;
-            }
-            const uint32_t nthreads = chunks_per_set * wn;
-            if (quad_tail_large) {
-                // one thread per 16-bucket chunk leaves its (weighted sum, sum) pair; the chunk offsets are applied by 8:1 quad-lane
-                // folds (span 16 → 128 → 1024 → …), the last ≤ 64 entries of a set inside one CTA
-                k_bucket_reduce<true><<<(nthreads + 127) / 128, 128, 0, stream>>>(final_partial, final_start, plan.nbuckets, chunk, chunks_per_set, wn, red_a,
-                                                                                    partial2, quad_rounds);
-                count_launch(1);
-                const uint32_t* ent = red_a;
-                uint32_t* other = red_b;
-                uint32_t m = chunks_per_set;
-                int lgw = 0;
-                while ((1u << lgw) < chunk) lgw++;
-                while (m > 64u) {
-                    const uint32_t groups = (m + 7u) / 8u;
-                    if ((size_t)wn * groups >= 2048)                    // many groups: one quad each, sequential
-                        k_combine_level_quadseq<<<(unsigned)(((size_t)wn * groups * 4 + 127) / 128), 128, 0, stream>>>(ent, m, wn, lgw, other);
-                    else
-                        k_combine_level_quad<<<(wn * groups * 32u + 127u) / 128u, 128, 0, stream>>>(ent, m, wn, lgw, other);
-                    count_launch();
-                    uint32_t* done = other; other = (uint32_t*)ent; ent = done;
-                    m = groups; lgw += 3;
-                }
-                k_window_combine_quad<<<wn, 32u * ((m + 7u) / 8u), 0, stream>>>(ent, m, lgw, group_sums, so);
-                count_launch();
-                continue;
-            }
-            k_bucket_reduce<false><<<(nthreads + 127) / 128, 128, 0, stream>>>(final_partial, final_start, plan.nbuckets, chunk, chunks_per_set, wn, red_a,
-                                                                                 nullptr, 0, so);
-            count_launch(1);
-            // tree over the per-chunk sums: groups of `tree` until one point per bucket set remains
-            uint32_t per_row = chunks_per_set;
-            const uint32_t* src = red_a;
-            uint32_t* bufs[2] = {red_b, red_a};
-            int which = 0;
-            while (per_row > 1) {
-                uint32_t out_per_row = (per_row + tree - 1) / tree;
-                uint32_t* target = out_per_row == 1 ? group_sums : bufs[which];
-                uint32_t nt = out_per_row * wn;
-                k_group_sum<<<(nt + 127) / 128, 128, 0, stream>>>(src, per_row, tree, out_per_row, wn, target);
-                count_launch();
-                src = target; which ^= 1; per_row = out_per_row;
-            }
-            if (chunks_per_set == 1)
-                CUDA_TRY(cudaMemcpyAsync(group_sums, red_a, (size_t)wn * XYZZ_WORDS * 4, cudaMemcpyDeviceToDevice, stream));
-        }
-        CUDA_TRY(cudaGetLastError());
+    rc = (int)cudaMemsetAsync(mc.hist, 0, (size_t)(TB + 1) * 4, stream);
+    if (rc == 0 && mc.sm_slots) rc = (int)cudaMemsetAsync(mc.sm_slots, 0, 256 * 4, stream);
+    // the hot list: one window group here, reset per group below with folds to one partial
+    if (rc == 0 && mc.path.fold == MsmPath::FOLD_HOT32) rc = (int)cudaMemsetAsync(mc.hot_dev, 0, 4, stream);
+    if (rc == 0) {
+        ProfScope sort_scope(PROF_MSM_SORT, stream);
+        rc = msm_bucket_sort(plan, segs, nsegs, sets_per_job, mc.flat_n, TB, mc.hist, mc.bucket_start, mc.cursors, mc.sorted, mc.cub_tmp,
+                             mc.cub_bytes, scan_counted_once, d_flags, stream);
     }
-done:
+    if (rc == 0 && !flat && levels == 0) {
+        ProfScope acc_scope(PROF_MSM_ACCUMULATE, stream);
+        rc = msm_densify(bases, nbases, mc.dense_bases, stream);
+    }
+    for (uint32_t u0 = 0; rc == 0 && u0 < nwins; u0 += gu) {
+        MsmGroup g = {};
+        g.u0 = u0;
+        g.un = nwins - u0 < gu ? nwins - u0 : gu;
+        g.w0 = set_of(u0);
+        g.wn = set_of(u0 + g.un) - g.w0;
+        g.tb = g.wn * plan.nbuckets;
+        g.bs = mc.bucket_start + (size_t)g.w0 * plan.nbuckets;
+        g.entries = set_cap * (size_t)g.un;
+        if (g.entries > max_entries) g.entries = max_entries;
+        if (mc.path.fold == MsmPath::FOLD_HOT1 && (rc = (int)cudaMemsetAsync(mc.hot_dev, 0, 4, stream)) != 0) break;
+        rc = levels == 0 ? msm_gather_accumulate(mc, g) : msm_pair_accumulate(mc, g, segs, nsegs, seg_points.data(), seg_stride.data());
+        if (rc) break;
+        ProfScope red_scope(PROF_MSM_REDUCE, stream);
+        rc = msm_fold(mc, g);
+        if (rc == 0) rc = msm_tail(mc, g, d_window_sums + (size_t)g.w0 * XYZZ_WORDS);
+    }
     scratch_release(block, scratch_bytes, stream, ds);
     return rc;
 }
@@ -1842,27 +1874,55 @@ int msm_sort_indices(const MsmPlan& plan, const void* d_scalars, size_t n, int m
                      uint32_t* sorted, void* cub_tmp, size_t cub_bytes, uint32_t* d_flags, cudaStream_t stream) {
     if (plan.nsets != plan.nwin || plan.c_top != plan.c) return (int)cudaErrorInvalidValue;        // G2 takes the uniform plans
     const uint32_t TB = (uint32_t)plan.nwin * plan.nbuckets;
-    int rc = (int)cudaMemsetAsync(hist, 0, (size_t)(TB + 1) * 4, stream);
+    const int rc = (int)cudaMemsetAsync(hist, 0, (size_t)(TB + 1) * 4, stream);
     if (rc) return rc;
-    const unsigned grid = (unsigned)((n + 255) / 256);
-    const uint32_t* sc = (const uint32_t*)d_scalars;
-    if (mont) k_digits<false, true><<<grid, 256, 0, stream>>>(sc, n, plan.c, plan.c_top, plan.nwin, plan.nbuckets, hist, nullptr, 0, 0u, 0u, d_flags);
-    else k_digits<false, false><<<grid, 256, 0, stream>>>(sc, n, plan.c, plan.c_top, plan.nwin, plan.nbuckets, hist, nullptr, 0, 0u, 0u, d_flags);
-    if ((rc = msm_exclusive_scan(cub_tmp, cub_bytes, hist, bucket_start, (size_t)TB + 1, stream)) != 0) return rc;
-    if ((rc = (int)cudaMemcpyAsync(cursors, bucket_start, (size_t)(TB + 1) * 4, cudaMemcpyDeviceToDevice, stream)) != 0) return rc;
-    if (mont) k_digits<true, true><<<grid, 256, 0, stream>>>(sc, n, plan.c, plan.c_top, plan.nwin, plan.nbuckets, cursors, sorted, 0, 0u, 0u, d_flags);
-    else k_digits<true, false><<<grid, 256, 0, stream>>>(sc, n, plan.c, plan.c_top, plan.nwin, plan.nbuckets, cursors, sorted, 0, 0u, 0u, d_flags);
-    count_launch(3);
-    return (int)cudaGetLastError();
+    const MsmSegment sg{d_scalars, n, 0u, 0u, mont};
+    return msm_bucket_sort(plan, &sg, 1, (uint32_t)plan.nwin, 0, TB, hist, bucket_start, cursors, sorted, cub_tmp, cub_bytes, msm_exclusive_scan,
+                           d_flags, stream);
 }
 int msm_items_per_bucket(const uint32_t* hist, uint32_t* items, uint32_t total_buckets, uint32_t cap, cudaStream_t stream) {
     k_items_per_bucket<<<(total_buckets + 256) / 256, 256, 0, stream>>>(hist, items, total_buckets, cap, nullptr, 0u, 32u);
     count_launch();
     return (int)cudaGetLastError();
 }
-int msm_group_counts(const uint32_t* start_in, uint32_t* cnt_out, uint32_t total_buckets, cudaStream_t stream) {
-    k_group_counts<<<(total_buckets + 256) / 256, 256, 0, stream>>>(start_in, cnt_out, total_buckets);
-    count_launch();
+// fold item partials 32:1 until no bucket can hold more than one (worst case: all entries in one bucket).  `worst` (≥ the item
+// count of any single bucket) only decides when to stop; a round's launch covers Σ_b ceil(items_b / 32) ≤ #buckets + total/32
+// outputs, where `total_bound` bounds the items of ALL buckets (a few hot buckets over a full background need far more outputs
+// than total_buckets + worst/32).
+int msm_scan_fold(MsmFoldKernel fold, MsmScan scan, uint32_t** partial, uint32_t* partial2, uint32_t** start, uint32_t* start2, uint32_t* cnt_tmp,
+                  uint32_t total_buckets, size_t worst, size_t total_bound, void* cub_tmp, size_t cub_bytes, cudaStream_t stream) {
+    uint32_t *p_in = *partial, *p_out = partial2, *st_in = *start, *st_out = start2;
+    int rc = 0;
+    while (worst > 1) {
+        k_group_counts<<<(total_buckets + 256) / 256, 256, 0, stream>>>(st_in, cnt_tmp, total_buckets);
+        count_launch();
+        if ((rc = scan(cub_tmp, cub_bytes, cnt_tmp, st_out, (size_t)total_buckets + 1, stream)) != 0) break;
+        const size_t out_bound = (size_t)total_buckets + total_bound / 32 + 1;
+        total_bound = out_bound;
+        fold<<<(unsigned)((out_bound + 127) / 128), 128, 0, stream>>>(p_in, st_in, st_out, total_buckets, p_out);
+        count_launch();
+        worst = (worst + 31) / 32;
+        std::swap(p_in, p_out);
+        std::swap(st_in, st_out);
+    }
+    *partial = p_in;
+    *start = st_in;
+    return rc ? rc : (int)cudaGetLastError();
+}
+// tree over `rows` rows of `per_row` partial sums (red_a): groups of MSM_TREE_FANIN until one point per row remains in `out`
+int msm_tree_sum(MsmTreeKernel sum, uint32_t* red_a, uint32_t* red_b, uint32_t per_row, uint32_t rows, size_t point_words, uint32_t* out,
+                 cudaStream_t stream) {
+    if (per_row == 1) return (int)cudaMemcpyAsync(out, red_a, (size_t)rows * point_words * 4, cudaMemcpyDeviceToDevice, stream);
+    const uint32_t* src = red_a;
+    uint32_t* bufs[2] = {red_b, red_a};
+    int which = 0;
+    while (per_row > 1) {
+        const uint32_t out_per_row = (per_row + MSM_TREE_FANIN - 1) / MSM_TREE_FANIN;
+        uint32_t* target = out_per_row == 1 ? out : bufs[which];
+        sum<<<(out_per_row * rows + 127) / 128, 128, 0, stream>>>(src, per_row, MSM_TREE_FANIN, out_per_row, rows, target);
+        count_launch();
+        src = target; which ^= 1; per_row = out_per_row;
+    }
     return (int)cudaGetLastError();
 }
 

@@ -81,14 +81,40 @@ int msm_precompute_tables_device(uint32_t* d_table, const MsmPlan& plan, const v
 int msm_precomputed_sum_device(uint32_t* d_sum, uint32_t* d_flags, const MsmPlan& plan, const uint32_t* d_table, size_t table_n, const void* d_scalars,
                                size_t nscalars, int mont, cudaStream_t stream);
 
-// Curve-independent building blocks (signed-digit bucket sort, scans, work-item counts), shared with the G2 path:
+// Bump allocator over one scratch block: a pass with base = nullptr sizes a layout, a second one over the block hands out the
+// same 256-byte-aligned pieces.
+struct Arena {
+    uint8_t* base = nullptr;
+    size_t off = 0;
+    template <class T> T* take(size_t count) {
+        T* p = base ? (T*)(base + off) : nullptr;
+        off += (count * sizeof(T) + 255) & ~(size_t)255;
+        return p;
+    }
+};
+
+// Curve-independent building blocks (signed-digit bucket sort, scans, work-item counts, hot-bucket folds, the 8:1 tree), shared
+// with the G2 path:
 size_t msm_scan_bytes(size_t count);
+// an exclusive scan of `count` u32 that counts its launches (msm_exclusive_scan: two)
+using MsmScan = int (*)(void* tmp, size_t tmp_bytes, const uint32_t* in, uint32_t* out, size_t count, cudaStream_t stream);
 int msm_exclusive_scan(void* tmp, size_t tmp_bytes, const uint32_t* in, uint32_t* out, size_t count, cudaStream_t stream);
 // hist / bucket_start / cursors: nwin·nbuckets + 1 u32 each; sorted: n·nwin u32 (point index | sign << 31, grouped by (window, bucket))
 int msm_sort_indices(const MsmPlan& plan, const void* d_scalars, size_t n, int mont, uint32_t* hist, uint32_t* bucket_start, uint32_t* cursors,
                      uint32_t* sorted, void* cub_tmp, size_t cub_bytes, uint32_t* d_flags, cudaStream_t stream);
 int msm_items_per_bucket(const uint32_t* hist, uint32_t* items, uint32_t total_buckets, uint32_t cap, cudaStream_t stream);
-int msm_group_counts(const uint32_t* start_in, uint32_t* cnt_out, uint32_t total_buckets, cudaStream_t stream);
+// Scan-driven 32:1 folds of item partials until every bucket holds one: per round k_group_counts, `scan` and the curve's `fold`
+// kernel (k_partial_group_sum, k_g2_partial_group_sum).  *partial / *start (item_start) come in as the accumulation's output and
+// go out as the last round's; partial2 / start2 are the other buffers of the ping-pong.
+using MsmFoldKernel = void (*)(const uint32_t* partial_in, const uint32_t* start_in, const uint32_t* start_out, uint32_t total_buckets,
+                               uint32_t* partial_out);
+int msm_scan_fold(MsmFoldKernel fold, MsmScan scan, uint32_t** partial, uint32_t* partial2, uint32_t** start, uint32_t* start2, uint32_t* cnt_tmp,
+                  uint32_t total_buckets, size_t worst, size_t total_bound, void* cub_tmp, size_t cub_bytes, cudaStream_t stream);
+// the curve's `sum` kernel (k_group_sum, k_g2_group_sum) over groups of MSM_TREE_FANIN; red_a holds the input and is overwritten
+static constexpr uint32_t MSM_TREE_FANIN = 8;
+using MsmTreeKernel = void (*)(const uint32_t* in, uint32_t per_row, uint32_t group, uint32_t out_per_row, uint32_t rows, uint32_t* out);
+int msm_tree_sum(MsmTreeKernel sum, uint32_t* red_a, uint32_t* red_b, uint32_t per_row, uint32_t rows, size_t point_words, uint32_t* out,
+                 cudaStream_t stream);
 
 // BLS12-377 G2 (points over Fq2; the curves the reference sends to standard::msm, msm/variable_base/standard.rs:79-118):
 // per-window sums Σ_b b·S_{w,b} as XYZZ points over Fq2 (96 words each) into d_window_sums[plan.nwin][96].

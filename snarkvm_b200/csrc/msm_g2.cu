@@ -96,16 +96,6 @@ __global__ void __launch_bounds__(128) k_g2_group_sum(const uint32_t* __restrict
     s.store(out + (size_t)t * X2W);
 }
 
-struct Arena2 {
-    uint8_t* base = nullptr;
-    size_t off = 0;
-    template <class T> T* take(size_t count) {
-        T* p = base ? (T*)(base + off) : nullptr;
-        off += (count * sizeof(T) + 255) & ~(size_t)255;
-        return p;
-    }
-};
-
 int msm_g2_window_sums_device(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, const void* d_points, size_t stride,
                               const void* d_scalars, size_t npoints, int mont, cudaStream_t stream) {
     if (!d_window_sums || !d_flags || !d_points || !d_scalars || npoints == 0 || stride < 200 || (stride & 7)) return (int)cudaErrorInvalidValue;
@@ -113,13 +103,13 @@ int msm_g2_window_sums_device(uint32_t* d_window_sums, uint32_t* d_flags, const 
     const size_t entries = npoints * (size_t)plan.nwin;
     if (TB64 >= (1ull << 31) || npoints >= (1ull << 31) || entries >= (1ull << 32)) return (int)cudaErrorInvalidValue;
     const uint32_t TB = (uint32_t)TB64, cap = plan.cap;
-    const uint32_t chunk = plan.nbuckets < 16u ? plan.nbuckets : 16u, tree = 8, chunks_per_set = plan.nbuckets / chunk;
+    const uint32_t chunk = plan.nbuckets < 16u ? plan.nbuckets : 16u, tree = MSM_TREE_FANIN, chunks_per_set = plan.nbuckets / chunk;
     const size_t max_items = (size_t)TB + entries / cap + 1;
     const size_t cub_bytes = msm_scan_bytes((size_t)TB + 1);
     uint32_t *hist, *bucket_start, *cursors, *items, *item_start, *items2, *cnt_tmp, *sorted, *partial, *partial2, *red_a, *red_b;
     uint8_t* cub_tmp;
-    Arena2 ar;
-    auto layout = [&](Arena2& a) {
+    Arena ar;
+    auto layout = [&](Arena& a) {
         hist = a.take<uint32_t>((size_t)TB + 1); bucket_start = a.take<uint32_t>((size_t)TB + 1); cursors = a.take<uint32_t>((size_t)TB + 1);
         items = a.take<uint32_t>((size_t)TB + 1); item_start = a.take<uint32_t>((size_t)TB + 1); items2 = a.take<uint32_t>((size_t)TB + 1);
         cnt_tmp = a.take<uint32_t>((size_t)TB + 1);
@@ -142,36 +132,16 @@ int msm_g2_window_sums_device(uint32_t* d_window_sums, uint32_t* d_flags, const 
     if (rc == 0) {
         k_g2_accumulate<<<(unsigned)((max_items + 127) / 128), 128, 0, stream>>>((const uint8_t*)d_points, stride, sorted, bucket_start, item_start, TB, cap, partial);
         count_launch();
-        // fold item partials 32:1 until no bucket can hold more than one (worst case: every entry in one bucket)
-        size_t worst = npoints / cap + 1, total_bound = max_items;
-        uint32_t *p_in = partial, *p_out = partial2, *st_in = item_start, *st_out = items2;
-        while (rc == 0 && worst > 1) {
-            rc = msm_group_counts(st_in, cnt_tmp, TB, stream);
-            if (rc == 0) rc = msm_exclusive_scan(cub_tmp, cub_bytes, cnt_tmp, st_out, (size_t)TB + 1, stream);
-            const size_t out_bound = (size_t)TB + total_bound / 32 + 1;
-            total_bound = out_bound;
-            k_g2_partial_group_sum<<<(unsigned)((out_bound + 127) / 128), 128, 0, stream>>>(p_in, st_in, st_out, TB, p_out);
+        // worst case: every entry in one bucket
+        uint32_t *p = partial, *st = item_start;
+        rc = msm_scan_fold(k_g2_partial_group_sum, msm_exclusive_scan, &p, partial2, &st, items2, cnt_tmp, TB, npoints / cap + 1, max_items,
+                           cub_tmp, cub_bytes, stream);
+        if (rc == 0) {
+            const uint32_t nthreads = chunks_per_set * (uint32_t)plan.nwin;
+            k_g2_bucket_reduce<<<(nthreads + 127) / 128, 128, 0, stream>>>(p, st, plan.nbuckets, chunk, chunks_per_set, (uint32_t)plan.nwin, red_a);
             count_launch();
-            worst = (worst + 31) / 32;
-            uint32_t* t1 = p_in; p_in = p_out; p_out = t1;
-            uint32_t* t2 = st_in; st_in = st_out; st_out = t2;
+            rc = msm_tree_sum(k_g2_group_sum, red_a, red_b, chunks_per_set, (uint32_t)plan.nwin, X2W, d_window_sums, stream);
         }
-        const uint32_t nthreads = chunks_per_set * (uint32_t)plan.nwin;
-        k_g2_bucket_reduce<<<(nthreads + 127) / 128, 128, 0, stream>>>(p_in, st_in, plan.nbuckets, chunk, chunks_per_set, (uint32_t)plan.nwin, red_a);
-        count_launch();
-        uint32_t per_row = chunks_per_set;
-        const uint32_t* src = red_a;
-        uint32_t* bufs[2] = {red_b, red_a};
-        int which = 0;
-        while (per_row > 1) {
-            const uint32_t out_per_row = (per_row + tree - 1) / tree;
-            uint32_t* target = out_per_row == 1 ? d_window_sums : bufs[which];
-            k_g2_group_sum<<<(out_per_row * plan.nwin + 127) / 128, 128, 0, stream>>>(src, per_row, tree, out_per_row, (uint32_t)plan.nwin, target);
-            count_launch();
-            src = target; which ^= 1; per_row = out_per_row;
-        }
-        if (chunks_per_set == 1 && rc == 0) rc = (int)cudaMemcpyAsync(d_window_sums, red_a, (size_t)plan.nwin * X2W * 4, cudaMemcpyDeviceToDevice, stream);
-        if (rc == 0) rc = (int)cudaGetLastError();
     }
     cudaFreeAsync(block, stream);
     return rc;

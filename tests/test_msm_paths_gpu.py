@@ -1,5 +1,6 @@
-"""The G1 MSM's dispatch matrix (csrc/msm.cu, msm_core): every case pins one choice of accumulation, hot-bucket folds and
-reduction tail, asserts from a torch.profiler trace of one call which kernels ran (and which did not), then runs the input
+"""The G1 MSM's dispatch matrix (csrc/msm.cu, the MsmPath that msm_path() picks for msm_core): every case pins one choice of
+accumulation (MsmPath::acc, with its item_cap), hot-bucket folds (MsmPath::fold) and reduction tail (MsmPath::tail), asserts
+from a torch.profiler trace of one call which kernels ran (and which did not), then runs the input
 families of msm_corpus.py through it and compares every result with the closed form Σ s_i·k_i·G (+ the torsion rows' part
 in big integers), and with the oracle's MSM where the input has no torsion rows and is small.
 
