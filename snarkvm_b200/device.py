@@ -353,7 +353,15 @@ def msm_window_sums_host(out: torch.Tensor, flags: torch.Tensor | None, plan_npo
                          stride: int = AFFINE_STRIDE) -> torch.Tensor:
     """msm_window_sums from HOST buffers (numpy uint8 [n, stride] points, uint64 [n, 4] canonical scalars): the library uploads
     them (ranges overlapped with the kernels, pageable memory staged through pinned buffers) and leaves the sums in `out`
-    (CUDA, [nwin, 24] int64) without synchronising."""
+    (CUDA, [nwin, 24] int64) without synchronising.  Pageable inputs may be reused once the call returns; pinned inputs are
+    read by DMA after it returns, so the caller keeps them unchanged until the stream has passed the call."""
+    if not (isinstance(points, np.ndarray) and points.dtype == np.uint8 and points.ndim == 2 and points.flags["C_CONTIGUOUS"]):
+        raise TypeError(f"points must be a C-contiguous uint8 array [n, {stride}]")
+    if points.shape[1] != stride:
+        raise ValueError(f"points rows are {points.shape[1]} bytes, the stride is {stride}")
+    if not (isinstance(scalars, np.ndarray) and scalars.dtype == np.uint64 and scalars.ndim == 2 and scalars.shape[1] == 4
+            and scalars.flags["C_CONTIGUOUS"]):
+        raise TypeError("scalars must be a C-contiguous uint64 array [n, 4]")
     npoints = scalars.shape[0]
     if npoints > points.shape[0]:
         raise ValueError(f"length mismatch {points.shape[0]} points < {npoints} scalars")

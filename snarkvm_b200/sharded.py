@@ -49,7 +49,8 @@ def msm_sharded_async(bases_shard, scalars_shard, group=None, stride: int = devi
     All ranks run under the window plan of the LARGEST shard — pass it as `plan_npoints` when known, else it is found with one
     all-reduce(MAX) (a host round trip) — so the gathered window sums share one radix; an empty shard contributes infinity.
     CUDA tensors are used where they are; numpy arrays (HOST buffers: uint8 [n, stride] points, uint64 [n, 4] scalars) are
-    uploaded by the library with the upload overlapped with the shard's kernels."""
+    uploaded by the library with the upload overlapped with the shard's kernels.  Pinned numpy inputs are read by DMA after
+    this call returns, so the caller keeps them unchanged until `result()`; pageable ones may be reused at once."""
     world = dist.get_world_size(group) if dist.is_initialized() else 1
     host = isinstance(scalars_shard, np.ndarray)
     if host:
