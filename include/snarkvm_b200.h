@@ -365,6 +365,45 @@ typedef struct {
  * 32 B Montgomery HOST.  No synchronisation. */
 SNARKVM_API int snarkvm_b200_varuna_round4_evals_device(const snarkvm_b200_round4_segment_t* segs, size_t count, const void* alpha_mont,
                                                         const void* beta_mont, void* stream);
+/* A fourth-round segment with its own challenges (many proofs in one call): the members of snarkvm_b200_round4_segment_t, then
+ * alpha and beta (32 B Montgomery each). */
+typedef struct {
+    const void* d_row;
+    const void* d_col;
+    const void* d_row_col_val;
+    uint64_t n;
+    uint8_t v_rc_mont[32], rc_mont[32], f_scale_mont[32];
+    void* d_a;
+    void* d_b;
+    void* d_f;
+    uint8_t alpha_mont[32], beta_mont[32];
+} snarkvm_b200_round4_batch_segment_t;
+/* snarkvm_b200_varuna_round4_evals_device with each segment's own alpha and beta, in the same three launches; the entry point above
+ * is a call of this kernel with its alpha and beta in every segment.  No synchronisation. */
+SNARKVM_API int snarkvm_b200_varuna_round4_evals_batch_device(const snarkvm_b200_round4_batch_segment_t* segs, size_t count, void* stream);
+
+/* One polynomial of a segmented evaluation: m Montgomery Fr coefficients at d_coeffs (low degree first) and the point. */
+typedef struct {
+    const void* d_coeffs;
+    uint64_t m;
+    uint8_t point_mont[32];
+} snarkvm_b200_poly_eval_segment_t;
+/* DensePolynomial::evaluate of every segment in one pass: one partial-sum launch over all segments (a long polynomial spreads over
+ * many CTAs), one launch that adds each segment's partials, one D2H copy and one synchronisation.  out_mont_host: count x 32 B
+ * Montgomery HOST; a segment of length 0 evaluates to 0.  snarkvm_b200_poly_evaluate_device is a one-segment call. */
+SNARKVM_API int snarkvm_b200_poly_evaluate_batch_device(void* out_mont_host, const snarkvm_b200_poly_eval_segment_t* segs, size_t count,
+                                                        void* stream);
+/* One quotient of a segmented division by (x - point): d_q receives m - 1 coefficients of d_p (m coefficients) / (x - point). */
+typedef struct {
+    void* d_q;
+    const void* d_p;
+    uint64_t m;
+    uint8_t point_mont[32];
+} snarkvm_b200_poly_divide_segment_t;
+/* KZG10::compute_witness_polynomial of every segment in three launches (local chunk values, one carry CTA per segment, final scan);
+ * segments of length 0 and 1 have empty quotients.  No synchronisation.  snarkvm_b200_poly_divide_by_linear_device is a one-segment
+ * call. */
+SNARKVM_API int snarkvm_b200_poly_divide_by_linear_batch_device(const snarkvm_b200_poly_divide_segment_t* segs, size_t count, void* stream);
 
 /* Fr Montgomery <-> canonical, n elements in HBM (to_bigint / from_bigint, fields/src/fp_256.rs:362-413). */
 SNARKVM_API int snarkvm_b200_fr_from_mont_device(void* d_out, const void* d_in, size_t n, void* stream);

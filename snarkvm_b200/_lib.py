@@ -41,7 +41,8 @@ SYMBOLS = (
     "snarkvm_b200_test_tower_op_device", "snarkvm_b200_poseidon_transcripts_device",
     "snarkvm_b200_poseidon_transcripts_resume_device", "snarkvm_b200_g1_validate_device",
     "snarkvm_b200_g1_deserialize_device", "snarkvm_b200_g1_serialize_device", "snarkvm_b200_fr_records_decode_device",
-    "snarkvm_b200_matrix_row_walk",
+    "snarkvm_b200_matrix_row_walk", "snarkvm_b200_varuna_round4_evals_batch_device", "snarkvm_b200_poly_evaluate_batch_device",
+    "snarkvm_b200_poly_divide_by_linear_batch_device",
 )
 
 
@@ -93,6 +94,21 @@ class Round4Segment(ctypes.Structure):
     _fields_ = [("d_row", ctypes.c_void_p), ("d_col", ctypes.c_void_p), ("d_row_col_val", ctypes.c_void_p), ("n", ctypes.c_uint64),
                 ("v_rc_mont", ctypes.c_uint8 * 32), ("rc_mont", ctypes.c_uint8 * 32), ("f_scale_mont", ctypes.c_uint8 * 32),
                 ("d_a", ctypes.c_void_p), ("d_b", ctypes.c_void_p), ("d_f", ctypes.c_void_p)]
+
+
+class Round4BatchSegment(ctypes.Structure):
+    """snarkvm_b200_round4_batch_segment_t"""
+    _fields_ = Round4Segment._fields_ + [("alpha_mont", ctypes.c_uint8 * 32), ("beta_mont", ctypes.c_uint8 * 32)]
+
+
+class PolyEvalSegment(ctypes.Structure):
+    """snarkvm_b200_poly_eval_segment_t"""
+    _fields_ = [("d_coeffs", ctypes.c_void_p), ("m", ctypes.c_uint64), ("point_mont", ctypes.c_uint8 * 32)]
+
+
+class PolyDivideSegment(ctypes.Structure):
+    """snarkvm_b200_poly_divide_segment_t"""
+    _fields_ = [("d_q", ctypes.c_void_p), ("d_p", ctypes.c_void_p), ("m", ctypes.c_uint64), ("point_mont", ctypes.c_uint8 * 32)]
 
 
 class FrRecordsSegment(ctypes.Structure):
@@ -191,6 +207,9 @@ def lib():
     L.snarkvm_b200_sparse_matvec_batch_device.argtypes = [ctypes.POINTER(SpmvSegment), sz, ctypes.POINTER(ctypes.c_int64), vp]
     L.snarkvm_b200_polymul_batch_device.argtypes = [ctypes.POINTER(PolymulJob), sz, vp]
     L.snarkvm_b200_varuna_round4_evals_device.argtypes = [ctypes.POINTER(Round4Segment), sz, vp, vp, vp]
+    L.snarkvm_b200_varuna_round4_evals_batch_device.argtypes = [ctypes.POINTER(Round4BatchSegment), sz, vp]
+    L.snarkvm_b200_poly_evaluate_batch_device.argtypes = [vp, ctypes.POINTER(PolyEvalSegment), sz, vp]
+    L.snarkvm_b200_poly_divide_by_linear_batch_device.argtypes = [ctypes.POINTER(PolyDivideSegment), sz, vp]
     L.snarkvm_b200_g2_prepare_device.argtypes = [vp, vp, sz, sz, ctypes.POINTER(ctypes.c_int64), vp]
     L.snarkvm_b200_pairing_products_device.argtypes = [vp, vp, vp, vp, sz, vp, sz, vp, sz, vp, sz, ctypes.POINTER(ctypes.c_int64), vp]
     L.snarkvm_b200_poseidon_transcripts_device.argtypes = [i32, vp, vp, vp, sz, sz, vp, sz, vp, sz, vp, sz, ctypes.POINTER(ctypes.c_int64), vp]

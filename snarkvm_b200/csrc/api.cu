@@ -1210,6 +1210,15 @@ int snarkvm_b200_varuna_round4_evals_device(const snarkvm_b200_round4_segment_t*
                                             const void* beta_mont, void* stream) {
     return varuna_round4_evals_device(segs, count, alpha_mont, beta_mont, (cudaStream_t)stream);
 }
+int snarkvm_b200_varuna_round4_evals_batch_device(const snarkvm_b200_round4_batch_segment_t* segs, size_t count, void* stream) {
+    return varuna_round4_evals_batch_device(segs, count, (cudaStream_t)stream);
+}
+int snarkvm_b200_poly_evaluate_batch_device(void* out_mont_host, const snarkvm_b200_poly_eval_segment_t* segs, size_t count, void* stream) {
+    return poly_evaluate_batch_device(out_mont_host, segs, count, (cudaStream_t)stream);
+}
+int snarkvm_b200_poly_divide_by_linear_batch_device(const snarkvm_b200_poly_divide_segment_t* segs, size_t count, void* stream) {
+    return poly_divide_by_linear_batch_device(segs, count, (cudaStream_t)stream);
+}
 
 int snarkvm_b200_fr_from_mont_device(void* d_out, const void* d_in, size_t n, void* stream) {
     return fr_from_mont_device(d_out, d_in, n, (cudaStream_t)stream);

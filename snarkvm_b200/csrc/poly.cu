@@ -28,6 +28,17 @@ FF_DEV Fr fr_from_arg(const FrArg& a) { Fr r;
 #pragma unroll
     for (int i = 0; i < 8; i++) r.v[i] = a.v[i]; return r; }
 
+// Segmented launches: thread (or CTA) g of the grid belongs to the last segment whose `first` is ≤ g (segments hold consecutive
+// ranges of the grid; empty ones are skipped by the search).
+template <class Seg> FF_DEV uint32_t seg_of(const Seg* __restrict__ segs, uint32_t nsegs, uint64_t g) {
+    uint32_t lo = 0, hi = nsegs;
+    while (hi - lo > 1) {
+        const uint32_t mid = lo + (hi - lo) / 2;
+        if (segs[mid].first <= g) lo = mid; else hi = mid;
+    }
+    return lo;
+}
+
 // ---------------------------------------------------------------------------------------------------------------------
 // v_i ← coeff · v_i^{-1}; zeros are skipped and stay zero (lib.rs:107, 121).  Montgomery's trick per thread over K
 // elements taken with a grid stride (coalesced), one Fermat inversion per K: ≈ 3 + 380/K multiplications per element.
@@ -146,8 +157,9 @@ int poly_divide_by_vanishing_device(void* d_q, void* d_r, const void* d_p, size_
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// Σ c_i z^i: a thread runs Horner over EVAL_K consecutive coefficients and shifts its partial by z^{first index}; the
-// CTA adds its 256 partials in shared memory; a second single-CTA launch adds the per-CTA sums.
+// Σ c_i z^i for many polynomials at once: a thread runs Horner over EVAL_K consecutive coefficients of its segment and shifts its
+// partial by z^{first index}; the CTA adds its 256 partials in shared memory.  Segment j owns the CTAs [first, first + nctas), so
+// a long polynomial spreads over many CTAs and a short one takes one; a second launch, one CTA per segment, adds its CTA sums.
 // ---------------------------------------------------------------------------------------------------------------------
 static constexpr int EVAL_K = 64, EVAL_THREADS = 256;
 FF_DEV Fr fr_pow_u64(Fr base, uint64_t e) {
@@ -164,75 +176,120 @@ FF_DEV Fr cta_sum(Fr mine, uint32_t* sh) {
     }
     return Fr::load(sh);
 }
-__global__ void __launch_bounds__(EVAL_THREADS) k_poly_eval_partial(const uint32_t* __restrict__ c, size_t m, FrArg z_arg,
+struct EvalSeg {
+    const uint32_t* c;
+    uint64_t m, first;                                  // first: the segment's first CTA of the partial-sum launch
+    uint32_t nctas, reserved;
+    FrArg z;
+};
+__global__ void __launch_bounds__(EVAL_THREADS) k_poly_eval_partial(const EvalSeg* __restrict__ segs, uint32_t nsegs,
                                                                      uint32_t* __restrict__ partial) {
     __shared__ uint4 sh4[EVAL_THREADS * 2];
-    const Fr z = fr_from_arg(z_arg);
-    const size_t t = (size_t)blockIdx.x * blockDim.x + threadIdx.x, i0 = t * EVAL_K;
+    const EvalSeg& s = segs[seg_of(segs, nsegs, blockIdx.x)];
+    const uint32_t* __restrict__ c = s.c;
+    const size_t m = s.m, t = (size_t)(blockIdx.x - s.first) * blockDim.x + threadIdx.x, i0 = t * EVAL_K;
+    const Fr z = fr_from_arg(s.z);
     Fr acc = Fr::zero();
     if (i0 < m) {
         const size_t i1 = i0 + EVAL_K < m ? i0 + EVAL_K : m;
         for (size_t i = i1; i-- > i0;) acc = acc * z + Fr::load_ldg(c + i * 8);
         acc = acc * fr_pow_u64(z, (uint64_t)i0);
     }
-    Fr s = cta_sum(acc, reinterpret_cast<uint32_t*>(sh4));
-    if (threadIdx.x == 0) s.store(partial + (size_t)blockIdx.x * 8);
+    Fr sum = cta_sum(acc, reinterpret_cast<uint32_t*>(sh4));
+    if (threadIdx.x == 0) sum.store(partial + (size_t)blockIdx.x * 8);
 }
-// CTA b adds in[b·count … (b + 1)·count) into out[b]: one CTA per row of partials
-__global__ void __launch_bounds__(EVAL_THREADS) k_fr_sum(const uint32_t* __restrict__ in, size_t count, uint32_t* __restrict__ out) {
+// CTA j adds segment j's CTA sums into out[j] (zero for an empty segment)
+__global__ void __launch_bounds__(EVAL_THREADS) k_poly_eval_sum(const EvalSeg* __restrict__ segs, const uint32_t* __restrict__ partial,
+                                                                 uint32_t* __restrict__ out) {
     __shared__ uint4 sh4[EVAL_THREADS * 2];
-    in += (size_t)blockIdx.x * count * 8;
-    out += (size_t)blockIdx.x * 8;
+    const EvalSeg& s = segs[blockIdx.x];
+    const uint32_t* in = partial + s.first * 8;
     Fr acc = Fr::zero();
-    for (size_t i = threadIdx.x; i < count; i += EVAL_THREADS) acc = acc + Fr::load_ldg(in + i * 8);
-    Fr s = cta_sum(acc, reinterpret_cast<uint32_t*>(sh4));
-    if (threadIdx.x == 0) s.store(out);
+    for (size_t i = threadIdx.x; i < s.nctas; i += EVAL_THREADS) acc = acc + Fr::load_ldg(in + i * 8);
+    Fr sum = cta_sum(acc, reinterpret_cast<uint32_t*>(sh4));
+    if (threadIdx.x == 0) sum.store(out + (size_t)blockIdx.x * 8);
+}
+
+int poly_evaluate_batch_device(void* out_mont_host, const snarkvm_b200_poly_eval_segment_t* segs, size_t count, cudaStream_t stream) {
+    if (count == 0) return 0;
+    if (!out_mont_host || !segs || count >= ((size_t)1 << 31)) return (int)cudaErrorInvalidValue;
+    std::vector<EvalSeg> table(count);
+    uint64_t ctas = 0;
+    for (size_t i = 0; i < count; i++) {
+        const snarkvm_b200_poly_eval_segment_t& s = segs[i];
+        if (s.m && !s.d_coeffs) return (int)cudaErrorInvalidValue;
+        const uint64_t blocks = ((s.m + EVAL_K - 1) / EVAL_K + EVAL_THREADS - 1) / EVAL_THREADS;
+        table[i] = EvalSeg{(const uint32_t*)s.d_coeffs, s.m, ctas, (uint32_t)blocks, 0, FrArg{}};
+        memcpy(table[i].z.v, s.point_mont, 32);
+        ctas += blocks;
+    }
+    if (ctas >= ((uint64_t)1 << 31)) return (int)cudaErrorInvalidValue;
+    if (ctas == 0) { memset(out_mont_host, 0, count * 32); return 0; }
+    // scratch: table | partial[ctas] | out[count]
+    const size_t off_partial = (count * sizeof(EvalSeg) + 255) & ~(size_t)255, off_out = off_partial + ctas * 32;
+    uint8_t* scratch = nullptr;
+    cudaError_t e = pool_alloc(&scratch, off_out + count * 32, stream);
+    if (e != cudaSuccess) return (int)e;
+    const EvalSeg* d_table = (const EvalSeg*)scratch;
+    uint32_t *partial = (uint32_t*)(scratch + off_partial), *out = (uint32_t*)(scratch + off_out);
+    int rc = (int)cudaMemcpyAsync(scratch, table.data(), count * sizeof(EvalSeg), cudaMemcpyHostToDevice, stream);
+    if (rc == 0) {
+        k_poly_eval_partial<<<(unsigned)ctas, EVAL_THREADS, 0, stream>>>(d_table, (uint32_t)count, partial);
+        k_poly_eval_sum<<<(unsigned)count, EVAL_THREADS, 0, stream>>>(d_table, partial, out);
+        count_launch(2);
+        rc = (int)cudaGetLastError();
+    }
+    if (rc == 0) rc = (int)cudaMemcpyAsync(out_mont_host, out, count * 32, cudaMemcpyDeviceToHost, stream);
+    cudaFreeAsync(scratch, stream);
+    if (rc == 0) rc = (int)cudaStreamSynchronize(stream);
+    return rc;
 }
 
 int poly_evaluate_device(void* out_mont_host, const void* d_coeffs, size_t m, const void* point_mont_host, cudaStream_t stream) {
     if (!out_mont_host || !point_mont_host) return (int)cudaErrorInvalidValue;
-    if (m == 0) { memset(out_mont_host, 0, 32); return 0; }
-    if (!d_coeffs) return (int)cudaErrorInvalidValue;
-    FrArg z;
-    memcpy(z.v, point_mont_host, 32);
-    const size_t threads = (m + EVAL_K - 1) / EVAL_K, blocks = (threads + EVAL_THREADS - 1) / EVAL_THREADS;
-    uint32_t* scratch = nullptr;
-    cudaError_t e = pool_alloc(&scratch, (blocks + 1) * 32, stream);
-    if (e != cudaSuccess) return (int)e;
-    k_poly_eval_partial<<<(unsigned)blocks, EVAL_THREADS, 0, stream>>>((const uint32_t*)d_coeffs, m, z, scratch);
-    k_fr_sum<<<1, EVAL_THREADS, 0, stream>>>(scratch, blocks, scratch + blocks * 8);
-    count_launch(2);
-    int rc = (int)cudaGetLastError();
-    if (rc == 0) rc = (int)cudaMemcpyAsync(out_mont_host, scratch + blocks * 8, 32, cudaMemcpyDeviceToHost, stream);
-    cudaFreeAsync(scratch, stream);
-    if (rc == 0) rc = (int)cudaStreamSynchronize(stream);
-    return rc;
+    snarkvm_b200_poly_eval_segment_t s{d_coeffs, m, {}};
+    memcpy(s.point_mont, point_mont_host, 32);
+    return poly_evaluate_batch_device(out_mont_host, &s, 1, stream);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
 // Quotient of p / (x − z) — the KZG witness polynomial (polycommit/kzg10/mod.rs:220-241).  q_{L−1} = p_L, q_{i−1} = p_i + z·q_i
 // (L = m − 1) is a first-order linear recurrence; it is cut into chunks of LIN_K coefficients:
 //   pass 1: each chunk's value at its low end assuming a zero carry-in (A_k),
-//   pass 2: one CTA chains the chunks, C_k = A_k + z^{len_k}·C_{k+1}, two levels deep, and leaves every chunk's carry-in,
+//   pass 2: one CTA per polynomial chains its chunks, C_k = A_k + z^{len_k}·C_{k+1}, two levels deep, and leaves every chunk's
+//           carry-in,
 //   pass 3: each chunk reruns its recurrence from the true carry-in and writes q.
-// 2 Fr multiplications per coefficient.
+// 2 Fr multiplications per coefficient.  Many polynomials share the three launches: segment j owns the chunks [first, first +
+// ⌈L/LIN_K⌉) of passes 1 and 3 and CTA j of pass 2.
 // ---------------------------------------------------------------------------------------------------------------------
 static constexpr int LIN_K = 64, LIN_THREADS = 256;
-__global__ void k_lin_local(const uint32_t* __restrict__ p, size_t L, FrArg z_arg, uint32_t* __restrict__ A) {
-    const size_t k = (size_t)blockIdx.x * blockDim.x + threadIdx.x, bot = k * LIN_K;
-    if (bot >= L) return;
-    const size_t top = bot + LIN_K < L ? bot + LIN_K : L;
-    const Fr z = fr_from_arg(z_arg);
+struct LinSeg {
+    const uint32_t* p;
+    uint32_t* q;
+    uint64_t L, first;                                  // first: the segment's first chunk
+    FrArg z;
+};
+__global__ void k_lin_local(const LinSeg* __restrict__ segs, uint32_t nsegs, uint64_t total, uint32_t* __restrict__ A) {
+    const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= total) return;
+    const LinSeg& s = segs[seg_of(segs, nsegs, g)];
+    const uint32_t* __restrict__ p = s.p;
+    const size_t L = s.L, bot = (g - s.first) * LIN_K, top = bot + LIN_K < L ? bot + LIN_K : L;
+    const Fr z = fr_from_arg(s.z);
     Fr acc = Fr::zero();
     for (size_t i = top; i-- > bot;) acc = acc * z + Fr::load_ldg(p + (i + 1) * 8);
-    acc.store(A + k * 8);
+    acc.store(A + g * 8);
 }
-__global__ void __launch_bounds__(LIN_THREADS) k_lin_carry(const uint32_t* __restrict__ A, size_t nchunks, size_t L, FrArg z_arg,
+__global__ void __launch_bounds__(LIN_THREADS) k_lin_carry(const LinSeg* __restrict__ segs, const uint32_t* __restrict__ A,
                                                             uint32_t* __restrict__ cin) {
     __shared__ uint4 shB4[LIN_THREADS * 2], shW4[LIN_THREADS * 2];
     uint32_t* shB = reinterpret_cast<uint32_t*>(shB4);
     uint32_t* shW = reinterpret_cast<uint32_t*>(shW4);
-    const Fr z = fr_from_arg(z_arg);
+    const LinSeg& s = segs[blockIdx.x];
+    const size_t L = s.L, nchunks = (L + LIN_K - 1) / LIN_K;
+    A += s.first * 8;
+    cin += s.first * 8;
+    const Fr z = fr_from_arg(s.z);
     const Fr zK = fr_pow_u64(z, LIN_K);
     const Fr zlast = fr_pow_u64(z, (uint64_t)(L - (nchunks - 1) * LIN_K));      // the highest chunk may be short
     const size_t per = (nchunks + LIN_THREADS - 1) / LIN_THREADS;
@@ -262,32 +319,61 @@ __global__ void __launch_bounds__(LIN_THREADS) k_lin_carry(const uint32_t* __res
         C = Fr::load_ldg(A + k * 8) + zl * C;
     }
 }
-__global__ void k_lin_final(const uint32_t* __restrict__ p, size_t L, FrArg z_arg, const uint32_t* __restrict__ cin, uint32_t* __restrict__ q) {
-    const size_t k = (size_t)blockIdx.x * blockDim.x + threadIdx.x, bot = k * LIN_K;
-    if (bot >= L) return;
-    const size_t top = bot + LIN_K < L ? bot + LIN_K : L;
-    const Fr z = fr_from_arg(z_arg);
-    Fr acc = Fr::load_ldg(cin + k * 8);
+__global__ void k_lin_final(const LinSeg* __restrict__ segs, uint32_t nsegs, uint64_t total, const uint32_t* __restrict__ cin) {
+    const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (g >= total) return;
+    const LinSeg& s = segs[seg_of(segs, nsegs, g)];
+    const uint32_t* __restrict__ p = s.p;
+    uint32_t* __restrict__ q = s.q;
+    const size_t L = s.L, bot = (g - s.first) * LIN_K, top = bot + LIN_K < L ? bot + LIN_K : L;
+    const Fr z = fr_from_arg(s.z);
+    Fr acc = Fr::load_ldg(cin + g * 8);
     for (size_t i = top; i-- > bot;) { acc = acc * z + Fr::load_ldg(p + (i + 1) * 8); acc.store(q + i * 8); }
+}
+
+int poly_divide_by_linear_batch_device(const snarkvm_b200_poly_divide_segment_t* segs, size_t count, cudaStream_t stream) {
+    if (count == 0) return 0;
+    if (!segs || count >= ((size_t)1 << 31)) return (int)cudaErrorInvalidValue;
+    std::vector<LinSeg> table;                               // the segments with a non-empty quotient
+    uint64_t total = 0;
+    for (size_t i = 0; i < count; i++) {
+        const snarkvm_b200_poly_divide_segment_t& s = segs[i];
+        if (s.m <= 1) continue;
+        if (!s.d_q || !s.d_p) return (int)cudaErrorInvalidValue;
+        LinSeg t{(const uint32_t*)s.d_p, (uint32_t*)s.d_q, s.m - 1, total, FrArg{}};
+        memcpy(t.z.v, s.point_mont, 32);
+        table.push_back(t);
+        total += (s.m - 1 + LIN_K - 1) / LIN_K;
+    }
+    if (table.empty()) return 0;
+    const size_t n = table.size();
+    if (total >= ((uint64_t)1 << 38)) return (int)cudaErrorInvalidValue;      // grid < 2^31 CTAs
+    // scratch: table | A[total] | cin[total]
+    const size_t off_a = (n * sizeof(LinSeg) + 255) & ~(size_t)255;
+    uint8_t* scratch = nullptr;
+    cudaError_t e = pool_alloc(&scratch, off_a + total * 64, stream);
+    if (e != cudaSuccess) return (int)e;
+    const LinSeg* d_table = (const LinSeg*)scratch;
+    uint32_t *A = (uint32_t*)(scratch + off_a), *cin = A + total * 8;
+    int rc = (int)cudaMemcpyAsync(scratch, table.data(), n * sizeof(LinSeg), cudaMemcpyHostToDevice, stream);
+    if (rc == 0) {
+        const unsigned grid = (unsigned)((total + 127) / 128);
+        k_lin_local<<<grid, 128, 0, stream>>>(d_table, (uint32_t)n, total, A);
+        k_lin_carry<<<(unsigned)n, LIN_THREADS, 0, stream>>>(d_table, A, cin);
+        k_lin_final<<<grid, 128, 0, stream>>>(d_table, (uint32_t)n, total, cin);
+        count_launch(3);
+        rc = (int)cudaGetLastError();
+    }
+    cudaFreeAsync(scratch, stream);
+    return rc;
 }
 
 int poly_divide_by_linear_device(void* d_q, const void* d_p, size_t m, const void* point_mont_host, cudaStream_t stream) {
     if (m <= 1) return 0;
-    if (!d_q || !d_p || !point_mont_host) return (int)cudaErrorInvalidValue;
-    FrArg z;
-    memcpy(z.v, point_mont_host, 32);
-    const size_t L = m - 1, nchunks = (L + LIN_K - 1) / LIN_K;
-    uint32_t* scratch = nullptr;                             // A[nchunks] then cin[nchunks]
-    cudaError_t e = pool_alloc(&scratch, nchunks * 64, stream);
-    if (e != cudaSuccess) return (int)e;
-    const unsigned grid = (unsigned)((nchunks + 127) / 128);
-    k_lin_local<<<grid, 128, 0, stream>>>((const uint32_t*)d_p, L, z, scratch);
-    k_lin_carry<<<1, LIN_THREADS, 0, stream>>>(scratch, nchunks, L, z, scratch + nchunks * 8);
-    k_lin_final<<<grid, 128, 0, stream>>>((const uint32_t*)d_p, L, z, scratch + nchunks * 8, (uint32_t*)d_q);
-    count_launch(3);
-    int rc = (int)cudaGetLastError();
-    cudaFreeAsync(scratch, stream);
-    return rc;
+    if (!point_mont_host) return (int)cudaErrorInvalidValue;
+    snarkvm_b200_poly_divide_segment_t s{d_q, d_p, m, {}};
+    memcpy(s.point_mont, point_mont_host, 32);
+    return poly_divide_by_linear_batch_device(&s, 1, stream);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -299,16 +385,6 @@ int poly_divide_by_linear_device(void* d_q, const void* d_p, size_t m, const voi
 // 2^20-constraint circuit.  They leave the thread-per-row kernel through a device-side work list — no host round trip —
 // and are cut into segments of SPMV_SEG entries, one CTA per segment, then one CTA per long row adds its segments.
 static constexpr uint32_t SPMV_LONG = 256, SPMV_SEG = 2048;
-// Segmented launches: thread g of the grid belongs to the last segment whose `first` is ≤ g (segments hold consecutive ranges of
-// the grid; empty ones are skipped by the search).
-template <class Seg> FF_DEV uint32_t seg_of(const Seg* __restrict__ segs, uint32_t nsegs, uint64_t g) {
-    uint32_t lo = 0, hi = nsegs;
-    while (hi - lo > 1) {
-        const uint32_t mid = lo + (hi - lo) / 2;
-        if (segs[mid].first <= g) lo = mid; else hi = mid;
-    }
-    return lo;
-}
 // Many mat-vecs in one pass (every instance of every circuit, or the three transposes of every circuit): thread g takes row
 // g − first of its segment; the long rows of all segments share one work list, each entry naming its segment.
 struct SpmvSeg {
@@ -1063,15 +1139,14 @@ struct Round4Seg {
     const uint32_t *row, *col, *rcv;
     uint32_t *a, *b, *f;
     uint64_t first, n;
-    FrArg v_rc, rc, scale;
+    FrArg v_rc, rc, scale, alpha, beta;
 };
-__global__ void k_round4_evals(const Round4Seg* __restrict__ segs, uint32_t nsegs, uint64_t total, FrArg alpha_arg, FrArg beta_arg,
-                               uint32_t* __restrict__ den) {
+__global__ void k_round4_evals(const Round4Seg* __restrict__ segs, uint32_t nsegs, uint64_t total, uint32_t* __restrict__ den) {
     const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (g >= total) return;
     const Round4Seg& s = segs[seg_of(segs, nsegs, g)];
     const uint64_t i = g - s.first;
-    const Fr d = (Fr::load_ldg(s.row + i * 8) - fr_from_arg(alpha_arg)) * (Fr::load_ldg(s.col + i * 8) - fr_from_arg(beta_arg));
+    const Fr d = (Fr::load_ldg(s.row + i * 8) - fr_from_arg(s.alpha)) * (Fr::load_ldg(s.col + i * 8) - fr_from_arg(s.beta));
     (fr_from_arg(s.v_rc) * Fr::load_ldg(s.rcv + i * 8)).store(s.a + i * 8);
     (fr_from_arg(s.rc) * d).store(s.b + i * 8);
     d.store(den + g * 8);
@@ -1084,23 +1159,10 @@ __global__ void k_round4_f(const Round4Seg* __restrict__ segs, uint32_t nsegs, u
     (fr_from_arg(s.scale) * Fr::load(inv + g * 8) * Fr::load_ldg(s.rcv + i * 8)).store(s.f + i * 8);
 }
 
-int varuna_round4_evals_device(const snarkvm_b200_round4_segment_t* segs, size_t count, const void* alpha_mont, const void* beta_mont,
-                               cudaStream_t stream) {
-    if (count == 0) return 0;
-    if (!segs || !alpha_mont || !beta_mont || count >= ((size_t)1 << 31)) return (int)cudaErrorInvalidValue;
-    std::vector<Round4Seg> table(count);
-    uint64_t total = 0;
-    for (size_t i = 0; i < count; i++) {
-        const snarkvm_b200_round4_segment_t& s = segs[i];
-        if (s.n == 0 || !s.d_row || !s.d_col || !s.d_row_col_val || !s.d_a || !s.d_b || !s.d_f) return (int)cudaErrorInvalidValue;
-        Round4Seg& t = table[i];
-        t = Round4Seg{(const uint32_t*)s.d_row, (const uint32_t*)s.d_col, (const uint32_t*)s.d_row_col_val, (uint32_t*)s.d_a, (uint32_t*)s.d_b,
-                      (uint32_t*)s.d_f, total, s.n, FrArg{}, FrArg{}, FrArg{}};
-        memcpy(t.v_rc.v, s.v_rc_mont, 32); memcpy(t.rc.v, s.rc_mont, 32); memcpy(t.scale.v, s.f_scale_mont, 32);
-        total += s.n;
-    }
-    FrArg alpha, beta, one{};
-    memcpy(alpha.v, alpha_mont, 32); memcpy(beta.v, beta_mont, 32);
+// the table's segments (first and n set) in one launch, one batch inversion and one launch for f
+static int round4_impl(const std::vector<Round4Seg>& table, uint64_t total, cudaStream_t stream) {
+    const size_t count = table.size();
+    FrArg one{};
     for (int k = 0; k < 8; k++) one.v[k] = FrParams::r1(k);                   // Montgomery one
     uint8_t* scratch = nullptr;                                                  // segment table | denominators, concatenated
     const size_t off_den = (count * sizeof(Round4Seg) + 255) & ~(size_t)255;
@@ -1112,7 +1174,7 @@ int varuna_round4_evals_device(const snarkvm_b200_round4_segment_t* segs, size_t
     if (rc == 0) {
         const unsigned grid = (unsigned)((total + 255) / 256);
         const size_t threads = (total + BINV_K - 1) / BINV_K;
-        k_round4_evals<<<grid, 256, 0, stream>>>(d_table, (uint32_t)count, total, alpha, beta, den);
+        k_round4_evals<<<grid, 256, 0, stream>>>(d_table, (uint32_t)count, total, den);
         k_fr_batch_inverse<<<(unsigned)((threads + 127) / 128), 128, 0, stream>>>(den, total, one);
         k_round4_f<<<grid, 256, 0, stream>>>(d_table, (uint32_t)count, total, den);
         count_launch(3);
@@ -1120,6 +1182,41 @@ int varuna_round4_evals_device(const snarkvm_b200_round4_segment_t* segs, size_t
     }
     cudaFreeAsync(scratch, stream);
     return rc;
+}
+
+template <class S> static bool round4_segment(const S& s, uint64_t first, Round4Seg* t) {
+    if (s.n == 0 || !s.d_row || !s.d_col || !s.d_row_col_val || !s.d_a || !s.d_b || !s.d_f) return false;
+    *t = Round4Seg{(const uint32_t*)s.d_row, (const uint32_t*)s.d_col, (const uint32_t*)s.d_row_col_val, (uint32_t*)s.d_a, (uint32_t*)s.d_b,
+                   (uint32_t*)s.d_f, first, s.n, FrArg{}, FrArg{}, FrArg{}, FrArg{}, FrArg{}};
+    memcpy(t->v_rc.v, s.v_rc_mont, 32); memcpy(t->rc.v, s.rc_mont, 32); memcpy(t->scale.v, s.f_scale_mont, 32);
+    return true;
+}
+
+int varuna_round4_evals_batch_device(const snarkvm_b200_round4_batch_segment_t* segs, size_t count, cudaStream_t stream) {
+    if (count == 0) return 0;
+    if (!segs || count >= ((size_t)1 << 31)) return (int)cudaErrorInvalidValue;
+    std::vector<Round4Seg> table(count);
+    uint64_t total = 0;
+    for (size_t i = 0; i < count; i++) {
+        if (!round4_segment(segs[i], total, &table[i])) return (int)cudaErrorInvalidValue;
+        memcpy(table[i].alpha.v, segs[i].alpha_mont, 32); memcpy(table[i].beta.v, segs[i].beta_mont, 32);
+        total += segs[i].n;
+    }
+    return round4_impl(table, total, stream);
+}
+
+int varuna_round4_evals_device(const snarkvm_b200_round4_segment_t* segs, size_t count, const void* alpha_mont, const void* beta_mont,
+                               cudaStream_t stream) {
+    if (count == 0) return 0;
+    if (!segs || !alpha_mont || !beta_mont || count >= ((size_t)1 << 31)) return (int)cudaErrorInvalidValue;
+    std::vector<Round4Seg> table(count);
+    uint64_t total = 0;
+    for (size_t i = 0; i < count; i++) {
+        if (!round4_segment(segs[i], total, &table[i])) return (int)cudaErrorInvalidValue;
+        memcpy(table[i].alpha.v, alpha_mont, 32); memcpy(table[i].beta.v, beta_mont, 32);
+        total += segs[i].n;
+    }
+    return round4_impl(table, total, stream);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------

@@ -72,6 +72,11 @@ int sparse_matvec_batch_device(const snarkvm_b200_spmv_segment_t* segs, size_t c
 int polymul_batch_device(const snarkvm_b200_polymul_job_t* jobs, size_t count, cudaStream_t stream);
 int varuna_round4_evals_device(const snarkvm_b200_round4_segment_t* segs, size_t count, const void* alpha_mont, const void* beta_mont,
                                cudaStream_t stream);
+// Many proofs per call: round 4 with per-segment challenges, and the segmented forms of poly_evaluate_device and
+// poly_divide_by_linear_device (both of which are one-segment calls of these).
+int varuna_round4_evals_batch_device(const snarkvm_b200_round4_batch_segment_t* segs, size_t count, cudaStream_t stream);
+int poly_evaluate_batch_device(void* out_mont_host, const snarkvm_b200_poly_eval_segment_t* segs, size_t count, cudaStream_t stream);
+int poly_divide_by_linear_batch_device(const snarkvm_b200_poly_divide_segment_t* segs, size_t count, cudaStream_t stream);
 
 // Group FFT over G1 (DomainCoeff = G1Projective, fft/domain.rs:169-221 generic path): n = 2^lg affine points in, affine points
 // out (natural order both sides).  direction 1 = inverse (includes n^{-1}): UniversalParams::lagrange_basis

@@ -917,27 +917,32 @@ def varuna_round4_evals(jobs: list, alpha_mont, beta_mont) -> list:
     """Varuna's fourth-round evaluations on K for every (row, col, row_col_val, v_rc_mont, rc_mont, f_scale_mont): three launches for all
     of them → [(a, b, f)], views of one buffer: a = v_rc·row_col_val, b = rc·(row − α)(col − β), f = f_scale·row_col_val /
     ((row − α)(col − β)), zero where the denominator is zero"""
+    return varuna_round4_evals_batch([tuple(j) + (alpha_mont, beta_mont) for j in jobs])
+
+
+def varuna_round4_evals_batch(jobs: list) -> list:
+    """varuna_round4_evals with each job's own challenges, for many proofs in one pass: every (row, col, row_col_val, v_rc_mont, rc_mont,
+    f_scale_mont, alpha_mont, beta_mont) in the same three launches → [(a, b, f)], views of one buffer"""
     if not jobs:
         return []
     dev = jobs[0][0].device
     sizes = [_nbytes(j[0]) // 32 for j in jobs]
     buf = torch.empty((3 * sum(sizes), 4), dtype=torch.int64, device=dev)
-    segs = (_lib.Round4Segment * len(jobs))()
+    segs = (_lib.Round4BatchSegment * len(jobs))()
     outs, off = [], 0
-    for k, ((row, col, rcv, v_rc, rc, scale), n) in enumerate(zip(jobs, sizes)):
+    for k, ((row, col, rcv, v_rc, rc, scale, alpha, beta), n) in enumerate(zip(jobs, sizes)):
         if _nbytes(col) != n * 32 or _nbytes(rcv) != n * 32:
             raise ValueError("length mismatch")
         trio = (buf[off: off + n], buf[off + n: off + 2 * n], buf[off + 2 * n: off + 3 * n])
         off += 3 * n
         s = segs[k]
         s.d_row, s.d_col, s.d_row_col_val, s.n = _check(row, "row"), _check(col, "col"), _check(rcv, "row_col_val"), n
-        for name, v in (("v_rc_mont", v_rc), ("rc_mont", rc), ("f_scale_mont", scale)):
+        for name, v in (("v_rc_mont", v_rc), ("rc_mont", rc), ("f_scale_mont", scale), ("alpha_mont", alpha), ("beta_mont", beta)):
             ctypes.memmove(getattr(s, name), _fr_host(v).ctypes.data, 32)
         s.d_a, s.d_b, s.d_f = (t.data_ptr() for t in trio)
         outs.append(trio)
-    a, b = _fr_host(alpha_mont), _fr_host(beta_mont)
     with torch.cuda.device(dev):
-        _lib.check(_lib.lib().snarkvm_b200_varuna_round4_evals_device(segs, len(jobs), a.ctypes.data, b.ctypes.data, _stream()))
+        _lib.check(_lib.lib().snarkvm_b200_varuna_round4_evals_batch_device(segs, len(jobs), _stream()))
     return outs
 
 
@@ -959,6 +964,41 @@ def poly_evaluate(coeffs: torch.Tensor, point_mont) -> np.ndarray:
     m = _nbytes(coeffs) // 32
     with torch.cuda.device(coeffs.device):
         _lib.check(_lib.lib().snarkvm_b200_poly_evaluate_device(out.ctypes.data, _check(coeffs, "coeffs") if m else None, m, z.ctypes.data, _stream()))
+    return out
+
+
+def poly_divide_by_linear_batch(jobs: list) -> list:
+    """poly_divide_by_linear of every (p, point_mont) in one pass of three launches → one CUDA tensor [m − 1, 4] per job (empty for m ≤ 1),
+    each equal to poly_divide_by_linear(p, point_mont)"""
+    if not jobs:
+        return []
+    segs = (_lib.PolyDivideSegment * len(jobs))()
+    outs = []
+    for k, (p, point) in enumerate(jobs):
+        m = _nbytes(p) // 32
+        q = torch.empty((max(m - 1, 0), 4), dtype=torch.int64, device=p.device)
+        s = segs[k]
+        s.d_q, s.d_p, s.m = (q.data_ptr(), _check(p, "p"), m) if m > 1 else (None, None, m)
+        ctypes.memmove(s.point_mont, _fr_host(point).ctypes.data, 32)
+        outs.append(q)
+    with torch.cuda.device(jobs[0][0].device):
+        _lib.check(_lib.lib().snarkvm_b200_poly_divide_by_linear_batch_device(segs, len(jobs), _stream()))
+    return outs
+
+
+def poly_evaluate_batch(jobs: list) -> np.ndarray:
+    """poly_evaluate of every (coeffs, point_mont) in one pass and one synchronisation → Montgomery Fr uint64[count, 4] on the host, row
+    k equal to poly_evaluate of job k (zero for an empty polynomial)"""
+    out = np.zeros((len(jobs), 4), dtype=np.uint64)
+    if not jobs:
+        return out
+    segs = (_lib.PolyEvalSegment * len(jobs))()
+    for k, (c, point) in enumerate(jobs):
+        m = _nbytes(c) // 32
+        segs[k].d_coeffs, segs[k].m = (_check(c, "coeffs") if m else None), m
+        ctypes.memmove(segs[k].point_mont, _fr_host(point).ctypes.data, 32)
+    with torch.cuda.device(jobs[0][0].device):
+        _lib.check(_lib.lib().snarkvm_b200_poly_evaluate_batch_device(out.ctypes.data, segs, len(jobs), _stream()))
     return out
 
 

@@ -169,12 +169,17 @@ class CommitterKey:
 
 def _check_degrees_and_bounds(ck: CommitterKey, p: LabeledPolynomial) -> None:
     """kzg10/mod.rs check_degrees_and_bounds: a bounded polynomial needs degree ≤ bound ≤ max_degree and an enforced bound"""
-    if p.degree_bound is not None:
-        if ck.enforced_degree_bounds is None or p.degree_bound not in ck.enforced_degree_bounds:
-            raise ValueError(f"UnsupportedDegreeBound({p.degree_bound})")
+    _check_bound(ck, p.label, p.polynomial.shape[0], p.degree_bound)
+
+
+def _check_bound(ck: CommitterKey, label: str, length: int, degree_bound: int | None) -> None:
+    """_check_degrees_and_bounds of a polynomial of `length` coefficients"""
+    if degree_bound is not None:
+        if ck.enforced_degree_bounds is None or degree_bound not in ck.enforced_degree_bounds:
+            raise ValueError(f"UnsupportedDegreeBound({degree_bound})")
         # a key read from bytes has no max_degree: its enforced bounds, all within its SRS, stand for it
-        if p.polynomial.shape[0] - 1 > p.degree_bound or (ck.max_degree is not None and p.degree_bound > ck.max_degree):
-            raise ValueError(f"IncorrectDegreeBound for {p.label}")
+        if length - 1 > degree_bound or (ck.max_degree is not None and degree_bound > ck.max_degree):
+            raise ValueError(f"IncorrectDegreeBound for {label}")
 
 
 class SonicKZG10:
@@ -183,33 +188,40 @@ class SonicKZG10:
         """mod.rs:177-257 → (commitments uint64[count, 18], [Randomness]).  All MSMs of the round — plain powers, shifted powers,
         Lagrange bases, blinding terms — go through ONE device pass (device.sonic_commit_batch).  `blindings[i]`: the blinding
         polynomial of polynomial i (hiding_bound + 2 Montgomery coefficients) when it is hiding, else None."""
-        count = len(polynomials)
-        blindings = list(blindings) if blindings is not None else [None] * count
-        bases, gammas, polys, rands = [], [], [], []
-        for p, b in zip(polynomials, blindings):
-            _check_degrees_and_bounds(ck, p)
-            if p.lagrange:
-                n = p.polynomial.shape[0]
-                size = 1 << max(n - 1, 0).bit_length()
-                basis, gamma = ck.lagrange_basis(size)
-                if n == 0 or size != basis.shape[0]:
-                    raise ValueError("evaluations do not match the Lagrange basis size")
-            elif p.degree_bound is not None:
-                basis, gamma = ck.shifted_powers(p.degree_bound)
-            else:
-                basis, gamma = ck.powers()
-            if p.hiding_bound is not None:
-                if b is None or b.shape[0] != p.hiding_bound + 2:
-                    raise ValueError(f"{p.label}: a hiding commitment needs a blinding polynomial of hiding_bound + 2 coefficients")
-                rands.append(Randomness(b))
-            else:
-                b = None
-                rands.append(Randomness())
-            bases.append(basis); gammas.append(gamma); polys.append(p.polynomial)
+        return SonicKZG10.commit_many([(ck, polynomials, blindings)])[0]
+
+    @staticmethod
+    def commit_many(items: list) -> list:
+        """commit of every (committer key, polynomials, blindings or None) in `items`, all of them in ONE device.sonic_commit_batch
+        pass → [(commitments uint64[count, 18], [Randomness])], entry k equal to commit(*items[k])"""
+        bases, gammas, polys, rands, counts = [], [], [], [], []
+        for ck, polynomials, blindings in items:
+            blindings = list(blindings) if blindings is not None else [None] * len(polynomials)
+            for p, b in zip(polynomials, blindings):
+                _check_degrees_and_bounds(ck, p)
+                if p.lagrange:
+                    n = p.polynomial.shape[0]
+                    size = 1 << max(n - 1, 0).bit_length()
+                    basis, gamma = ck.lagrange_basis(size)
+                    if n == 0 or size != basis.shape[0]:
+                        raise ValueError("evaluations do not match the Lagrange basis size")
+                elif p.degree_bound is not None:
+                    basis, gamma = ck.shifted_powers(p.degree_bound)
+                else:
+                    basis, gamma = ck.powers()
+                if p.hiding_bound is not None:
+                    if b is None or b.shape[0] != p.hiding_bound + 2:
+                        raise ValueError(f"{p.label}: a hiding commitment needs a blinding polynomial of hiding_bound + 2 coefficients")
+                    rands.append(Randomness(b))
+                else:
+                    rands.append(Randomness())
+                bases.append(basis); gammas.append(gamma); polys.append(p.polynomial)
+            counts.append(len(polynomials))
         any_hiding = any(r.is_hiding() for r in rands)
         out = device.sonic_commit_batch(bases, polys, gammas if any_hiding else None,
                                         [r.blinding_polynomial for r in rands] if any_hiding else None)
-        return out, rands
+        offs = np.concatenate([[0], np.cumsum(counts)]).astype(np.int64).tolist()
+        return [(out[a: b], rands[a: b]) for a, b in zip(offs, offs[1:])]
 
     @staticmethod
     def combine_for_open(ck: CommitterKey, labeled_polynomials: list, rands: list, challenges):
@@ -259,32 +271,81 @@ class SonicKZG10:
     def open_combinations(ck: CommitterKey, linear_combinations: list, polynomials: list, rands: list, query_set: list, challenges):
         """mod.rs:413-475.  linear_combinations: [(lc_label, [(coeff as int, polynomial label or None for the constant term)])];
         the query set names LC labels.  Returns the BatchLCProof's list of (w, random_v)."""
-        label_map = {p.label: (p, r) for p, r in zip(polynomials, rands)}
-        lc_polys, lc_rands = [], []
-        for lc_label, terms in linear_combinations:
-            poly, rand = None, Randomness()
-            degree_bound = hiding_bound = None
-            num_polys = len(terms)
-            for coeff, label in terms:
-                if label is None:                                              # LCTerm::One: not committed, used by the verifier directly
-                    continue
-                if label not in label_map:
-                    raise KeyError(f"MissingPolynomial {{ label: {label} }}")
-                cur, cur_rand = label_map[label]
-                if cur.degree_bound is not None:
-                    if num_polys != 1:
-                        raise ValueError(f"EquationHasDegreeBounds({lc_label})")
-                    assert int(coeff) % _R_MOD == 1, "Coefficient must be one for degree-bounded equations"
-                    assert degree_bound is None or degree_bound == cur.degree_bound
-                    degree_bound = cur.degree_bound
-                if cur.hiding_bound is not None:
-                    hiding_bound = cur.hiding_bound if hiding_bound is None else max(hiding_bound, cur.hiding_bound)
-                poly = poly_axpy(poly, int(coeff), cur.polynomial)
-                rand = rand.axpy(int(coeff), cur_rand)
-            dev = ck.powers_of_beta_g.device
-            lc_polys.append(LabeledPolynomial(lc_label, poly if poly is not None else _zeros(0, dev), degree_bound, hiding_bound))
-            lc_rands.append(rand)
-        return SonicKZG10.batch_open(ck, lc_polys, query_set, lc_rands, challenges)
+        return SonicKZG10.open_combinations_many([(ck, linear_combinations, polynomials, rands, query_set, challenges)])[0]
+
+    @staticmethod
+    def open_combinations_many(items: list) -> list:
+        """open_combinations of every (ck, linear_combinations, polynomials, rands, query_set, challenges) in `items` in one pass →
+        one BatchLCProof list of (w, random_v) per item, equal to open_combinations of that item.  Each query point's opening
+        challenges are folded into its linear combinations' coefficients on the host, so every (item, point) combined polynomial, and
+        its blinding polynomial, is one output of one device.fr_lincomb_terms launch; the witnesses of all of them are one
+        device.poly_divide_by_linear_batch, the random_v one device.poly_evaluate_batch and the witness commitments, hiding parts
+        included, one device.sonic_commit_batch pass.  The field is exact, so the reassociation gives the same bytes."""
+        opened = []                                  # per (item, point): (item, z, combined polynomial job, blinding job or None)
+        for k, (ck, linear_combinations, polynomials, rands, query_set, challenges) in enumerate(items):
+            label_map = {p.label: (p, r) for p, r in zip(polynomials, rands)}
+            lcs = {}                                 # lc label → (degree bound, [(coefficient, LabeledPolynomial, Randomness)])
+            for lc_label, terms in linear_combinations:
+                degree_bound, used = None, []
+                for coeff, label in terms:
+                    if label is None:                                          # LCTerm::One: not committed, used by the verifier directly
+                        continue
+                    if label not in label_map:
+                        raise KeyError(f"MissingPolynomial {{ label: {label} }}")
+                    cur, cur_rand = label_map[label]
+                    if cur.degree_bound is not None:
+                        if len(terms) != 1:
+                            raise ValueError(f"EquationHasDegreeBounds({lc_label})")
+                        assert int(coeff) % _R_MOD == 1, "Coefficient must be one for degree-bounded equations"
+                        degree_bound = cur.degree_bound
+                    used.append((int(coeff) % _R_MOD, cur, cur_rand))
+                lcs[lc_label] = (degree_bound, used)
+            by_point: dict = {}
+            for label, (point_name, point) in query_set:
+                by_point.setdefault(point_name, (point, set()))[1].add(label)
+            powers = ck.powers_of_beta_g
+            for point_name in sorted(by_point):
+                point, labels = by_point[point_name]
+                poly_terms, blind_terms = [], []
+                for label in sorted(labels):
+                    if label not in lcs:
+                        raise KeyError(f"MissingPolynomial {{ label: {label} }}")
+                    degree_bound, used = lcs[label]
+                    _check_bound(ck, label, max([p.polynomial.shape[0] for c, p, _r in used if c], default=0), degree_bound)
+                    ch = int(next(challenges)) % _R_MOD
+                    for c, p, r in used:
+                        c = c * ch % _R_MOD
+                        if c == 0:
+                            continue
+                        if p.polynomial.shape[0]:
+                            poly_terms.append((p.polynomial, _fr_int_to_mont(c)))
+                        if r.is_hiding():
+                            blind_terms.append((r.blinding_polynomial, _fr_int_to_mont(c)))
+                next(challenges)                                                   # `_randomizer`
+                n = max([t[0].shape[0] for t in poly_terms], default=0)
+                if n > powers.shape[0]:
+                    raise ValueError("check_degree_is_too_large")
+                blind = (max(t[0].shape[0] for t in blind_terms), blind_terms) if blind_terms else None
+                opened.append((k, _fr_int_to_mont(int(point) % _R_MOD), (n, poly_terms), blind))
+        if not opened:
+            return [[] for _ in items]
+        # kzg10::open (mod.rs:303-321) of every (item, point): combined polynomials, witnesses, random_v, then ONE commitment pass
+        hiding = [i for i, o in enumerate(opened) if o[3] is not None]
+        combined = device.fr_lincomb_terms([o[2] for o in opened] + [opened[i][3] for i in hiding])
+        witnesses = device.poly_divide_by_linear_batch([(p, o[1]) for p, o in zip(combined, opened)] +
+                                                       [(b, opened[i][1]) for b, i in zip(combined[len(opened):], hiding)])
+        random_vs = device.poly_evaluate_batch([(b, opened[i][1]) for b, i in zip(combined[len(opened):], hiding)])
+        hiding_witnesses = [None] * len(opened)
+        for j, i in enumerate(hiding):
+            hiding_witnesses[i] = witnesses[len(opened) + j]
+        powers = [items[o[0]][0].powers() for o in opened]
+        ws = device.sonic_commit_batch([p for p, _g in powers], witnesses[: len(opened)], [g for _p, g in powers] if hiding else None,
+                                       hiding_witnesses if hiding else None)
+        out = [[] for _ in items]
+        rv = dict(zip(hiding, random_vs))
+        for i, o in enumerate(opened):
+            out[o[0]].append((ws[i], rv[i].copy() if i in rv else None))
+        return out
 
 
 def check_combinations_scalars(linear_combinations: list, query_set: list, evaluations: dict, degree_bounds: dict, random_vs: list,

@@ -859,6 +859,11 @@ class BatchProver:
     sums, whatever the number of circuits and instances (launches grow only with the number of distinct domain sizes)."""
 
     def __init__(self, program: list):
+        self._setup(program)
+        BatchProver._load_many([self])
+
+    def _setup(self, program: list):
+        """the checks, the circuit order and the domains: everything before the first device pass"""
         if not program:
             raise ValueError("no circuits to prove")
         for k, (c, zs) in enumerate(program):
@@ -885,36 +890,47 @@ class BatchProver:
         self.max_constraint_domain = _largest(c.constraint_domain for c in cs)
         self.max_variable_domain = _largest(c.variable_domain for c in cs)
         self.max_non_zero_domain = _largest(c.max_non_zero_domain for c in cs)
-        # z_A, z_B, z_C of every instance (round_functions/mod.rs:128-152): one pass, each written into a zeroed |R|-row slot so that
-        # round 2 interpolates them without a per-instance copy
-        slots = [(i, j, m) for i, c in enumerate(cs) for j in range(self.batch[i]) for m in range(3)]
-        sizes = [cs[i].constraint_domain.size for i, _j, _m in slots]
-        self._zbuf = _zeros(sum(sizes), self.dev)
-        offs = np.concatenate([[0], np.cumsum(sizes)]).tolist()
-        outs = [self._zbuf[o: o + cs[i].num_constraints] for o, (i, _j, _m) in zip(offs, slots)]
-        self._zslots = list(zip(offs, sizes))
-        jobs = [(mat.row_ptr, mat.cols, mat.vals, self.z[i][j]) for i, j, m in slots for mat in ((cs[i].a, cs[i].b, cs[i].c)[m],)]
+        self.mask_poly = None
+
+    @staticmethod
+    def _load_many(provers: list):
+        """z_A, z_B, z_C of every instance of every prover (round_functions/mod.rs:128-152) in one mat-vec pass, each written into a
+        zeroed |R|-row slot of its prover's buffer so that round 2 interpolates them without a per-instance copy; x_poly of every
+        instance (state.rs:137-139) in one batched iNTT.  A bad matrix raises CudaError naming the circuit (and the prover, when
+        there are several)."""
+        jobs, outs, owners = [], [], []
+        for n, p in enumerate(provers):
+            cs = p.circuits
+            slots = [(i, j, m) for i, c in enumerate(cs) for j in range(p.batch[i]) for m in range(3)]
+            sizes = [cs[i].constraint_domain.size for i, _j, _m in slots]
+            p._zbuf = _zeros(sum(sizes), p.dev)
+            offs = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64).tolist()
+            p._zslots = list(zip(offs, sizes))
+            mine = [p._zbuf[o: o + cs[i].num_constraints] for o, (i, _j, _m) in zip(offs, slots)]
+            jobs += [(mat.row_ptr, mat.cols, mat.vals, p.z[i][j]) for i, j, m in slots for mat in ((cs[i].a, cs[i].b, cs[i].c)[m],)]
+            outs += mine
+            owners += [(n, slot) for slot in slots]
+            p.z_a, p.z_b, p.z_c = ([[None] * b for b in p.batch] for _ in range(3))
+            for (i, j, m), out in zip(slots, mine):
+                (p.z_a, p.z_b, p.z_c)[m][i][j] = out
         try:
             device.sparse_matvec_batch(jobs, outs)
         except CudaError as e:
             seg = getattr(e, "segment", None)
             if seg is None:
                 raise
-            i, _j, m = slots[seg]
-            raise CudaError(e.code, f"circuit {self.positions[i]}: matrix {'abc'[m]} has a column ≥ num_variables or a row_ptr that does not "
-                                    "run from 0 to nnz") from None
-        it = iter(outs)
-        self.z_a, self.z_b, self.z_c = ([[None] * b for b in self.batch] for _ in range(3))
-        for i, j, m in slots:
-            (self.z_a, self.z_b, self.z_c)[m][i][j] = next(it)
-        # x_poly (state.rs:137-139): the interpolations of every instance's public part in one batched iNTT
-        pubs = [self.z[i][j][: c.num_public] for i, c in enumerate(cs) for j in range(self.batch[i])]
+            n, (i, _j, m) = owners[seg]
+            job = f"job {n}: " if len(provers) > 1 else ""
+            raise CudaError(e.code, f"{job}circuit {provers[n].positions[i]}: matrix {'abc'[m]} has a column ≥ num_variables or a row_ptr "
+                                    "that does not run from 0 to nnz") from None
+        pubs = [z[: c.num_public] for p in provers for c, zs in zip(p.circuits, p.z) for z in zs]
         xbuf = torch.cat(pubs) if len(pubs) > 1 else pubs[0].clone()
-        offs = np.concatenate([[0], np.cumsum([p.shape[0] for p in pubs])]).tolist()
+        offs = np.concatenate([[0], np.cumsum([x.shape[0] for x in pubs])]).astype(np.int64).tolist()
         flat = [xbuf[a: b] for a, b in zip(offs, offs[1:])]
         device.ntt_batch_(flat, NTTDirection.Inverse, NTTType.Standard)
-        self.x_polys = self._per_circuit(flat)
-        self.mask_poly = None
+        it = iter(flat)
+        for p in provers:
+            p.x_polys = p._per_circuit([next(it) for _ in range(sum(p.batch))])
 
     def _per_circuit(self, flat: list) -> list:
         out, it = [], iter(flat)
@@ -981,36 +997,51 @@ class BatchProver:
 
     # ---- calculate_assignments (third.rs:207-234): z = w·v_I + x, one launch for every instance ----
     def assignments(self):
+        return BatchProver._assignments_many([self])[0]
+
+    @staticmethod
+    def _assignments_many(provers: list) -> list:
         jobs = []
-        for c, ws, xs in zip(self.circuits, self.w_polys, self.x_polys):
-            I = c.input_domain.size
-            for w, x in zip(ws, xs):
-                jobs.append((I + w.shape[0], [(x, _mont(1)), (w, _mont(-1)), (w, _mont(1), I)]))
-        self.z_polys = self._per_circuit(device.fr_lincomb_terms(jobs))
-        return self.z_polys
+        for p in provers:
+            for c, ws, xs in zip(p.circuits, p.w_polys, p.x_polys):
+                I = c.input_domain.size
+                for w, x in zip(ws, xs):
+                    jobs.append((I + w.shape[0], [(x, _mont(1)), (w, _mont(-1)), (w, _mont(1), I)]))
+        it = iter(device.fr_lincomb_terms(jobs))
+        for p in provers:
+            p.z_polys = p._per_circuit([next(it) for _ in range(sum(p.batch))])
+        return [p.z_polys for p in provers]
 
     # ---- round 2: h_0 (second.rs:76-142) ----
     def second_round(self, batch_combiners=None):
         """h_0 = Σ over circuits and instances of apply_randomized_selector(comb_inst·rowcheck, comb_circuit, R_max, R_i, false).  The
         rowcheck z_A·z_B − z_C has degree < 2|R_i| and z_C degree < |R_i|, so its quotient by v_{R_i} is the upper half of z_A·z_B:
         one batched iNTT, one batched product and one selector sum for the whole batch."""
-        combs = self._combiners(batch_combiners)
-        R = self.max_constraint_domain
-        evals = self._zbuf.clone()                                        # z_A, z_B of every instance, interpolated in place
-        ab = [evals[o: o + n] for k, (o, n) in enumerate(self._zslots) if k % 3 != 2]
-        device.ntt_batch_(ab, NTTDirection.Inverse, NTTType.Standard)
-        prods = device.polymul_batch(list(zip(ab[0::2], ab[1::2])))
-        terms, k = [], 0
-        for c, (cc, inst) in zip(self.circuits, combs):
-            n = c.constraint_domain.size
-            scale = cc * n % R_MOD * pow(R.size, -1, R_MOD) % R_MOD
-            for comb in inst:
-                p = prods[k]
-                k += 1
-                terms.append((p[n:], _mont(comb * scale)))
-        n_out = max(t[0].shape[0] for t in terms)
-        self.h_0 = device.fr_lincomb_terms([(n_out, terms)])[0]
-        return self.h_0
+        return BatchProver._second_round_many([self], [batch_combiners])[0]
+
+    @staticmethod
+    def _second_round_many(provers: list, batch_combiners: list) -> list:
+        """second_round of every prover (with its own combiners) in the same batched iNTT, product and selector-sum launch"""
+        combs = [p._combiners(bc) for p, bc in zip(provers, batch_combiners)]
+        abs_ = []
+        for p in provers:
+            evals = p._zbuf.clone()                                       # z_A, z_B of every instance, interpolated in place
+            abs_.append([evals[o: o + n] for k, (o, n) in enumerate(p._zslots) if k % 3 != 2])
+        device.ntt_batch_([t for ab in abs_ for t in ab], NTTDirection.Inverse, NTTType.Standard)
+        prods = iter(device.polymul_batch([pair for ab in abs_ for pair in zip(ab[0::2], ab[1::2])]))
+        jobs = []
+        for p, comb in zip(provers, combs):
+            R = p.max_constraint_domain
+            terms = []
+            for c, (cc, inst) in zip(p.circuits, comb):
+                n = c.constraint_domain.size
+                scale = cc * n % R_MOD * pow(R.size, -1, R_MOD) % R_MOD
+                for comb_inst in inst:
+                    terms.append((next(prods)[n:], _mont(comb_inst * scale)))
+            jobs.append((max(t[0].shape[0] for t in terms), terms))
+        for p, h_0 in zip(provers, device.fr_lincomb_terms(jobs)):
+            p.h_0 = h_0
+        return [p.h_0 for p in provers]
 
     # ---- evaluate_all_lagrange_coefficients (fft/domain.rs:258-292) on the device ----
     @staticmethod
@@ -1023,88 +1054,120 @@ class BatchProver:
         M(α, ·) of every transpose is one segmented mat-vec (α is shared: one Lagrange vector per distinct |R|), their interpolation
         one batched iNTT, the 3·Σ instances products M(α)·z one batched product; the sums and both selector sums are one launch and
         the sums reach the host in one copy."""
-        combs = self._combiners(batch_combiners)
-        cs, C = self.circuits, self.max_variable_domain
-        lag = {}
-        for c in cs:
-            if c.constraint_domain.size not in lag:
-                lag[c.constraint_domain.size] = self.lagrange_coefficients(c.constraint_domain, alpha, self.dev)
-        m_evals = device.sparse_matvec_batch([(t.row_ptr, t.cols, t.vals, lag[c.constraint_domain.size]) for c in cs for t in c.transposes])
-        device.ntt_batch_(m_evals, NTTDirection.Inverse, NTTType.Standard)
-        pairs, owners = [], []
-        for i, c in enumerate(cs):
-            for j, z_poly in enumerate(self.z_polys[i]):
-                for m in range(3):
-                    pairs.append((m_evals[3 * i + m], z_poly))
-                    owners.append((i, j, m))
-        prods = device.polymul_batch(pairs)
-        sums_buf = _zeros(len(prods), self.dev)
-        sum_jobs, h_terms, xg_terms = [], [], []
-        etas = (1, eta_b % R_MOD, eta_c % R_MOD)
-        for (i, j, m), z_m in zip(owners, prods):
-            n = cs[i].variable_domain.size
-            # Σ_{c ∈ C_i} z_m(c) = |C_i| · Σ_j coefficient_{j·|C_i|}
-            sum_jobs.append((1, [(z_m[k: k + 1], _mont(1)) for k in range(0, z_m.shape[0], n)]))
-            cc, inst = combs[i]
-            mult = cc * inst[j] % R_MOD * etas[m] % R_MOD * n % R_MOD * pow(C.size, -1, R_MOD) % R_MOD
-            assert z_m.shape[0] <= 2 * n
-            lo, hi = z_m[:n], z_m[n:]
-            h_terms.append((hi, _mont(mult)))
-            # the remainder lo + hi times v_{C_max} / v_{C_i}: |C_max| / |C_i| copies of it, |C_i| apart
-            xg_terms += [(lo, _mont(mult), 0, n, C.size // n), (hi, _mont(mult), 0, n, C.size // n)]
-        if self.mask_poly is not None:                                  # third.rs:207-213 (hiding mode)
-            h_mask, xg_mask = divide_by_vanishing(self.mask_poly, C)
-            h_terms.append((h_mask, _mont(1)))
-            xg_terms.append((xg_mask, _mont(1)))
-        n_h = max(t[0].shape[0] for t in h_terms)
-        n_xg = C.size
-        *_sums, self.h_1, xg_1 = device.fr_lincomb_terms(sum_jobs + [(n_h, h_terms), (n_xg, xg_terms)],
-                                                         [sums_buf[k: k + 1] for k in range(len(prods))] + [None, None])
-        self.g_1 = xg_1[1:]
-        host = device.fr_from_mont(sums_buf).cpu().numpy().view(np.uint64)
-        self.third_sums = [[[0, 0, 0] for _ in range(b)] for b in self.batch]
-        for (i, j, m), row in zip(owners, host):
-            n = cs[i].variable_domain.size
-            self.third_sums[i][j][m] = n * sum(int(v) << (64 * t) for t, v in enumerate(row)) % R_MOD
+        BatchProver._third_round_many([self], [(alpha, eta_b, eta_c)], [batch_combiners])
         return self.g_1, self.h_1
+
+    @staticmethod
+    def _third_round_many(provers: list, challenges: list, batch_combiners: list) -> None:
+        """third_round of every prover with its own (α, η_b, η_c) and combiners: one Lagrange vector per (prover, distinct |R|), then
+        the same mat-vec pass, iNTT, product, sum launch and copy for all of them"""
+        combs = [p._combiners(bc) for p, bc in zip(provers, batch_combiners)]
+        spmv, pairs, owners = [], [], []
+        for p, (alpha, _eb, _ec) in zip(provers, challenges):
+            lag = {}
+            for c in p.circuits:
+                if c.constraint_domain.size not in lag:
+                    lag[c.constraint_domain.size] = p.lagrange_coefficients(c.constraint_domain, alpha, p.dev)
+            spmv += [(t.row_ptr, t.cols, t.vals, lag[c.constraint_domain.size]) for c in p.circuits for t in c.transposes]
+        m_evals = device.sparse_matvec_batch(spmv)
+        device.ntt_batch_(m_evals, NTTDirection.Inverse, NTTType.Standard)
+        base = 0
+        for n, p in enumerate(provers):
+            for i, _c in enumerate(p.circuits):
+                for j, z_poly in enumerate(p.z_polys[i]):
+                    for m in range(3):
+                        pairs.append((m_evals[base + 3 * i + m], z_poly))
+                        owners.append((n, i, j, m))
+            base += 3 * len(p.circuits)
+        prods = device.polymul_batch(pairs)
+        sums_buf = _zeros(len(prods), provers[0].dev)
+        sum_jobs, h_terms, xg_terms = [], [[] for _ in provers], [[] for _ in provers]
+        for (n, i, j, m), z_m in zip(owners, prods):
+            p, (_alpha, eta_b, eta_c), C = provers[n], challenges[n], provers[n].max_variable_domain
+            nv = p.circuits[i].variable_domain.size
+            # Σ_{c ∈ C_i} z_m(c) = |C_i| · Σ_j coefficient_{j·|C_i|}
+            sum_jobs.append((1, [(z_m[k: k + 1], _mont(1)) for k in range(0, z_m.shape[0], nv)]))
+            cc, inst = combs[n][i]
+            etas = (1, eta_b % R_MOD, eta_c % R_MOD)
+            mult = cc * inst[j] % R_MOD * etas[m] % R_MOD * nv % R_MOD * pow(C.size, -1, R_MOD) % R_MOD
+            assert z_m.shape[0] <= 2 * nv
+            lo, hi = z_m[:nv], z_m[nv:]
+            h_terms[n].append((hi, _mont(mult)))
+            # the remainder lo + hi times v_{C_max} / v_{C_i}: |C_max| / |C_i| copies of it, |C_i| apart
+            xg_terms[n] += [(lo, _mont(mult), 0, nv, C.size // nv), (hi, _mont(mult), 0, nv, C.size // nv)]
+        for n, p in enumerate(provers):
+            if p.mask_poly is not None:                                   # third.rs:207-213 (hiding mode)
+                h_mask, xg_mask = divide_by_vanishing(p.mask_poly, p.max_variable_domain)
+                h_terms[n].append((h_mask, _mont(1)))
+                xg_terms[n].append((xg_mask, _mont(1)))
+        hx = [job for n, p in enumerate(provers)
+              for job in ((max(t[0].shape[0] for t in h_terms[n]), h_terms[n]), (p.max_variable_domain.size, xg_terms[n]))]
+        out = device.fr_lincomb_terms(sum_jobs + hx, [sums_buf[k: k + 1] for k in range(len(prods))] + [None] * len(hx))
+        for n, p in enumerate(provers):
+            p.h_1, xg_1 = out[len(sum_jobs) + 2 * n], out[len(sum_jobs) + 2 * n + 1]
+            p.g_1 = xg_1[1:]
+            p.third_sums = [[[0, 0, 0] for _ in range(b)] for b in p.batch]
+        host = device.fr_from_mont(sums_buf).cpu().numpy().view(np.uint64)
+        for (n, i, j, m), row in zip(owners, host):
+            nv = provers[n].circuits[i].variable_domain.size
+            provers[n].third_sums[i][j][m] = nv * sum(int(v) << (64 * t) for t, v in enumerate(row)) % R_MOD
 
     # ---- round 4: matrix sumchecks (fourth.rs:79-245) ----
     def fourth_round(self, alpha: int, beta: int):
         """per matrix of every circuit, with that circuit's v_{R_i}(α)·v_{C_i}(β) and |R_i|·|C_i|; the selector goes from K_matrix to the
         global K_max.  The evaluations of all 3K matrices are three launches, their 9K interpolations one batched iNTT, the products
         b·f one batched product, the 3K quotients one launch; the 3K sums f[0] reach the host in one copy."""
-        cs, Kmax = self.circuits, self.max_non_zero_domain
-        jobs = []
-        for c in cs:
-            Rd, V = c.constraint_domain, c.variable_domain
-            v_rc = _vanish(Rd, alpha) * _vanish(V, beta) % R_MOD
-            rc = Rd.size * V.size % R_MOD
-            scale = v_rc * pow(Rd.size, -1, R_MOD) % R_MOD * pow(V.size, -1, R_MOD) % R_MOD
-            for arith in c.ariths:
-                jobs.append((arith.row, arith.col, arith.row_col_val, _mont(v_rc), _mont(rc), _mont(scale)))
-        evals = device.varuna_round4_evals(jobs, _mont(alpha), _mont(beta))
+        return BatchProver._fourth_round_many([self], [(alpha, beta)])[0]
+
+    @staticmethod
+    def _fourth_round_many(provers: list, challenges: list) -> list:
+        """fourth_round of every prover with its own (α, β): the matrices of all of them in the same launches, α and β per segment"""
+        jobs, doms, kmax = [], [], []
+        for p, (alpha, beta) in zip(provers, challenges):
+            for c in p.circuits:
+                Rd, V = c.constraint_domain, c.variable_domain
+                v_rc = _vanish(Rd, alpha) * _vanish(V, beta) % R_MOD
+                rc = Rd.size * V.size % R_MOD
+                scale = v_rc * pow(Rd.size, -1, R_MOD) % R_MOD * pow(V.size, -1, R_MOD) % R_MOD
+                for arith in c.ariths:
+                    jobs.append((arith.row, arith.col, arith.row_col_val, _mont(v_rc), _mont(rc), _mont(scale), _mont(alpha), _mont(beta)))
+                    doms.append(arith.domain)
+                    kmax.append(p.max_non_zero_domain.size)
+        evals = device.varuna_round4_evals_batch(jobs)
         device.ntt_batch_([t for trio in evals for t in trio], NTTDirection.Inverse, NTTType.Standard)
         bf = device.polymul_batch([(b, f) for _a, b, f in evals])
-        doms = [a.domain for c in cs for a in c.ariths]
-        lhs = device.fr_lincomb_terms([(d.size, [(p[d.size:], _mont(-d.size * pow(Kmax.size, -1, R_MOD)))]) for p, d in zip(bf, doms)])
+        lhs = device.fr_lincomb_terms([(d.size, [(q[d.size:], _mont(-d.size * pow(km, -1, R_MOD)))]) for q, d, km in zip(bf, doms, kmax)])
         f0 = torch.stack([f[0] for _a, _b, f in evals]).cpu().numpy().view(np.uint64)
-        self.gs, self.lhs, self.fourth_sums, self.a_polys, self.b_polys = [], [], [], [], []
-        for i in range(len(cs)):
-            trio = evals[3 * i: 3 * i + 3]
-            self.gs.append([f[1:] for _a, _b, f in trio])
-            self.lhs.append(lhs[3 * i: 3 * i + 3])
-            self.fourth_sums.append([_fr_mont_to_int(f0[3 * i + m]) for m in range(3)])
-            self.a_polys.append([a for a, _b, _f in trio])
-            self.b_polys.append([b for _a, b, _f in trio])
-        return self.gs
+        base = 0
+        for p in provers:
+            p.gs, p.lhs, p.fourth_sums, p.a_polys, p.b_polys = [], [], [], [], []
+            for i in range(len(p.circuits)):
+                at = base + 3 * i
+                trio = evals[at: at + 3]
+                p.gs.append([f[1:] for _a, _b, f in trio])
+                p.lhs.append(lhs[at: at + 3])
+                p.fourth_sums.append([_fr_mont_to_int(f0[at + m]) for m in range(3)])
+                p.a_polys.append([a for a, _b, _f in trio])
+                p.b_polys.append([b for _a, b, _f in trio])
+            base += 3 * len(p.circuits)
+        return [p.gs for p in provers]
 
     # ---- round 5 (fifth.rs:43-67): h_2 = Σ δ·lhs over all 3K matrices, one launch ----
     def fifth_round(self, deltas):
-        if len(deltas) != len(self.circuits) or any(len(d) != 3 for d in deltas):
-            raise ValueError(f"one (δ_a, δ_b, δ_c) per circuit: {len(self.circuits)} circuits")
-        terms = [(lhs, _mont(int(d) % R_MOD)) for ds, ls in zip(deltas, self.lhs) for d, lhs in zip(ds, ls)]
-        self.h_2 = device.fr_lincomb_terms([(max(t[0].shape[0] for t in terms), terms)])[0]
-        return self.h_2
+        return BatchProver._fifth_round_many([self], [deltas])[0]
+
+    @staticmethod
+    def _fifth_round_many(provers: list, deltas: list) -> list:
+        for p, ds in zip(provers, deltas):
+            if len(ds) != len(p.circuits) or any(len(d) != 3 for d in ds):
+                raise ValueError(f"one (δ_a, δ_b, δ_c) per circuit: {len(p.circuits)} circuits")
+        jobs = []
+        for p, ds in zip(provers, deltas):
+            terms = [(lhs, _mont(int(d) % R_MOD)) for dd, ls in zip(ds, p.lhs) for d, lhs in zip(dd, ls)]
+            jobs.append((max(t[0].shape[0] for t in terms), terms))
+        for p, h_2 in zip(provers, device.fr_lincomb_terms(jobs)):
+            p.h_2 = h_2
+        return [p.h_2 for p in provers]
 
     # ---- labels, oracles, linear combinations ----
     def _labels(self):
@@ -1169,16 +1232,35 @@ class BatchProver:
     def _eval(poly: torch.Tensor, point: int) -> int:
         return _fr_mont_to_int(device.poly_evaluate(poly.contiguous(), _mont(point))) if poly.shape[0] else 0
 
+    def _eval_points(self, beta: int, gamma: int) -> list:
+        """the evaluations the linear combinations and the proof need, as (polynomial, point): g_1(β), every g_M(γ), every x(β)"""
+        return ([(self.g_1, beta)] + [(g, gamma) for gs in self.gs for g in gs] +
+                [(x, beta) for xs in self.x_polys for x in xs])
+
+    def _take_evals(self, vals: list) -> tuple:
+        """_eval_points' values → (g_1(β), per circuit [g_a(γ), g_b(γ), g_c(γ)], per circuit per instance x(β))"""
+        it = iter(vals)
+        g_1 = next(it)
+        gs = [[next(it) for _ in range(3)] for _ in self.gs]
+        return g_1, gs, [[next(it) for _ in xs] for xs in self.x_polys]
+
+    @staticmethod
+    def _evals_many(provers: list, points: list) -> list:
+        """_take_evals of every prover at its (β, γ) from one device.poly_evaluate_batch pass"""
+        jobs = [p._eval_points(beta, gamma) for p, (beta, gamma) in zip(provers, points)]
+        host = device.poly_evaluate_batch([(poly.contiguous(), _mont(x)) for js in jobs for poly, x in js])
+        vals = iter(_fr_mont_to_int(row) for row in host)
+        return [p._take_evals([next(vals) for _ in js]) for p, js in zip(provers, jobs)]
+
     def linear_combinations(self, alpha, eta_b, eta_c, beta, deltas, gamma, batch_combiners=None, label=None):
         """AHPForR1CS::construct_linear_combinations (ahp/ahp.rs:172-389) on the prover's side and the query set for K circuits
-        (linear_combinations below), with the evaluations it needs (g_1(β), g_M(γ), x(β)) from device Horner passes"""
+        (linear_combinations below), with the evaluations it needs (g_1(β), g_M(γ), x(β)) from one device Horner pass"""
         if len(deltas) != len(self.circuits) or any(len(d) != 3 for d in deltas):
             raise ValueError(f"one (δ_a, δ_b, δ_c) per circuit: {len(self.circuits)} circuits")
+        g_1_at_beta, g_at_gamma, x_at_beta = BatchProver._evals_many([self], [(beta, gamma)])[0]
         return linear_combinations(self.circuits, self._combiners(batch_combiners), self.third_sums, self.fourth_sums,
-                                   (alpha, eta_b, eta_c, beta, deltas, gamma), self._eval(self.g_1, beta),
-                                   [[self._eval(g, gamma) for g in gs] for gs in self.gs],
-                                   [[self._eval(x, beta) for x in xs] for xs in self.x_polys], label or self._labels(),
-                                   self.mask_poly is not None)
+                                   (alpha, eta_b, eta_c, beta, deltas, gamma), g_1_at_beta, g_at_gamma, x_at_beta,
+                                   label or self._labels(), self.mask_poly is not None)
 
 
 def linear_combinations(circuits: list, combs: list, third_sums: list, fourth_sums: list, challenges: tuple, g_1_at_beta: int,
@@ -1401,31 +1483,53 @@ class TranscriptOps:
 class Transcript(TranscriptOps):
     """The prover's PoseidonSponge<Fq, 2, 1>, its state kept in HBM between calls as one state record
     (device.poseidon_transcripts with `state`).  Absorbs only queue operations; `squeeze` runs everything queued and its squeezes
-    in one device call, so a round costs one call.  `calls` and `permutations` count what the sponge has run."""
+    in one device call, so a round costs one call.  `calls` and `permutations` count what the sponge has run.  `state`, when given,
+    is the record to use (a row of a tensor whose rows are the records of several transcripts that squeeze together,
+    squeeze_many)."""
 
-    def __init__(self, dev):
+    def __init__(self, dev, state: torch.Tensor | None = None):
         super().__init__()
         self.dev = torch.device(dev)
-        self.state = poseidon.fresh_states(poseidon.FIELD_FQ, 1, self.dev)
+        self.state = poseidon.fresh_states(poseidon.FIELD_FQ, 1, self.dev) if state is None else state
         self.calls = 0
 
     def squeeze(self, counts: list, short: bool = False) -> list:
         """one squeeze_nonnative_field_elements(n) call (squeeze_short_… when `short`) per entry of `counts`, after everything
         queued, in one device call → [[canonical Fr] per call]"""
-        self.queue_squeeze(counts, short)
-        off = self._nout
-        ops = torch.from_numpy(np.array(self._ops, dtype=np.int32).reshape(-1, 3)).to(self.dev)
-        start = torch.tensor([0, len(self._ops)], dtype=torch.int32, device=self.dev)
-        _out, fr = device.poseidon_transcripts(poseidon.FIELD_FQ, ops, start, torch.from_numpy(self.inputs().view(np.int64)).to(self.dev),
-                                               0, off, self.state)
-        self.calls += 1
-        self._ops, self._inputs, self._nin, self._nout = [], [], 0, 0
-        vals = [_fr_mont_to_int(row) for row in fr.cpu().numpy().view(np.uint64)] if off else []
-        out, k = [], 0
-        for n in counts:
-            out.append(vals[k: k + n])
+        return squeeze_many([self], [counts], self.state, short)[0]
+
+
+def squeeze_many(transcripts: list, counts: list, states: torch.Tensor, short: bool = False) -> list:
+    """Transcript.squeeze of every transcript with its own `counts`, all of them as transcripts of ONE device.poseidon_transcripts
+    call.  `states`: the state records of the transcripts, in order, as the rows of one tensor (each transcript's `state` a view of
+    its row) → per transcript [[canonical Fr] per call].  A malformed operation or record raises CudaError whose .transcript is the
+    index of the lowest such transcript in `transcripts`."""
+    ops_all, starts, inputs, nin, nfr, offs = [], [0], [], 0, 0, []
+    for t, cs in zip(transcripts, counts):
+        t.queue_squeeze(cs, short)
+        ops = np.array(t._ops, dtype=np.int64).reshape(-1, 3)
+        ops[:, 2] += np.where(ops[:, 0] == poseidon.OP_ABSORB, nin, nfr)
+        ops_all.append(ops)
+        starts.append(starts[-1] + ops.shape[0])
+        inputs.append(t.inputs())
+        offs.append(nfr)
+        nin += t._nin
+        nfr += t._nout
+    dev = transcripts[0].dev
+    _out, fr = device.poseidon_transcripts(poseidon.FIELD_FQ, torch.from_numpy(np.concatenate(ops_all).astype(np.int32)).to(dev),
+                                           torch.tensor(starts, dtype=torch.int32, device=dev),
+                                           torch.from_numpy(np.concatenate(inputs).view(np.int64)).to(dev), 0, nfr, states)
+    vals = [_fr_mont_to_int(row) for row in fr.cpu().numpy().view(np.uint64)] if nfr else []
+    out = []
+    for t, cs, off in zip(transcripts, counts, offs):
+        t.calls += 1
+        t._ops, t._inputs, t._nin, t._nout = [], [], 0, 0
+        mine, k = [], off
+        for n in cs:
+            mine.append(vals[k: k + n])
             k += n
-        return out
+        out.append(mine)
+    return out
 
 
 @dataclass
@@ -1522,12 +1626,6 @@ def _union_committer_key(cks: list):
                         max_degree)
 
 
-def _nonzero_vanishing(domain: EvaluationDomain, x: int, name: str):
-    """the verifier's check that v_domain(x) ≠ 0 (verifier.rs:151, 165, 208)"""
-    if _vanish(domain, x) == 0:
-        raise ValueError(f"the vanishing polynomial of the largest domain is zero at {name}")
-
-
 def _public_inputs(prover: "BatchProver") -> list:
     """every instance's padded public input as canonical integers: per circuit (id order), per instance"""
     out = []
@@ -1540,98 +1638,7 @@ def _public_inputs(prover: "BatchProver") -> list:
 
 def _prove_batch(pks_to_assignments: list, zk: bool = False, rng=None):
     """prove_batch (below) → (Proof, challenges, transcript): challenges is a dict of everything the transcript yielded"""
-    from .sonic_pc import LabeledPolynomial, Randomness, SonicKZG10
-    if not pks_to_assignments:
-        raise ValueError("EmptyBatch: no circuits to prove")
-    if zk and rng is None:
-        rng = random.SystemRandom()
-    prover = BatchProver([(pk.circuit, list(zs)) for pk, zs in pks_to_assignments])
-    pks = [pks_to_assignments[k][0] for k in prover.positions]
-    K, dev = len(pks), prover.dev
-    ck = _union_committer_key([pk.committer_key for pk in pks])
-    rand_fr = lambda n: [rng.randrange(R_MOD) for _ in range(n)]          # noqa: E731
-
-    # init_sponge (varuna.rs:136-153)
-    transcript = Transcript(dev)
-    _init_sponge(transcript, prover.batch, _public_inputs(prover), [pk.circuit_verifying_key.circuit_commitments for pk in pks])
-
-    def commit(labeled):
-        blind = [None if lp.hiding_bound is None else
-                 torch.from_numpy(np.array([_mont(v) for v in rand_fr(lp.hiding_bound + 2)], dtype=np.uint64).view(np.int64)).to(dev)
-                 for lp in labeled]
-        comms, rands = SonicKZG10.commit(ck, labeled, blind)
-        return list(comms), list(rands)
-
-    label = prover._labels()
-    rounds = {}
-
-    def round_commit(r):
-        rounds[r] = prover.labeled_oracles(zk, label, rounds=(r,))[r]
-        return commit(rounds[r])
-
-    # round 1
-    if zk:
-        prover.set_mask_poly(rand_fr(4), rand_fr(6))
-    prover.first_round()
-    prover.assignments()
-    c1, r1 = round_commit(1)
-    transcript.absorb_commitments(np.stack(c1))
-    elems = transcript.squeeze([b - 1 + (1 if i else 0) for i, b in enumerate(prover.batch)])
-    combs = [(e[b - 1] if i else 1, [1] + e[: b - 1]) for i, (b, e) in enumerate(zip(prover.batch, elems))]
-    # round 2
-    prover.second_round(combs)
-    c2, r2 = round_commit(2)
-    transcript.absorb_commitments(np.stack(c2))
-    alpha, eta_b, eta_c = transcript.squeeze([3])[0]
-    _nonzero_vanishing(prover.max_constraint_domain, alpha, "α")
-    # round 3
-    prover.third_round(alpha, eta_b, eta_c, combs)
-    c3, r3 = round_commit(3)
-    transcript.absorb_commitments(np.stack(c3))
-    for sums in prover.third_sums:
-        for s in sums:
-            transcript.absorb_nonnative(s)
-    beta = transcript.squeeze([1])[0][0]
-    _nonzero_vanishing(prover.max_variable_domain, beta, "β")
-    # round 4
-    prover.fourth_round(alpha, beta)
-    c4, r4 = round_commit(4)
-    transcript.absorb_commitments(np.stack(c4))
-    for s in prover.fourth_sums:
-        transcript.absorb_nonnative(s)
-    d = transcript.squeeze([2] + [3] * (K - 1))
-    deltas = [[1] + d[0]] + d[1:]
-    # round 5
-    prover.fifth_round(deltas)
-    c5, r5 = round_commit(5)
-    transcript.absorb_commitments(np.stack(c5))
-    gamma = transcript.squeeze([1])[0][0]
-    _nonzero_vanishing(prover.max_non_zero_domain, gamma, "γ")
-
-    lcs, query_set = prover.linear_combinations(alpha, eta_b, eta_c, beta, deltas, gamma, combs, label)
-    evaluations = Evaluations(BatchProver._eval(prover.g_1, beta), *([BatchProver._eval(gs[m], gamma) for gs in prover.gs] for m in range(3)))
-    transcript.absorb_nonnative(evaluations.to_field_elements())
-    # open_combinations: per point (by name), one short challenge per linear combination opened there, then `_randomizer`
-    per_point = {}
-    for _lc, (point_name, _x) in query_set:
-        per_point[point_name] = per_point.get(point_name, 0) + 1
-    opening = [x for [x] in transcript.squeeze([1] * sum(n + 1 for n in per_point.values()), short=True)]
-    polys = prover.polynomials(label)
-    ab = [LabeledPolynomial(k, v, None, None) for k, v in polys.items() if "_a_poly_" in k or "_b_poly_" in k]
-    labeled = ab + [lp for r in sorted(rounds) for lp in rounds[r]]
-    rands = [Randomness() for _ in ab] + r1 + r2 + r3 + r4 + r5
-    pc_proof = SonicKZG10.open_combinations(ck, lcs, labeled, rands, query_set, iter(opening))
-
-    nw = sum(prover.batch)
-    gs = [c4[3 * i: 3 * i + 3] for i in range(K)]
-    commitments = Commitments(c1[:nw], c1[nw] if zk else None, c2[0], c3[0], c3[1], [g[0] for g in gs], [g[1] for g in gs],
-                              [g[2] for g in gs], c5[0])
-    proof = Proof(list(prover.batch), commitments, evaluations, [[list(s) for s in sums] for sums in prover.third_sums],
-                  [list(s) for s in prover.fourth_sums], pc_proof)
-    proof.check_batch_sizes()
-    challenges = {"batch_combiners": combs, "alpha": alpha, "eta_b": eta_b, "eta_c": eta_c, "beta": beta, "deltas": deltas,
-                  "gamma": gamma, "opening": opening}
-    return proof, challenges, transcript
+    return _prove_batch_many([pks_to_assignments], zk, None if rng is None else [rng])[0]
 
 
 def prove_batch(pks_to_assignments: list, zk: bool = False, rng=None) -> Proof:
@@ -1649,8 +1656,195 @@ def prove_batch(pks_to_assignments: list, zk: bool = False, rng=None) -> Proof:
     The committer key is the union of the proving keys' keys.  In the hiding mode (zk) the mask polynomial (4 then 6 coefficients)
     and each hiding commitment's blinding polynomial (3 coefficients, in commitment order) are drawn from `rng` (anything with
     randrange; a SystemRandom when None).  That stream cannot equal the reference's ChaCha stream, so a hiding proof is valid but not
-    the reference's bytes; a non-hiding proof is deterministic."""
+    the reference's bytes; a non-hiding proof is deterministic.  This is prove_batch_many with one job."""
     return _prove_batch(pks_to_assignments, zk, rng)[0]
+
+
+def prove_batch_many(jobs: list, zk: bool = False, rngs: list | None = None, stats: dict | None = None) -> list:
+    """prove_batch of every job in `jobs` (each a pks_to_assignments list) in one call → one Proof per job, in input order.  Proof k
+    is byte for byte prove_batch(jobs[k]) when not hiding, and prove_batch(jobs[k], True, rngs[k]) in the hiding mode: job k draws
+    from its own rng (`rngs`: one per job, or None for a SystemRandom each) in prove_batch's order, the mask and then the blindings
+    in commitment order.  The jobs run through the rounds in lockstep and share every device call of a round:
+        transcript     the queued operations of every job's sponge as transcripts of one device.poseidon_transcripts call (their
+                       state records rows of one tensor), six calls in all
+        rounds         each segmented pass BatchProver makes for one job (mat-vecs, batched NTTs and products, linear combinations,
+                       round 4 with each job's α and β) over the segments of all jobs; the Lagrange vectors at α stay one call per
+                       (job, |R|), round 1's per-instance work stays per instance
+        commitments    each round's polynomials of every job in one device.sonic_commit_batch pass (SonicKZG10.commit_many)
+        evaluations    g_1(β), every g_M(γ) and every x(β) of every job in one device.poly_evaluate_batch pass
+        openings       every job's linear combinations in one pass (SonicKZG10.open_combinations_many)
+    Every job's round polynomials are resident at once: a caller whose jobs do not fit in device memory splits the call.
+    ValueError, naming the lowest job at fault, for an empty `jobs`, an empty job, an instance that does not match its index, jobs on
+    different devices, committer keys of different SRSs, and a vanishing polynomial that is zero at α, β or γ; nothing is returned
+    then.  A transcript's CudaError names the job.  `stats`, when given, receives the seconds of each stage ("transcript", "rounds",
+    "commitments", "openings", "host" for the rest) and the counts "transcript_calls" and "commitment_passes"."""
+    return [proof for proof, _ch, _t in _prove_batch_many(jobs, zk, rngs, stats)]
+
+
+def _prove_batch_many(jobs: list, zk: bool = False, rngs: list | None = None, stats: dict | None = None) -> list:
+    """prove_batch_many → [(Proof, challenges, transcript)] per job"""
+    import time
+    from .sonic_pc import LabeledPolynomial, Randomness, SonicKZG10
+    clock = time.perf_counter
+    t_start = clock()
+    spent = {"transcript": 0.0, "rounds": 0.0, "commitments": 0.0, "openings": 0.0}
+    passes = [0]
+    if not jobs:
+        raise ValueError("EmptyBatch: no jobs to prove")
+    P = len(jobs)
+    if zk:
+        rngs = [random.SystemRandom() for _ in jobs] if rngs is None else list(rngs)
+        if len(rngs) != P:
+            raise ValueError(f"{len(rngs)} rngs for {P} jobs")
+    provers, cks, pks = [], [], []
+    for k, job in enumerate(jobs):
+        try:
+            if not job:
+                raise ValueError("EmptyBatch: no circuits to prove")
+            p = BatchProver.__new__(BatchProver)
+            p._setup([(pk.circuit, list(zs)) for pk, zs in job])
+            if k and p.dev != provers[0].dev:
+                raise ValueError(f"the job is on {p.dev}, job 0 on {provers[0].dev}: every job must be on one device")
+            pks.append([job[i][0] for i in p.positions])
+            cks.append(_union_committer_key([pk.committer_key for pk in pks[-1]]))
+        except ValueError as e:
+            raise ValueError(f"job {k}: {e}") from None
+        provers.append(p)
+    dev = provers[0].dev
+
+    def timed(stage, fn, *args):
+        t = clock()
+        out = fn(*args)
+        if stats is not None and stage == "rounds":
+            torch.cuda.synchronize(dev)
+        spent[stage] += clock() - t
+        return out
+
+    def rand_fr(k, n):
+        return [rngs[k].randrange(R_MOD) for _ in range(n)]
+
+    timed("rounds", BatchProver._load_many, provers)
+    # init_sponge (varuna.rs:136-153): one state record per job, rows of one tensor
+    states = poseidon.fresh_states(poseidon.FIELD_FQ, P, dev)
+    ts = [Transcript(dev, states[k: k + 1]) for k in range(P)]
+    for t, p, pk in zip(ts, provers, pks):
+        _init_sponge(t, p.batch, _public_inputs(p), [x.circuit_verifying_key.circuit_commitments for x in pk])
+
+    def squeeze(counts, short=False):
+        try:
+            return timed("transcript", squeeze_many, ts, counts, states, short)
+        except CudaError as e:
+            if getattr(e, "transcript", None) is None:
+                raise
+            err = CudaError(e.code, f"job {e.transcript}: its transcript's operations or state record are malformed")
+            err.job = e.transcript
+            raise err from None
+
+    def check_vanishing(points, domains, name):
+        for k, (x, d) in enumerate(zip(points, domains)):
+            if _vanish(d, x) == 0:
+                raise ValueError(f"job {k}: the vanishing polynomial of the largest domain is zero at {name}")
+
+    labels = [p._labels() for p in provers]
+    rounds, rands, comms = [{} for _ in provers], [{} for _ in provers], [{} for _ in provers]
+
+    def round_commit(r):
+        items = []
+        for k, p in enumerate(provers):
+            rounds[k][r] = p.labeled_oracles(zk, labels[k], rounds=(r,))[r]
+            blind = [None if lp.hiding_bound is None else
+                     torch.from_numpy(np.array([_mont(v) for v in rand_fr(k, lp.hiding_bound + 2)], dtype=np.uint64).view(np.int64)).to(dev)
+                     for lp in rounds[k][r]]
+            items.append((cks[k], rounds[k][r], blind))
+        passes[0] += 1
+        for k, (c, rr) in enumerate(timed("commitments", SonicKZG10.commit_many, items)):
+            comms[k][r], rands[k][r] = list(c), list(rr)
+            ts[k].absorb_commitments(np.stack(comms[k][r]))
+
+    # round 1
+    if zk:
+        for k, p in enumerate(provers):
+            p.set_mask_poly(rand_fr(k, 4), rand_fr(k, 6))
+    for p in provers:
+        timed("rounds", p.first_round)
+    timed("rounds", BatchProver._assignments_many, provers)
+    round_commit(1)
+    elems = squeeze([[b - 1 + (1 if i else 0) for i, b in enumerate(p.batch)] for p in provers])
+    combs = [[(e[b - 1] if i else 1, [1] + e[: b - 1]) for i, (b, e) in enumerate(zip(p.batch, el))] for p, el in zip(provers, elems)]
+    # round 2
+    timed("rounds", BatchProver._second_round_many, provers, combs)
+    round_commit(2)
+    abc = [o[0] for o in squeeze([[3]] * P)]
+    check_vanishing([x[0] for x in abc], [p.max_constraint_domain for p in provers], "α")
+    # round 3
+    timed("rounds", BatchProver._third_round_many, provers, abc, combs)
+    round_commit(3)
+    for t, p in zip(ts, provers):
+        for sums in p.third_sums:
+            for s in sums:
+                t.absorb_nonnative(s)
+    betas = [o[0][0] for o in squeeze([[1]] * P)]
+    check_vanishing(betas, [p.max_variable_domain for p in provers], "β")
+    # round 4
+    timed("rounds", BatchProver._fourth_round_many, provers, [(x[0], b) for x, b in zip(abc, betas)])
+    round_commit(4)
+    for t, p in zip(ts, provers):
+        for s in p.fourth_sums:
+            t.absorb_nonnative(s)
+    deltas = [[[1] + d[0]] + d[1:] for d in squeeze([[2] + [3] * (len(p.circuits) - 1) for p in provers])]
+    # round 5
+    timed("rounds", BatchProver._fifth_round_many, provers, deltas)
+    round_commit(5)
+    gammas = [o[0][0] for o in squeeze([[1]] * P)]
+    check_vanishing(gammas, [p.max_non_zero_domain for p in provers], "γ")
+
+    # the evaluations of every job in one pass, then the linear combinations and the openings
+    evals = timed("openings", BatchProver._evals_many, provers, list(zip(betas, gammas)))
+    lcs, evaluations, per_point = [], [], []
+    for k, p in enumerate(provers):
+        (alpha, eta_b, eta_c), beta, gamma = abc[k], betas[k], gammas[k]
+        g_1_at_beta, g_at_gamma, x_at_beta = evals[k]
+        lcs.append(linear_combinations(p.circuits, p._combiners(combs[k]), p.third_sums, p.fourth_sums,
+                                       (alpha, eta_b, eta_c, beta, deltas[k], gamma), g_1_at_beta, g_at_gamma, x_at_beta, labels[k],
+                                       p.mask_poly is not None))
+        evaluations.append(Evaluations(g_1_at_beta, *([g[m] for g in g_at_gamma] for m in range(3))))
+        ts[k].absorb_nonnative(evaluations[k].to_field_elements())
+        # open_combinations: per point (by name), one short challenge per linear combination opened there, then `_randomizer`
+        count = {}
+        for _lc, (point_name, _x) in lcs[k][1]:
+            count[point_name] = count.get(point_name, 0) + 1
+        per_point.append(sum(n + 1 for n in count.values()))
+    opening = [[x for [x] in o] for o in squeeze([[1] * n for n in per_point], short=True)]
+    items = []
+    for k, p in enumerate(provers):
+        polys = p.polynomials(labels[k])
+        ab = [LabeledPolynomial(key, v, None, None) for key, v in polys.items() if "_a_poly_" in key or "_b_poly_" in key]
+        labeled = ab + [lp for r in sorted(rounds[k]) for lp in rounds[k][r]]
+        rr = [Randomness() for _ in ab] + [x for r in sorted(rands[k]) for x in rands[k][r]]
+        items.append((cks[k], lcs[k][0], labeled, rr, lcs[k][1], iter(opening[k])))
+    passes[0] += 1
+    pc_proofs = timed("openings", SonicKZG10.open_combinations_many, items)
+
+    out = []
+    for k, p in enumerate(provers):
+        K, c = len(p.circuits), comms[k]
+        nw = sum(p.batch)
+        gs = [c[4][3 * i: 3 * i + 3] for i in range(K)]
+        commitments = Commitments(c[1][:nw], c[1][nw] if zk else None, c[2][0], c[3][0], c[3][1], [g[0] for g in gs], [g[1] for g in gs],
+                                  [g[2] for g in gs], c[5][0])
+        proof = Proof(list(p.batch), commitments, evaluations[k], [[list(s) for s in sums] for sums in p.third_sums],
+                      [list(s) for s in p.fourth_sums], pc_proofs[k])
+        proof.check_batch_sizes()
+        alpha, eta_b, eta_c = abc[k]
+        challenges = {"batch_combiners": combs[k], "alpha": alpha, "eta_b": eta_b, "eta_c": eta_c, "beta": betas[k], "deltas": deltas[k],
+                      "gamma": gammas[k], "opening": opening[k]}
+        out.append((proof, challenges, ts[k]))
+    if stats is not None:
+        stats.update(spent)
+        stats["host"] = clock() - t_start - sum(spent.values())
+        stats["transcript_calls"] = ts[0].calls
+        stats["commitment_passes"] = passes[0]
+    return out
 
 
 # ---- verify_batch: the verifier (varuna.rs:625-933; sonic_pc/mod.rs:344-411, 477-544, 582-677) ----
