@@ -613,6 +613,35 @@ SNARKVM_API int snarkvm_b200_g1_deserialize_device(void* d_points, int32_t* d_st
  * synchronisation. */
 SNARKVM_API int snarkvm_b200_g1_serialize_device(void* d_bytes, const void* d_points, size_t n, int form, void* stream);
 
+/* G2 points taken from outside.  These three entry points report the SNARKVM_B200_G1_* status values above: the values are shared
+ * by both groups, and there is no G2 enum.
+ *
+ * Validation (Valid for Affine<G2> of the reference: is_on_curve and [r]·P = O, curves/src/bls12_377/g2.rs:120-124).  d_points
+ * holds n Affine<G2> images (x.c0, x.c1, y.c0, y.c1 Montgomery Fq, infinity flag; stride ≥ 200, a multiple of 8, 8-byte aligned);
+ * d_status[i] (device int32) receives point i's status: VALID (the point at infinity included), NOT_CANONICAL (a coordinate image
+ * not below q), NOT_ON_CURVE (y² ≠ x³ + B', B' = (0, −1/5)) or NOT_IN_SUBGROUP ([r]·P ≠ O, r the order of G1 and G2), the first
+ * test that fails.  One launch, one thread per point, no synchronisation. */
+SNARKVM_API int snarkvm_b200_g2_validate_device(int32_t* d_status, const void* d_points, size_t n, size_t stride, void* stream);
+/* G2 points from their byte forms (CanonicalDeserialize of Affine<G2>: curves/src/templates/macros.rs:118-144, Fp2 of
+ * fields/src/fp2.rs:450-457).  d_bytes holds n points of 96 bytes (compressed != 0: x.c0, x.c1, 48 bytes little-endian each, bit 7
+ * of the last byte PositiveY, bit 6 Infinity) or 192 bytes (compressed = 0: x.c0, x.c1, y.c0, y.c1, the flags on y.c1), no
+ * alignment needed.  d_points (8-byte aligned, 200-byte stride) receives each point's Affine<G2> image and d_status[i] (device
+ * int32, 4-byte aligned) its status.  The coordinates are read in order: bit 7 of the last byte of a coordinate other than the
+ * last gives BAD_FLAGS (EmptyFlags), as do both flag bits of the last one; then a value not below q (flags masked) gives
+ * NOT_CANONICAL.  A compressed x whose x³ + B' has no square root in Fq2 gives NOT_ON_CURVE.  Otherwise VALID, and with `validate`
+ * the status of Affine::check as snarkvm_b200_g2_validate_device reports it.  An infinity decodes to Affine::zero() (0, 1,
+ * infinity) whatever the coordinates below q were.  A compressed point's y is the root of x³ + B' that is the larger of y, −y in
+ * the reference's order on Fp2 (c1 compared first, then c0, as canonical integers) when PositiveY is set, the smaller otherwise.
+ * An uncompressed point is not tested against the curve unless `validate`.  Bytes that decode to no point leave an all-zero image.
+ * One launch, one thread per point, no synchronisation. */
+SNARKVM_API int snarkvm_b200_g2_deserialize_device(void* d_points, int32_t* d_status, const void* d_bytes, size_t n, int compressed,
+                                                   int validate, void* stream);
+/* G2 points to their byte forms (CanonicalSerialize of Affine<G2>, macros.rs:67-97).  d_points holds n Affine<G2> images
+ * (200-byte stride, 8-byte aligned); d_bytes receives 96 bytes per point (compressed != 0: canonical x, PositiveY iff y > −y in the
+ * order above; infinity: x = 0 with the Infinity bit) or 192 (uncompressed: canonical x and y, no sign flag; infinity: x = 0, y = 1
+ * with the Infinity bit).  One launch, one thread per point, no synchronisation. */
+SNARKVM_API int snarkvm_b200_g2_serialize_device(void* d_bytes, const void* d_points, size_t n, int compressed, void* stream);
+
 /* One run of Fr records in a proving key's bytes (CanonicalSerialize of Circuit: snark/varuna/ahp/indexer/circuit.rs:158-237).
  * stride 32: `count` canonical Fr at d_blob + offset, 32 bytes apart (an Evaluations vector).  stride 40: matrix entries, each a
  * canonical Fr and a u64 column; with d_row_ptr (int32 [nrows + 1], device) `offset` is the matrix section (its u64 row count) and

@@ -42,7 +42,8 @@ SYMBOLS = (
     "snarkvm_b200_poseidon_transcripts_resume_device", "snarkvm_b200_g1_validate_device",
     "snarkvm_b200_g1_deserialize_device", "snarkvm_b200_g1_serialize_device", "snarkvm_b200_fr_records_decode_device",
     "snarkvm_b200_matrix_row_walk", "snarkvm_b200_varuna_round4_evals_batch_device", "snarkvm_b200_poly_evaluate_batch_device",
-    "snarkvm_b200_poly_divide_by_linear_batch_device",
+    "snarkvm_b200_poly_divide_by_linear_batch_device", "snarkvm_b200_g2_validate_device", "snarkvm_b200_g2_deserialize_device",
+    "snarkvm_b200_g2_serialize_device",
 )
 
 
@@ -218,6 +219,9 @@ def lib():
     L.snarkvm_b200_g1_validate_device.argtypes = [vp, vp, sz, sz, vp]
     L.snarkvm_b200_g1_deserialize_device.argtypes = [vp, vp, vp, sz, i32, i32, vp]
     L.snarkvm_b200_g1_serialize_device.argtypes = [vp, vp, sz, i32, vp]
+    L.snarkvm_b200_g2_validate_device.argtypes = [vp, vp, sz, sz, vp]
+    L.snarkvm_b200_g2_deserialize_device.argtypes = [vp, vp, vp, sz, i32, i32, vp]
+    L.snarkvm_b200_g2_serialize_device.argtypes = [vp, vp, sz, i32, vp]
     L.snarkvm_b200_fr_records_decode_device.argtypes = [vp, sz, ctypes.POINTER(FrRecordsSegment), sz, ctypes.POINTER(u64), vp]
     L.snarkvm_b200_matrix_row_walk.argtypes = [vp, sz, u64, u64, vp, ctypes.POINTER(ctypes.c_int64)]
     L.snarkvm_b200_msm_batch_device.argtypes = [vp, vp, sz, vp, vp, sz, vp]

@@ -93,6 +93,22 @@ FF_DEV void store_affine(uint8_t* base, size_t stride, size_t i, const AffinePoi
     *reinterpret_cast<unsigned long long*>(p + 96) = a.inf ? 1ull : 0ull;
 }
 
+// Affine<G2>: x.c0 x.c1 y.c0 y.c1 (4 × 48 B) inf[1] pad, stride ≥ 200 and a multiple of 8
+FF_DEV AffineT<Fq2> load_affine_g2(const uint8_t* base, size_t stride, size_t i) {
+    const uint8_t* p = base + i * stride;
+    AffineT<Fq2> a;
+    a.x.c0 = load_fq_u64(p); a.x.c1 = load_fq_u64(p + 48);
+    a.y.c0 = load_fq_u64(p + 96); a.y.c1 = load_fq_u64(p + 144);
+    a.inf = __ldg(p + 192) != 0;
+    return a;
+}
+FF_DEV void store_affine_g2(uint8_t* base, size_t stride, size_t i, const AffineT<Fq2>& a) {
+    uint8_t* p = base + i * stride;
+    store_fq_u64(p, a.x.c0); store_fq_u64(p + 48, a.x.c1);
+    store_fq_u64(p + 96, a.y.c0); store_fq_u64(p + 144, a.y.c1);
+    *reinterpret_cast<unsigned long long*>(p + 192) = a.inf ? 1ull : 0ull;
+}
+
 // a < q on the raw limbs: a coordinate image ≥ q is no field element
 FF_DEV bool fq_is_canonical(const Fq& a) {
     (void)ptx_sub_cc(a.v[0], FqParams::mod(0));

@@ -18,21 +18,6 @@ namespace b200 {
 
 static constexpr int X2W = XYZZ2::WORDS;          // 96 words = 384 bytes
 
-FF_DEV AffineT<Fq2> load_affine_g2(const uint8_t* base, size_t stride, size_t i) {
-    const uint8_t* p = base + i * stride;
-    AffineT<Fq2> a;
-    a.x.c0 = load_fq_u64(p); a.x.c1 = load_fq_u64(p + 48);
-    a.y.c0 = load_fq_u64(p + 96); a.y.c1 = load_fq_u64(p + 144);
-    a.inf = __ldg(p + 192) != 0;
-    return a;
-}
-FF_DEV void store_affine_g2(uint8_t* base, size_t stride, size_t i, const AffineT<Fq2>& a) {
-    uint8_t* p = base + i * stride;
-    store_fq_u64(p, a.x.c0); store_fq_u64(p + 48, a.x.c1);
-    store_fq_u64(p + 96, a.y.c0); store_fq_u64(p + 144, a.y.c1);
-    *reinterpret_cast<unsigned long long*>(p + 192) = a.inf ? 1ull : 0ull;
-}
-
 // one thread per work item (≤ cap sorted entries of one bucket)
 __global__ void __launch_bounds__(128) k_g2_accumulate(const uint8_t* __restrict__ points, size_t stride, const uint32_t* __restrict__ sorted,
                                                        const uint32_t* __restrict__ bucket_start, const uint32_t* __restrict__ item_start,

@@ -230,6 +230,54 @@ def g1_serialize(projective: torch.Tensor, compressed=True) -> torch.Tensor:
     return out
 
 
+G2_COMPRESSED_BYTES, G2_UNCOMPRESSED_BYTES = 96, 192
+
+
+def g2_validate(points: torch.Tensor, stride: int = G2_AFFINE_STRIDE) -> torch.Tensor:
+    """Valid for Affine<G2> of every Affine<G2> image in HBM (snarkvm_b200_g2_validate_device) → int32 status per point in HBM,
+    the G1_* values: G1_VALID (infinity included), G1_NOT_CANONICAL (a coordinate image ≥ q), G1_NOT_ON_CURVE or
+    G1_NOT_IN_SUBGROUP ([r]·P ≠ O), the first test failed."""
+    n = _nbytes(points) // stride
+    status = torch.empty(n, dtype=torch.int32, device=points.device)
+    if n:
+        with torch.cuda.device(points.device):
+            _lib.check(_lib.lib().snarkvm_b200_g2_validate_device(status.data_ptr(), _check(points, "points"), n, stride, _stream()))
+    return status
+
+
+def g2_deserialize(bytes_u8: torch.Tensor, compressed: bool = True, validate: bool = True):
+    """G2 points from their byte forms (snarkvm_b200_g2_deserialize_device): `bytes_u8` a uint8 CUDA tensor of n × 96 compressed
+    or n × 192 uncompressed bytes → (Affine<G2> images uint8 [n, 200], int32 status [n]), both in HBM.  Status G1_BAD_FLAGS (both
+    flag bits set, or bit 7 of a coordinate that carries no flags), G1_NOT_CANONICAL (a coordinate ≥ q), G1_NOT_ON_CURVE
+    (compressed: x³ + B' has no square root in Fq2), else G1_VALID or, with `validate`, g2_validate's status.  Bytes that decode to
+    no point leave an all-zero image."""
+    size = G2_COMPRESSED_BYTES if compressed else G2_UNCOMPRESSED_BYTES
+    if bytes_u8.dtype != torch.uint8 or _nbytes(bytes_u8) % size:
+        raise ValueError(f"g2_deserialize takes uint8 bytes, {size} per point")
+    n = _nbytes(bytes_u8) // size
+    images = torch.empty((n, G2_AFFINE_STRIDE), dtype=torch.uint8, device=bytes_u8.device)
+    status = torch.empty(n, dtype=torch.int32, device=bytes_u8.device)
+    if n:
+        with torch.cuda.device(bytes_u8.device):
+            _lib.check(_lib.lib().snarkvm_b200_g2_deserialize_device(images.data_ptr(), status.data_ptr(), _check(bytes_u8, "bytes_u8"),
+                                                                     n, int(bool(compressed)), int(bool(validate)), _stream()))
+    return images, status
+
+
+def g2_serialize(images: torch.Tensor, compressed: bool = True) -> torch.Tensor:
+    """G2 points to their byte forms (snarkvm_b200_g2_serialize_device): `images` a CUDA tensor of n Affine<G2> images (200 bytes
+    each) → uint8 [n, 96] compressed or [n, 192] uncompressed, in HBM"""
+    if _nbytes(images) % G2_AFFINE_STRIDE:
+        raise ValueError(f"g2_serialize takes {G2_AFFINE_STRIDE}-byte Affine<G2> images")
+    n = _nbytes(images) // G2_AFFINE_STRIDE
+    out = torch.empty((n, G2_COMPRESSED_BYTES if compressed else G2_UNCOMPRESSED_BYTES), dtype=torch.uint8, device=images.device)
+    if n:
+        with torch.cuda.device(images.device):
+            _lib.check(_lib.lib().snarkvm_b200_g2_serialize_device(out.data_ptr(), _check(images, "images"), n, int(bool(compressed)),
+                                                                   _stream()))
+    return out
+
+
 FR_RECORD_NOT_CANONICAL, FR_RECORD_BAD_COLUMN = 1, 2
 
 

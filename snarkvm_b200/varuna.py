@@ -620,6 +620,29 @@ G2_GENERATOR = (
     (1843833842842620867708835993770650838640642469700861403869757682057607397502738488921663703124647238454792872005,
      33145532013610981697337930729788870077912093258611421158732879580766461459275194744385880708057348608045241477209),
 )
+# the G1 generator of curves/src/bls12_377/g1.rs, out of Montgomery form
+G1_GENERATOR = (89363714989903307245735717098563574705733591463163614225748337416674727625843187853442697973404985688481508350822,
+                3702177272937190650578065972808860481433820514072818216637796320125658674906330993856598323293086021583822603349)
+
+
+def _generator_bytes(coords, compressed: bool) -> bytes:
+    """the byte form of a generator ((x, y) over Fq, or ((x0, x1), (y0, y1)) over Fq2) without flag bits: y's sign in the
+    compressed form is compared apart"""
+    x, y = coords
+    x, y = (x, y) if isinstance(x, tuple) else ((x,), (y,))
+    return b"".join(v.to_bytes(48, "little") for v in (x if compressed else x + y))
+
+
+def _is_generator(b: bytes, coords, compressed: bool) -> bool:
+    """the bytes of a point decode to the generator: the same coordinates, no Infinity bit and, compressed, the generator's
+    sign (PositiveY iff y > −y; in the uncompressed form the sign bit is ignored, as the reference ignores it)"""
+    y = coords[1]
+    y_pos = (y[1], y[0]) > ((-y[1]) % Q_MOD, (-y[0]) % Q_MOD) if isinstance(y, tuple) else y > (-y) % Q_MOD
+    flags = b[-1] & 0xC0
+    body = b[:-1] + bytes([b[-1] & 0x3F])
+    if flags & 0x40 or body != _generator_bytes(coords, compressed):
+        return False
+    return not compressed or (flags == 0x80) == y_pos
 
 
 def _g2_affine(p) -> np.ndarray:
@@ -690,6 +713,15 @@ def parse_gamma_powers(blob: bytes) -> dict:
     return {i: _parse_g1(p, f"γβ^{i}·G") for i, p in _u64_map(blob, 96, "powers of β·γ·G")}
 
 
+def _validate_g2(named: list, dev) -> None:
+    """Valid for Affine<G2> of every (name, 200-byte Affine<G2> image) in one device.g2_validate launch; ValueError names the
+    first that fails"""
+    status = device.g2_validate(torch.from_numpy(np.stack([img for _n, img in named])).to(dev)).cpu().numpy()
+    bad = np.nonzero(status)[0]
+    if bad.size:
+        raise ValueError(f"{named[int(bad[0])][0]}: {_G1_STATUS[int(status[bad[0]])]}")
+
+
 class UniversalVerifier:
     """The pairing half of the universal verifier (kzg10/data_structures.rs UniversalParams: h, prepared_h, prepared_beta_h,
     gamma_g, prepared_negative_powers_of_beta_h; g is the first power of β·G): g and gamma_g (γ·G, None when unknown) as 104-byte
@@ -710,19 +742,76 @@ class UniversalVerifier:
         self.device = self.prepared.device
 
     @classmethod
-    def from_usrs(cls, blob: bytes, device_="cuda") -> "UniversalVerifier":
+    def from_usrs(cls, blob: bytes, device_="cuda", validate: bool = False) -> "UniversalVerifier":
         """β·H from the mainnet `beta-h.usrs` bytes: x.c0, x.c1, y.c0, y.c1 (48 B LE each), bit 6 of the last byte = infinity and
-        bit 7 = y's sign (utilities/src/serialize/flags.rs).  A coordinate ≥ q raises ValueError."""
-        return cls(_parse_g2(blob, "β·H"), device_)
+        bit 7 = y's sign (utilities/src/serialize/flags.rs).  A coordinate ≥ q raises ValueError.  The reference reads this file
+        unchecked (deserialize_uncompressed_unchecked, parameters/src/mainnet/powers.rs:86-96); with `validate`, β·H must also pass
+        Valid for Affine<G2> (device.g2_validate), or ValueError names it."""
+        beta_h = _parse_g2(blob, "β·H")
+        if validate:
+            _validate_g2([("β·H", beta_h)], torch.device(device_))
+        return cls(beta_h, device_)
 
     @classmethod
-    def from_mainnet(cls, beta_h: bytes, neg_powers: bytes, gamma_powers: bytes, device_="cuda") -> "UniversalVerifier":
+    def from_mainnet(cls, beta_h: bytes, neg_powers: bytes, gamma_powers: bytes, device_="cuda",
+                     validate: bool = False) -> "UniversalVerifier":
         """the mainnet verifier from the bytes of `beta-h.usrs`, `neg-powers-of-beta.usrs` (every degree bound 2^k − 2 with its
-        β^{-(D − d)}·H) and `powers-of-beta-gamma.usrs` (its key 0 is γ·G).  A coordinate ≥ q raises ValueError."""
+        β^{-(D − d)}·H) and `powers-of-beta-gamma.usrs` (its key 0 is γ·G).  A coordinate ≥ q raises ValueError.  With `validate`,
+        β·H and every negative power pass Valid for Affine<G2> in one device.g2_validate launch and γ·G passes Affine::check
+        (device.g1_validate); a failure raises ValueError naming β·H, the degree bound of the negative power, or γ·G."""
         gammas = parse_gamma_powers(gamma_powers)
         if 0 not in gammas:
             raise ValueError("the powers of β·γ·G hold no γ·G")
-        return cls(_parse_g2(beta_h, "β·H"), device_, gammas[0], parse_neg_powers(neg_powers))
+        bh, neg = _parse_g2(beta_h, "β·H"), parse_neg_powers(neg_powers)
+        if validate:
+            dev = torch.device(device_)
+            _validate_g2([("β·H", bh)] + [(f"the negative power for bound {d}", neg[d]) for d in sorted(neg)], dev)
+            status = int(device.g1_validate(torch.from_numpy(gammas[0][None].copy()).to(dev)).cpu()[0])
+            if status != device.G1_VALID:
+                raise ValueError(f"γ·G: {_G1_BYTES_STATUS[status]}")
+        return cls(bh, device_, gammas[0], neg)
+
+    def to_bytes(self, compressed: bool = True) -> bytes:
+        """CanonicalSerialize of kzg10::VerifierKey (kzg10/data_structures.rs:200-214): g, γ·G, h, β·h; 288 bytes compressed (the
+        reference's write_le), 576 uncompressed.  The G1 points go through one device.g1_serialize call and the G2 points through
+        one device.g2_serialize call.  A verifier without γ·G raises ValueError."""
+        if self.gamma_g is None:
+            raise ValueError("this verifier holds no γ·G, which the verifier key's bytes need")
+        g1 = torch.from_numpy(_projective_limbs(np.stack([self.g, self.gamma_g])).view(np.int64)).to(self.device)
+        g2 = torch.from_numpy(np.stack([self.h, self.beta_h])).to(self.device)
+        b1 = device.g1_serialize(g1, compressed).cpu().numpy()
+        b2 = device.g2_serialize(g2, compressed).cpu().numpy()
+        return b1.tobytes() + b2.tobytes()
+
+    @classmethod
+    def from_bytes(cls, blob, compressed: bool = True, validate: bool = True, neg_powers: dict | None = None,
+                   device_="cuda") -> "UniversalVerifier":
+        """the inverse of to_bytes (CanonicalDeserialize of kzg10::VerifierKey, data_structures.rs:217-232; read_le is the
+        compressed form, validated): g and γ·G in one device.g1_deserialize launch, h and β·h in one device.g2_deserialize launch.
+        `neg_powers` ({degree bound: 200-byte Affine<G2> image}, as parse_neg_powers gives) is held as the constructor holds it.
+        A wrong length or trailing bytes, or a g or h other than the G1 or G2 generator (which this verifier assumes, DESIGN §4c),
+        raises ValueError on the host before any device call; a point that fails to decode (or, with `validate`, Valid) raises
+        ValueError naming the field."""
+        blob = bytes(blob)
+        g1_size, g2_size = _g1_size(compressed), device.G2_COMPRESSED_BYTES if compressed else device.G2_UNCOMPRESSED_BYTES
+        want = 2 * g1_size + 2 * g2_size
+        if len(blob) != want:
+            raise ValueError(f"a verifier key is {want} bytes in this form, not {len(blob)}"
+                             + (" (trailing bytes)" if len(blob) > want else ""))
+        if not _is_generator(blob[:g1_size], G1_GENERATOR, compressed):
+            raise ValueError("g: not the G1 generator, which this verifier assumes")
+        if not _is_generator(blob[2 * g1_size: 2 * g1_size + g2_size], G2_GENERATOR, compressed):
+            raise ValueError("h: not the G2 generator, which this verifier assumes")
+        dev = torch.device(device_)
+        raw1 = torch.from_numpy(np.frombuffer(blob[:2 * g1_size], dtype=np.uint8).copy()).to(dev)
+        raw2 = torch.from_numpy(np.frombuffer(blob[2 * g1_size:], dtype=np.uint8).copy()).to(dev)
+        img1, st1 = device.g1_deserialize(raw1, compressed, validate)
+        img2, st2 = device.g2_deserialize(raw2, compressed, validate)
+        img1, st1, img2, st2 = img1.cpu().numpy(), st1.cpu().numpy(), img2.cpu().numpy(), st2.cpu().numpy()
+        for name, s in zip(("g", "gamma_g", "h", "beta_h"), list(st1) + list(st2)):
+            if s != device.G1_VALID:
+                raise ValueError(f"{name}: {_G1_BYTES_STATUS[int(s)]}")
+        return cls(img2[1], device_, img1[1], neg_powers)
 
     @classmethod
     def synthetic(cls, beta: int, device_="cuda", max_degree: int | None = None, gamma: int | None = None,
