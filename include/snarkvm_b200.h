@@ -501,6 +501,12 @@ enum {
 };
 SNARKVM_API int snarkvm_b200_test_tower_op_device(int op, int k, void* d_out, const void* d_a, const void* d_b, const void* d_c, size_t n,
                                                   void* stream);
+/* The square roots of the point decoders (verify.cu), element-wise and compiled there: the same out-of-line fq_sqrt (Tonelli–Shanks)
+ * and fq2_sqrt (by the norm) that k_g1_deserialize and k_g2_deserialize call.  field FQ: d_in and d_out hold n Fq (12 words), field
+ * FQ2: n Fq2 (24 words, c0 then c1); Montgomery images below q, d_in and d_out 16-byte aligned.  d_ok[i] (int32, 4-byte aligned)
+ * is 1 when d_in[i] is a square and d_out[i] then holds the root the decoders would use (either sign), else 0 with d_out[i] zero.
+ * Another field returns cudaErrorInvalidValue.  One launch, one thread per element, no synchronisation. */
+SNARKVM_API int snarkvm_b200_test_sqrt_device(int field, void* d_out, int32_t* d_ok, const void* d_in, size_t n, void* stream);
 
 /* Deterministic synthetic bases P_i = h(seed, i) * G written in the reference affine layout. */
 /* ---- G2 (points over Fq2) ----------------------------------------------------------------------------------------------

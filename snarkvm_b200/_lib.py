@@ -43,7 +43,7 @@ SYMBOLS = (
     "snarkvm_b200_g1_deserialize_device", "snarkvm_b200_g1_serialize_device", "snarkvm_b200_fr_records_decode_device",
     "snarkvm_b200_matrix_row_walk", "snarkvm_b200_varuna_round4_evals_batch_device", "snarkvm_b200_poly_evaluate_batch_device",
     "snarkvm_b200_poly_divide_by_linear_batch_device", "snarkvm_b200_g2_validate_device", "snarkvm_b200_g2_deserialize_device",
-    "snarkvm_b200_g2_serialize_device",
+    "snarkvm_b200_g2_serialize_device", "snarkvm_b200_test_sqrt_device",
 )
 
 
@@ -238,6 +238,7 @@ def lib():
     L.snarkvm_b200_test_curve_op_device.argtypes = [i32, i32, vp, vp, vp, vp, sz, vp]
     L.snarkvm_b200_test_field_op_host.argtypes = [i32, i32, vp, vp, vp, sz]
     L.snarkvm_b200_test_tower_op_device.argtypes = [i32, i32, vp, vp, vp, vp, sz, vp]
+    L.snarkvm_b200_test_sqrt_device.argtypes = [i32, vp, vp, vp, sz, vp]
     L.snarkvm_b200_msm_window_sums_host.argtypes = [vp, vp, sz, vp, sz, vp, sz, vp]
     for s in SYMBOLS[5:]:
         getattr(L, s).restype = i32

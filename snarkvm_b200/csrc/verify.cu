@@ -16,6 +16,7 @@
 //                      point's y is a square root of x³ + B' in Fq2 (by the norm, on Tonelli–Shanks in Fq), signed by PositiveY
 //   k_g2_serialize     one thread per point: Affine<G2> image → the compressed or uncompressed bytes
 //   k_fr_records       one thread per record of every segment: canonical Fr (and column) → Montgomery Fr (and int32 column)
+//   k_test_sqrt        one thread per element: fq_sqrt or fq2_sqrt as the decoders call them, for the tests
 //
 // The G1 subgroup test is the reference's: x² (x = 0x8508c00000000001, the BLS parameter) is 127 bits, so the chain is 126
 // doublings and one mixed addition per set bit of x² in XYZZ coordinates, then one mixed addition of P.  The G2 test is the
@@ -548,6 +549,27 @@ __global__ void __launch_bounds__(256) k_fr_records(const FrRecordSeg* __restric
     if (reason) atomicMin(bad + lo, (e << 2) | reason);
 }
 
+// Element-wise square roots for the tests (snarkvm_b200_test_sqrt_device): the decoders' own out-of-line fq_sqrt / fq2_sqrt, one
+// thread per element; an element without a root gets a zero root
+__global__ void __launch_bounds__(128) k_test_sqrt(uint32_t* __restrict__ out, int32_t* __restrict__ ok, const uint32_t* __restrict__ in,
+                                                   size_t n, int field) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    bool s;
+    if (field == SNARKVM_B200_FIELD_FQ) {
+        Fq r = Fq::zero();
+        s = fq_sqrt(Fq::load(in + 12 * i), &r);
+        (s ? r : Fq::zero()).store(out + 12 * i);
+    } else {
+        Fq2 a, r = Fq2::zero();
+        a.c0 = Fq::load(in + 24 * i); a.c1 = Fq::load(in + 24 * i + 12);
+        s = fq2_sqrt(a, &r);
+        if (!s) r = Fq2::zero();
+        r.c0.store(out + 24 * i); r.c1.store(out + 24 * i + 12);
+    }
+    ok[i] = s ? 1 : 0;
+}
+
 }  // namespace
 }  // namespace b200
 
@@ -620,6 +642,18 @@ extern "C" int snarkvm_b200_g2_serialize_device(void* d_bytes, const void* d_poi
     if (!d_bytes || !d_points || ((uintptr_t)d_points & 7) || n > ((size_t)1 << 31)) return (int)cudaErrorInvalidValue;
     const unsigned blocks = (unsigned)((n + 127) / 128);
     k_g2_serialize<<<blocks, 128, 0, (cudaStream_t)stream>>>((uint8_t*)d_bytes, (const uint8_t*)d_points, n, compressed ? 1 : 0);
+    count_launch();
+    return (int)cudaGetLastError();
+}
+
+extern "C" int snarkvm_b200_test_sqrt_device(int field, void* d_out, int32_t* d_ok, const void* d_in, size_t n, void* stream) {
+    using namespace b200;
+    if (field != SNARKVM_B200_FIELD_FQ && field != SNARKVM_B200_FIELD_FQ2) return (int)cudaErrorInvalidValue;
+    if (n == 0) return 0;
+    if (!d_out || !d_ok || !d_in || ((uintptr_t)d_out & 15) || ((uintptr_t)d_in & 15) || ((uintptr_t)d_ok & 3) || n > ((size_t)1 << 31))
+        return (int)cudaErrorInvalidValue;
+    const unsigned blocks = (unsigned)((n + 127) / 128);
+    k_test_sqrt<<<blocks, 128, 0, (cudaStream_t)stream>>>((uint32_t*)d_out, d_ok, (const uint32_t*)d_in, n, field);
     count_launch();
     return (int)cudaGetLastError();
 }
