@@ -456,7 +456,8 @@ __global__ void __launch_bounds__(CTA_INV_THREADS) k_precompute_tables(const uin
 }
 
 static constexpr int PAIR_THREADS = CTA_INV_THREADS;
-// Resident CTAs per SM that k_pair_level2 is built for (128 registers per thread) and that the host sizes its waves by.
+// Resident CTAs per SM that k_pair_level2 is built for (128 registers per thread) and that the host sizes its waves by when a
+// group's pair levels have the GPU to themselves (half as many while another window group is in flight, msm_core).
 static constexpr int PAIR_MIN_BLOCKS = 4;
 // The pair-level kernels run as k_pair_desc<false> and k_pair_level2<false, PAIR_MIN_BLOCKS>, their only instances.  Their
 // template arguments keep the kernel names that profiles and the MSM path tests identify the pair levels by; the bool
@@ -1211,12 +1212,20 @@ int xyzz_sum_ranks_device(uint32_t* d_out, const uint32_t* d_in, int nranks, int
 // (sonic_pc/mod.rs:186-245): without the gate, a burst of large commitments would each take tens of GB and the
 // losers would fail with cudaErrorMemoryAllocation (⇒ silent CPU fallback on the Rust side); with it they queue.
 // ---------------------------------------------------------------------------
+// The second stream of a pipelined call (msm_core) and the events that order its window groups against the caller's stream.
+// One per lease that asks for it, created once and reused: a lease hands its MsmAux back when its call has enqueued its work,
+// so there are as many as there were concurrent pipelined calls, never one per call.
+struct MsmAux {
+    cudaStream_t stream = nullptr;
+    cudaEvent_t sorted = nullptr, joined = nullptr, handoff[2] = {nullptr, nullptr};
+};
 struct DeviceScratch {
     std::mutex mu;
     std::condition_variable cv;
     cudaMemPool_t pool = nullptr;
     size_t limit = 0, in_use = 0, peak = 0, total = 0;
     bool ready = false;
+    std::vector<MsmAux*> aux_free;
 };
 static DeviceScratch g_scratch[64];
 
@@ -1278,12 +1287,28 @@ static void CUDART_CB scratch_release_cb(void* p) {
     l->ds->cv.notify_all();
     delete l;
 }
-// blocks until `bytes` fit in the device's budget (a request larger than the whole budget runs alone), then allocates
-static int scratch_acquire(void** out, size_t bytes, cudaStream_t stream, DeviceScratch** ds_out) {
+static int aux_create(MsmAux** out) {
+    MsmAux* a = new MsmAux;
+    cudaError_t e = cudaStreamCreateWithFlags(&a->stream, cudaStreamNonBlocking);
+    for (cudaEvent_t* ev : {&a->sorted, &a->joined, &a->handoff[0], &a->handoff[1]})
+        if (e == cudaSuccess) e = cudaEventCreateWithFlags(ev, cudaEventDisableTiming);
+    if (e != cudaSuccess) {
+        for (cudaEvent_t ev : {a->sorted, a->joined, a->handoff[0], a->handoff[1]}) if (ev) cudaEventDestroy(ev);
+        if (a->stream) cudaStreamDestroy(a->stream);
+        delete a;
+        return (int)e;
+    }
+    *out = a;
+    return 0;
+}
+// blocks until `bytes` fit in the device's budget (a request larger than the whole budget runs alone), then allocates; with
+// `aux`, the lease also carries an auxiliary stream and its events
+static int scratch_acquire(void** out, size_t bytes, cudaStream_t stream, DeviceScratch** ds_out, MsmAux** aux = nullptr) {
     int dev = 0;
     cudaError_t e = cudaGetDevice(&dev);
     if (e != cudaSuccess) return (int)e;
     DeviceScratch& ds = g_scratch[dev & 63];
+    MsmAux* a = nullptr;
     {
         std::unique_lock<std::mutex> lock(ds.mu);
         int rc = scratch_init(ds, dev);
@@ -1291,18 +1316,28 @@ static int scratch_acquire(void** out, size_t bytes, cudaStream_t stream, Device
         ds.cv.wait(lock, [&] { return ds.in_use == 0 || ds.in_use + bytes <= ds.limit; });
         ds.in_use += bytes;
         if (ds.in_use > ds.peak) ds.peak = ds.in_use;
+        if (aux && !ds.aux_free.empty()) { a = ds.aux_free.back(); ds.aux_free.pop_back(); }
     }
-    e = cudaMallocFromPoolAsync(out, bytes, ds.pool, stream);
+    e = aux && !a ? (cudaError_t)aux_create(&a) : cudaSuccess;
+    if (e == cudaSuccess) e = cudaMallocFromPoolAsync(out, bytes, ds.pool, stream);
     if (e != cudaSuccess) {
-        { std::lock_guard<std::mutex> lock(ds.mu); ds.in_use -= bytes; }
+        {
+            std::lock_guard<std::mutex> lock(ds.mu);
+            ds.in_use -= bytes;
+            if (a) ds.aux_free.push_back(a);
+        }
         ds.cv.notify_all();
         return (int)e;
     }
     *ds_out = &ds;
+    if (aux) *aux = a;
     return 0;
 }
-// frees in stream order and returns the bytes to the budget when the stream gets there
-static void scratch_release(void* p, size_t bytes, cudaStream_t stream, DeviceScratch* ds) {
+// frees in stream order and returns the bytes to the budget when the stream gets there.  The auxiliary stream goes back to the
+// free list at once: whatever the call left on it is already ordered before the caller's stream reaches the free, and a later
+// call that takes it queues behind that work (its own event waits are captured when it enqueues them).
+static void scratch_release(void* p, size_t bytes, cudaStream_t stream, DeviceScratch* ds, MsmAux* aux = nullptr) {
+    if (aux) { std::lock_guard<std::mutex> lock(ds->mu); ds->aux_free.push_back(aux); }
     cudaFreeAsync(p, stream);
     ScratchLease* l = new ScratchLease{ds, bytes};
     if (cudaLaunchHostFunc(stream, scratch_release_cb, l) != cudaSuccess) scratch_release_cb(l);
@@ -1392,7 +1427,8 @@ static MsmPath msm_path(const MsmPlan& plan, uint32_t total_buckets, size_t max_
     return p;
 }
 
-// One msm_core call: what its phases read, and its scratch as msm_core lays it out
+// One msm_core call: what its phases read, and its scratch as msm_core lays it out.  A pipelined call has one MsmCall per
+// scratch set: the same shared arrays (hist, bucket_start, cursors, sm_slots), its own stream and everything else its own.
 struct MsmCall {
     MsmPlan plan;
     MsmPath path;
@@ -1404,6 +1440,7 @@ struct MsmCall {
     size_t set_cap, hot_max;
     int sm_count;
     cudaStream_t stream;
+    cudaEvent_t handoff;                  // pipelined: recorded on `stream` after a group's record scatter
     uint8_t* cub_tmp;
     size_t cub_bytes;
     uint32_t *hist, *bucket_start, *cursors, *items, *item_start, *items2, *sorted, *cnt_tmp, *partial, *partial2, *hot_dev, *red_a, *red_b;
@@ -1417,6 +1454,7 @@ struct MsmGroup {                         // windows [u0, u0 + un) of the call, 
     size_t items_bound, items_launched;   // from the accumulation: ≥ the item count of any single bucket, of the whole group
     const uint32_t *partial, *start;      // from the folds: the item partials and their per-bucket offsets the tail reads
     int quad_rounds;
+    int pair_ctas;                        // pair levels: resident CTAs per SM their waves are sized for
 };
 
 // the pair levels' dynamic shared memory limit (set once per device), and the current device's SM count
@@ -1535,6 +1573,12 @@ static int msm_pair_accumulate(const MsmCall& mc, MsmGroup& g, const MsmSegment*
             launch_scatter_records(mc, sg, seg_points[i], seg_stride[i], w_lo, w_hi, g.bs);
         }
     }
+    // the next group (other stream) scatters from here on.  Handing over later, once this group's first level is ready, ran
+    // that scatter beside this group's pair levels but slowed both (2^24 points, H100 80GB HBM3, 700 W: 92.2 against 90.1 ms).
+    if (mc.handoff) {
+        const cudaError_t e = cudaEventRecord(mc.handoff, stream);
+        if (e != cudaSuccess) return (int)e;
+    }
     ProfScope acc_scope(PROF_MSM_ACCUMULATE, stream);
     const uint32_t* off_in = g.bs;
     uint32_t* off_bufs[2] = {mc.off_a, mc.off_b};
@@ -1554,8 +1598,10 @@ static int msm_pair_accumulate(const MsmCall& mc, MsmGroup& g, const MsmSegment*
         bound = bound / 2 + tb;
         // Whole waves: 132 SMs × 4 resident CTAs × 128 threads = 67584 lanes run at once on an H100; give every lane
         // the same number T of pairs and launch an integer number of such waves, so no partial last wave
-        // idles most of the machine (a level is one long-running CTA per slot, not many short ones).
-        const size_t wave = (size_t)mc.sm_count * PAIR_MIN_BLOCKS * PAIR_THREADS;
+        // idles most of the machine (a level is one long-running CTA per slot, not many short ones).  While another
+        // group is in flight a wave is 2 CTAs per SM (g.pair_ctas), half the register file, so the other stream's
+        // launches find room beside it.
+        const size_t wave = (size_t)mc.sm_count * g.pair_ctas * PAIR_THREADS;
         size_t waves = (pair_bound + 1024 * wave - 1) / (1024 * wave);
         if (waves == 0) waves = 1;
         size_t T = (pair_bound + waves * wave - 1) / (waves * wave);
@@ -1728,9 +1774,7 @@ int msm_core(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, co
 
     // Everything after the bucket sort runs per GROUP of whole windows (all bucket sets of a window together), so the dense
     // scratch of the pair levels (≈ 212 B per entry with 128-byte level-0 records) stays inside the budget of the device's
-    // cached scratch: on an 80 GB H100, 2^24 points → all windows in one group (49 GB for 14), a 2^26-point shard three
-    // windows at a time.  Fewer groups mean fewer, larger pair-level launches (H100 SXM, 700 W: 116 ms of kernels in one group against 121 ms
-    // in two).  A window holds at most one entry per scalar whatever the number of its sets.
+    // cached scratch.  A window holds at most one entry per scalar whatever the number of its sets.
     size_t budget = 0;
     int rc = scratch_group_budget(&budget);
     if (rc) return rc;
@@ -1738,12 +1782,22 @@ int msm_core(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, co
     if (const char* e = getenv("SNARKVM_B200_MSM_SCRATCH_MB")) { long v = atol(e); if (v >= 1) budget = (size_t)v << 20; }      // tests: force many groups
     const uint32_t nwins = (uint32_t)njobs * wins_per_job;
     uint32_t gu = nwins;                                          // windows per group
+    // per entry: dense_a 48 + prefix 24 + descriptors 4, plus the level-0 records (dense_b reuses them: level 0 is their last
+    // reader), 96 or 128 B (rec_words), with 8 B for the item partials and per-bucket arrays
+    const size_t per_win = set_cap * (size_t)(84 + 4 * rec_words) + 1;
+    // Pipelined: at least two groups, alternating between the caller's stream and an auxiliary one, so that one group's pair
+    // levels run beside the other's (the two streams' CTAs share the SMs, 2 + 2 per SM) and one group's tail beside the other's
+    // levels.  Two groups are in flight, each with its own scratch set and sized for half the budget: on an 80 GB H100, 2^24
+    // points run 7 + 7 windows in about the scratch one 14-window group took (DESIGN §3).  Only while half the budget still
+    // holds two windows: each group re-reads every scalar and point for its scatter, and a 2^26-point shard in 14 one-window
+    // groups was slower than in five serial groups of three (H100 80GB HBM3, 700 W: 452.5 against 409.7 ms).  And only from
+    // 2^22 entries per window: below that a group's levels are a few milliseconds in all (2^20 points: 10.66 → 10.35 ms, within
+    // run-to-run spread), and one group keeps half the launches.
+    const bool pipelined = levels > 0 && !flat && nwins >= 2 && set_cap >= ((size_t)1 << 22) && budget / 2 / per_win >= 2;
     if (levels > 0) {
-        // per entry: dense_a 48 + prefix 24 + descriptors 4, plus the level-0 records (dense_b reuses them: level 0 is their
-        // last reader), 96 or 128 B (rec_words), with 8 B for the item partials and per-bucket arrays
-        size_t per_win = set_cap * (size_t)(84 + 4 * rec_words) + 1;
-        size_t fit = budget / per_win;
+        size_t fit = (pipelined ? budget / 2 : budget) / per_win;
         if (fit < 1) fit = 1;
+        if (pipelined && fit > (nwins + 1) / 2) fit = (nwins + 1) / 2;
         if (fit < gu) {
             const uint32_t ngroups = (uint32_t)((nwins + fit - 1) / fit);          // equal groups (15 windows in 3 groups: 5 + 5 + 5, not 7 + 7 + 1)
             gu = (nwins + ngroups - 1) / ngroups;
@@ -1785,36 +1839,42 @@ int msm_core(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, co
     if (cub::DeviceScan::ExclusiveSum(nullptr, mc.cub_bytes, (uint32_t*)nullptr, (uint32_t*)nullptr, (int)(TB + 1), stream) != cudaSuccess) return (int)cudaErrorUnknown;
     if (mc.cub_bytes < 16) mc.cub_bytes = 16;
 
-    // ---- one scratch block, carved up ----
+    // ---- one scratch block, carved up: the arrays every group shares, then one set of the rest per group in flight ----
+    const int nsets = pipelined ? 2 : 1;
+    MsmCall mcs[2];
     auto layout = [&](Arena& a) {
         mc.hist = a.take<uint32_t>((size_t)TB + 1);
         mc.bucket_start = a.take<uint32_t>((size_t)TB + 1);
         mc.cursors = a.take<uint32_t>((size_t)TB + 1);
-        mc.items = a.take<uint32_t>((size_t)TBg + 1);
-        mc.item_start = a.take<uint32_t>((size_t)TBg + 1);
-        mc.items2 = a.take<uint32_t>((size_t)TBg + 1);
         mc.sorted = levels > 0 ? nullptr : a.take<uint32_t>(max_entries);
-        mc.cnt_tmp = a.take<uint32_t>((size_t)TBg + 1);
-        mc.partial = a.take<uint32_t>(max_items * XYZZ_WORDS);
-        mc.partial2 = a.take<uint32_t>((mc.path.fold != MsmPath::FOLD_SCAN ? max_items : (size_t)TBg + max_items / 32 + 2) * XYZZ_WORDS);      // quad folds keep the item layout
-        mc.hot_dev = a.take<uint32_t>(mc.hot_max + 2);
-        mc.red_a = a.take<uint32_t>((size_t)gw * (2 * chunks_per_set > 2 * ((plan.nbuckets + 7u) / 8u) ? 2 * chunks_per_set : 2 * ((plan.nbuckets + 7u) / 8u)) * XYZZ_WORDS);
-        mc.red_b = a.take<uint32_t>((size_t)gw * (chunks_per_set / tree + 1 > 2 * ((plan.nbuckets + 63u) / 64u) + 2 ? chunks_per_set / tree + 1 : 2 * ((plan.nbuckets + 63u) / 64u) + 2) * XYZZ_WORDS);
-        mc.cub_tmp = a.take<uint8_t>(mc.cub_bytes);
         if (!flat && levels == 0) mc.dense_bases = a.take<uint32_t>(total_bases * (size_t)BASE_WORDS);
-        if (levels > 0) {
-            mc.dense0 = a.take<uint32_t>(entries_g * (size_t)rec_words);
-            mc.off_a = a.take<uint32_t>((size_t)TBg + 1);
-            mc.off_b = a.take<uint32_t>((size_t)TBg + 1);
-            mc.dense_a = a.take<uint32_t>(dense_cap_a * DENSE_WORDS);
-            // level 1 writes its outputs (96-byte points) over the level-0 records: only level 0 reads them, and the next
-            // group's scatter runs after this group's accumulation in stream order
-            if (levels > 1) mc.dense_b = dense_cap_b * DENSE_WORDS <= entries_g * (size_t)rec_words ? mc.dense0 : a.take<uint32_t>(dense_cap_b * DENSE_WORDS);
-            mc.prefix = a.take<uint32_t>(dense_cap_a * 12);
-            mc.desc = a.take<uint2>(dense_cap_a);
-            mc.pair_cnt = a.take<uint32_t>((size_t)TBg + 1);
-            mc.pair_off = a.take<uint32_t>((size_t)TBg + 1);
-            mc.sm_slots = a.take<uint32_t>(256);
+        if (levels > 0) mc.sm_slots = a.take<uint32_t>(256);   // one counter for both streams' CTAs on an SM
+        for (int k = 0; k < nsets; k++) {
+            MsmCall& m = mcs[k];
+            m = mc;
+            m.items = a.take<uint32_t>((size_t)TBg + 1);
+            m.item_start = a.take<uint32_t>((size_t)TBg + 1);
+            m.items2 = a.take<uint32_t>((size_t)TBg + 1);
+            m.cnt_tmp = a.take<uint32_t>((size_t)TBg + 1);
+            m.partial = a.take<uint32_t>(max_items * XYZZ_WORDS);
+            m.partial2 = a.take<uint32_t>((mc.path.fold != MsmPath::FOLD_SCAN ? max_items : (size_t)TBg + max_items / 32 + 2) * XYZZ_WORDS);      // quad folds keep the item layout
+            m.hot_dev = a.take<uint32_t>(mc.hot_max + 2);
+            m.red_a = a.take<uint32_t>((size_t)gw * (2 * chunks_per_set > 2 * ((plan.nbuckets + 7u) / 8u) ? 2 * chunks_per_set : 2 * ((plan.nbuckets + 7u) / 8u)) * XYZZ_WORDS);
+            m.red_b = a.take<uint32_t>((size_t)gw * (chunks_per_set / tree + 1 > 2 * ((plan.nbuckets + 63u) / 64u) + 2 ? chunks_per_set / tree + 1 : 2 * ((plan.nbuckets + 63u) / 64u) + 2) * XYZZ_WORDS);
+            m.cub_tmp = a.take<uint8_t>(mc.cub_bytes);           // CUB temp storage is never shared across streams
+            if (levels > 0) {
+                m.dense0 = a.take<uint32_t>(entries_g * (size_t)rec_words);
+                m.off_a = a.take<uint32_t>((size_t)TBg + 1);
+                m.off_b = a.take<uint32_t>((size_t)TBg + 1);
+                m.dense_a = a.take<uint32_t>(dense_cap_a * DENSE_WORDS);
+                // level 1 writes its outputs (96-byte points) over the level-0 records: only level 0 reads them, and the next
+                // group on this set scatters after this group's accumulation in stream order
+                if (levels > 1) m.dense_b = dense_cap_b * DENSE_WORDS <= entries_g * (size_t)rec_words ? m.dense0 : a.take<uint32_t>(dense_cap_b * DENSE_WORDS);
+                m.prefix = a.take<uint32_t>(dense_cap_a * 12);
+                m.desc = a.take<uint2>(dense_cap_a);
+                m.pair_cnt = a.take<uint32_t>((size_t)TBg + 1);
+                m.pair_off = a.take<uint32_t>((size_t)TBg + 1);
+            }
         }
     };
     Arena ar;
@@ -1822,9 +1882,16 @@ int msm_core(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, co
     const size_t scratch_bytes = ar.off;
     void* block = nullptr;
     DeviceScratch* ds = nullptr;
-    if ((rc = scratch_acquire(&block, scratch_bytes, stream, &ds)) != 0) return rc;
+    MsmAux* aux = nullptr;
+    if ((rc = scratch_acquire(&block, scratch_bytes, stream, &ds, pipelined ? &aux : nullptr)) != 0) return rc;
     ar.base = (uint8_t*)block; ar.off = 0;
     layout(ar);
+    mc = mcs[0];
+    if (pipelined) {
+        mcs[0].handoff = aux->handoff[0];
+        mcs[1].stream = aux->stream;
+        mcs[1].handoff = aux->handoff[1];
+    }
 
     rc = (int)cudaMemsetAsync(mc.hist, 0, (size_t)(TB + 1) * 4, stream);
     if (rc == 0 && mc.sm_slots) rc = (int)cudaMemsetAsync(mc.sm_slots, 0, 256 * 4, stream);
@@ -1839,7 +1906,17 @@ int msm_core(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, co
         ProfScope acc_scope(PROF_MSM_ACCUMULATE, stream);
         rc = msm_densify(bases, nbases, mc.dense_bases, stream);
     }
-    for (uint32_t u0 = 0; rc == 0 && u0 < nwins; u0 += gu) {
+    // Pipelined: group i runs on stream i & 1 with scratch set i & 1, so a set is reused only by the group two later on the
+    // same stream, after this one in stream order.  The auxiliary stream starts after the bucket sort, and every group starts
+    // its record scatter after the previous group's (on the other stream), so the two scatters never compete for HBM.
+    if (rc == 0 && pipelined) {
+        rc = (int)cudaEventRecord(aux->sorted, stream);
+        if (rc == 0) rc = (int)cudaStreamWaitEvent(aux->stream, aux->sorted, 0);
+    }
+    const uint32_t ngroups = (nwins + gu - 1) / gu;
+    for (uint32_t i = 0, u0 = 0; rc == 0 && u0 < nwins; i++, u0 += gu) {
+        const MsmCall& m = mcs[pipelined ? i & 1 : 0];
+        if (i > 0 && pipelined && (rc = (int)cudaStreamWaitEvent(m.stream, mcs[(i - 1) & 1].handoff, 0)) != 0) break;
         MsmGroup g = {};
         g.u0 = u0;
         g.un = nwins - u0 < gu ? nwins - u0 : gu;
@@ -1849,14 +1926,23 @@ int msm_core(uint32_t* d_window_sums, uint32_t* d_flags, const MsmPlan& plan, co
         g.bs = mc.bucket_start + (size_t)g.w0 * plan.nbuckets;
         g.entries = set_cap * (size_t)g.un;
         if (g.entries > max_entries) g.entries = max_entries;
-        if (mc.path.fold == MsmPath::FOLD_HOT1 && (rc = (int)cudaMemsetAsync(mc.hot_dev, 0, 4, stream)) != 0) break;
-        rc = levels == 0 ? msm_gather_accumulate(mc, g) : msm_pair_accumulate(mc, g, segs, nsegs, seg_points.data(), seg_stride.data());
+        // the last group runs alone once the one before it ends: full waves
+        g.pair_ctas = pipelined && i + 1 < ngroups ? PAIR_MIN_BLOCKS / 2 : PAIR_MIN_BLOCKS;
+        if (m.path.fold == MsmPath::FOLD_HOT1 && (rc = (int)cudaMemsetAsync(m.hot_dev, 0, 4, m.stream)) != 0) break;
+        rc = levels == 0 ? msm_gather_accumulate(m, g) : msm_pair_accumulate(m, g, segs, nsegs, seg_points.data(), seg_stride.data());
         if (rc) break;
-        ProfScope red_scope(PROF_MSM_REDUCE, stream);
-        rc = msm_fold(mc, g);
-        if (rc == 0) rc = msm_tail(mc, g, d_window_sums + (size_t)g.w0 * XYZZ_WORDS);
+        ProfScope red_scope(PROF_MSM_REDUCE, m.stream);
+        rc = msm_fold(m, g);
+        if (rc == 0) rc = msm_tail(m, g, d_window_sums + (size_t)g.w0 * XYZZ_WORDS);
     }
-    scratch_release(block, scratch_bytes, stream, ds);
+    // the result (and the free below) is in stream order on the caller's stream, whatever ran on the auxiliary one
+    if (pipelined) {
+        cudaError_t e = cudaEventRecord(aux->joined, aux->stream);
+        if (e == cudaSuccess) e = cudaStreamWaitEvent(stream, aux->joined, 0);
+        if (e != cudaSuccess) cudaStreamSynchronize(aux->stream);          // free nothing the auxiliary stream may still use
+        if (rc == 0) rc = (int)e;
+    }
+    scratch_release(block, scratch_bytes, stream, ds, aux);
     return rc;
 }
 
